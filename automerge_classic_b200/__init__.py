@@ -1,4 +1,4 @@
-"""amgpu — B200-native bulk change-replay engine behind automerge-classic's Backend API.
+"""amgpu — H100-native bulk change-replay engine behind automerge-classic's Backend API.
 
     from automerge_classic_b200 import Backend          # init / applyChanges / getPatch / ... (backend/index.js:1-8)
 

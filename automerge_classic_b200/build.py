@@ -1,6 +1,6 @@
 """Builds the native libraries in-tree (they travel to the GPU box with the repo snapshot).
 
-  libamgpu.so    nvcc, sm_100a only: CUDA kernels + C ABI (csrc/capi.cu and the .cuh it includes) + csrc/hostsha.cc (host compiler)
+  libamgpu.so    nvcc, sm_90a (H100) only: CUDA kernels + C ABI (csrc/capi.cu and the .cuh it includes) + csrc/hostsha.cc (host compiler)
   libamgtrace.so g++: synthetic trace generator (csrc/tracegen.cc)
 """
 import os
@@ -8,7 +8,7 @@ import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC', '-shared']
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC', '-shared']
 
 
 def _stale(target, sources):

@@ -1,8 +1,8 @@
-// amgpu — B200-native bulk change-replay engine: common device/host plumbing.
+// amgpu — H100-native bulk change-replay engine: common device/host plumbing.
 //
 // Every per-item kernel of the engine is a functor with `void operator()(size_t i) const`, launched
 // through foreach<F>() as a grid-stride CUDA kernel (k_foreach<F>; the functor name shows up in ncu).
-// Grids are sized in multiples of the SM count (148 on B200) times resident CTAs per SM.
+// Grids are sized in multiples of the SM count (132 on H100) times resident CTAs per SM.
 //
 // AMG_EMU: a *development and host-logic test aid only*. In this build container there is no GPU, so
 // the same functors can be compiled with g++ (-DAMG_EMU) and run as a serial loop to debug the
@@ -60,7 +60,7 @@ struct Ctx {
   volatile unsigned long long* peekFlag = nullptr; unsigned long long peekSeq = 0; bool peekFlagArmed = false;   // completion flag of the last k_peek_words (pinned)
 #endif
   int device = 0;
-  int numSMs = 148;
+  int numSMs = 132;
   uint64_t launches = 0;   // kernels launched (gpu_launches in bench.py)
 };
 
@@ -77,7 +77,7 @@ struct DevPool {
   struct Slab { char* base; size_t used, size; };
   std::mutex m; std::multimap<Key, void*> parked; std::unordered_map<void*, Block> blocks; size_t parkedBytes = 0;
   std::map<int, Slab> slab;   // per device: the slab new blocks are carved from
-  static const size_t kMaxParked = 32ull << 30;
+  static const size_t kMaxParked = 16ull << 30;   // a fifth of an H100's 80 GB
   static const size_t kSlabBytes = 256ull << 20;   // a fresh document needs ~200 tables: carved from a few slabs instead of ~200 cudaMallocs (0.1 - 1 ms each)
   static DevPool& get() { static DevPool* p = new DevPool(); return *p; }   // never destroyed: must outlive every engine and the runtime's own teardown
   // gives parked blocks that own their allocation back to the driver (blocks carved from a slab stay parked: a slab is never freed)

@@ -1,4 +1,4 @@
-// amgpu primitives: exclusive scan and stable LSD radix sort (key-value), hand-written for sm_100a.
+// amgpu primitives: exclusive scan and stable LSD radix sort (key-value), hand-written for sm_90a.
 //
 // scan_exclusive : one kernel, decoupled look-back over 2048-element tiles (tile status words tagged with an epoch, so
 //                  nothing is cleared between scans; warp 0 inspects 32 predecessor tiles per step). Measured against the

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — ops/sec applied for automerge-classic's Backend.applyChanges path on B200.
+"""bench.py — ops/sec applied for automerge-classic's Backend.applyChanges path on H100.
 
   python bench.py --gpus N --steps K --warmup W            (N>1: launched under torchrun, one rank per GPU)
   python bench.py --impl reference --gpus N --steps K --warmup W
+  python bench.py ... --dump-outputs DIR                   (rank 0 writes the patch of its last timed step as DIR/*.npy)
 
 Workload (BASELINE.json `metric`: "ops/sec applied (1M-op text trace)"; SURVEY.md §8d C3): a makeText
 change plus 10 actors x 100 000 single-op changes (70 % insert / 30 % delete, merge every 100 changes)
@@ -20,8 +21,8 @@ config C5): no data-path collective, weak scaling; the time of a step is the max
   e2e_ptr_array: the same through amg_apply_changes with one pageable buffer per change (pointer array), the shape
           Backend.applyChanges(state, Uint8Array[]) has in the reference
   roofline: the column decode kernel (header parse + column expansion fused) re-run on resident data: algorithmic bytes
-          of SURVEY.md §8d (encoded bytes + 48 B/op + 8 B/pred + 96 B/change) / CUDA-event time against the measured
-          HBM peak; the SHA-256 kernel over the same bytes is ALU-bound and stated next to it (`sha256_kernel`,
+          of SURVEY.md §8d (encoded bytes + 48 B/op + 8 B/pred + 96 B/change) / CUDA-event time against the H100 SXM
+          data sheet's 3.35 TB/s of HBM3 bandwidth; the SHA-256 kernel over the same bytes is ALU-bound and stated next to it (`sha256_kernel`,
           `with_sha256_frac` = both together)
   --workload C3|C4|C2|C2b: the configs of SURVEY.md §8d (C3 = headline); the default run also reports C4 / C2 / C2b
           briefly under config.other_workloads
@@ -57,21 +58,13 @@ CPU_SAMPLE_OPS = 200_000
 CPU_SAMPLE = {'C3': 200_000, 'C4': 30_000, 'C2': 100_000, 'C2b': 100_000}
 
 
-def read_traffic():
-    """DRAM bytes per launch of the decode kernels from the committed ncu capture (None if the file is missing)."""
-    try:
-        with open(os.path.join(ROOT, 'profiles', 'traffic_r02.json')) as fh:
-            return int(json.load(fh)['decode_total_bytes']), 'profiles/traffic_r02.json (ncu --set full of k_decode_tiles, dram__bytes_read.sum + dram__bytes_write.sum, see profiles/README_r02.md)'
-    except Exception:
-        return None, None
+HBM_PEAK_GBS = 3350.0, 'H100 SXM data sheet, 3.35 TB/s (not measured)'
 
 
-def read_peaks():
-    try:
-        with open(os.path.join(ROOT, 'MEASURED_PEAKS.json')) as fh:
-            return float(json.load(fh)['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
-    except Exception:
-        return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+def _die_with_parent():
+    """preexec_fn: the child gets SIGTERM when this process ends, however it ends (the watchdog exits through _exit)."""
+    import signal
+    C.CDLL(None, use_errno=True).prctl(1, signal.SIGTERM)   # PR_SET_PDEATHSIG
 
 
 class ClockSampler:
@@ -83,7 +76,7 @@ class ClockSampler:
         self.samples, self.marks = [], []
         try:
             self.proc = subprocess.Popen(['nvidia-smi', '-i', str(index), '--query-gpu=' + q, '--format=csv,noheader,nounits', '-lms', '50'],
-                                         stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+                                         stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, preexec_fn=_die_with_parent)
             self.thread = threading.Thread(target=self._read, daemon=True)
             self.thread.start()
         except Exception:
@@ -207,7 +200,7 @@ def measure(args, wl_name, rank, world, local, lib, torch, dist, full):
     L.amg_reserve(doc.h, C.c_size_t(nbytes + (1 << 20)), C.byref(err))
     state = {}
 
-    def step(ptr):
+    def step(ptr, keep=False):
         lib.check(L.amg_reset(doc.h, C.byref(err)), err)
         pp = C.c_void_p()
         torch.cuda.synchronize()
@@ -218,14 +211,16 @@ def measure(args, wl_name, rank, world, local, lib, torch, dist, full):
         dt = time.perf_counter() - t0
         lib.check(rc, err)
         n = C.c_size_t()
-        L.amg_patch_bytes(pp, C.byref(n))
+        p = L.amg_patch_bytes(pp, C.byref(n))
+        if keep:   # (after the clock stopped) the flat patch the caller receives
+            state['patch'] = bytes((C.c_uint8 * n.value).from_address(p))
         L.amg_patch_free(pp)
         return dt, doc.timings(), n.value
 
-    def timed(ptr, steps):
+    def timed(ptr, steps, keep_last=False):
         wall, dev, ph, pb = [], [], None, 0
-        for _ in range(steps):
-            dt, ph, pb = step(ptr)
+        for k in range(steps):
+            dt, ph, pb = step(ptr, keep_last and k == steps - 1)
             wall.append(dt)
             dev.append(sum(ph[0:12]) / 1e3)   # CUDA events on the engine's stream, first to last kernel of the call
         return wall, dev, ph, pb
@@ -245,7 +240,7 @@ def measure(args, wl_name, rank, world, local, lib, torch, dist, full):
     if world > 1:
         dist.barrier()
     launches0 = doc.launches()
-    wall, dev_e2e, last_ph, patch_bytes = timed(pinned.data_ptr(), args.steps)
+    wall, dev_e2e, last_ph, patch_bytes = timed(pinned.data_ptr(), args.steps, keep_last=full and bool(args.dump_outputs))
     torch.cuda.synchronize()
     sampler.mark()
     if world > 1:
@@ -258,10 +253,57 @@ def measure(args, wl_name, rank, world, local, lib, torch, dist, full):
         dist.all_reduce(tt, op=dist.ReduceOp.MAX)
         t_wall, t_dev = float(tt[0]), float(tt[1])
     res = {'trace': trace, 'nbytes': nbytes, 'desc': desc, 't_wall': t_wall, 't_dev': t_dev, 'wall_steps': wall, 'dev_steps': dev_res, 'last_ph': last_ph, 'ph_res': ph_res,
-           'patch_bytes': patch_bytes, 'launches': int(launches), 'call_ms': state['call_ms'], 'clocks': sampler.summary(), 'doc': doc, 'pinned': pinned, 'offs': offs, 'offs_pinned': offs_pinned}
+           'patch_bytes': patch_bytes, 'launches': int(launches), 'call_ms': state['call_ms'], 'clocks': sampler.summary(), 'doc': doc, 'pinned': pinned, 'offs': offs, 'offs_pinned': offs_pinned,
+           'patch': state.get('patch')}
     if not full:
         del doc
     return res
+
+
+DUMP_ROWS = 450_000   # rows kept per record table: 2 tables x 8 float64 columns x 450k rows stays under 64 MB
+
+
+def dump_outputs(out_dir, raw):
+    """Writes the flat patch of the last timed step as float64 .npy arrays under out_dir: the header numbers, the clock, the
+    heads, and the prop / edit records decoded to what they mean (op ids are counter << 16 | actor index, exact in
+    float64; a key or value is represented by its byte length and its first 6 bytes, a counter by its summed total). A table
+    of more than DUMP_ROWS records is a fixed, seeded sample of them; `<table>_row` holds the record indices."""
+    import numpy as np
+    from automerge_classic_b200.engine import FlatPatch
+    fp = FlatPatch(raw)
+    u8 = np.frombuffer(raw, dtype=np.uint8)
+
+    def lead(off, n):   # the first (up to) 6 bytes at off, little-endian
+        off, n, v = off.astype(np.int64), np.minimum(n.astype(np.int64), 6), np.zeros(len(off))
+        for k in range(6):
+            m = (n > k) & (off + k < len(u8))
+            v[m] += u8[off[m] + k] * float(256 ** k)
+        return v
+
+    def signed64(lo, hi):
+        return (lo.astype(np.uint64) | (hi.astype(np.uint64) << np.uint64(32))).view(np.int64).astype(np.float64)
+
+    pr, ed = fp.props, fp.edits
+    p_counter = ((pr['flags'] >> 8) == 1) & ((pr['flags'] & 2) != 0)
+    e_counter = ((ed['kind'] >> 16) == 1) & ((ed['kind'] & 0x1000) != 0)
+    tables = {
+        'props': {'obj': pr['obj'], 'op_id': pr['opId'], 'flags': pr['flags'], 'key_len': pr['keyLen'], 'key': lead(pr['keyOff'], pr['keyLen']),
+                  'val_len': pr['valLen'], 'value': np.where(p_counter, signed64(pr['valOff'], pr['pad']), lead(pr['valOff'], pr['valLen'] >> 4))},
+        'edits': {'obj': ed['obj'], 'op_id': ed['opId'], 'elem_id': fp.edit_elem, 'index': ed['index'], 'kind': ed['kind'], 'val_len': ed['valLen'],
+                  'value': np.where(e_counter, signed64(ed['valLen'], ed['valOff']), lead(ed['valOff'], ed['valLen'] >> 4))},
+    }
+    out = {'header': np.array([fp.max_op, fp.pending, len(fp.actors), len(fp.deps), len(pr), len(ed)], dtype=np.float64),
+           'clock': np.array([fp.clock.get(a, 0) for a in fp.actors], dtype=np.float64),
+           'heads': np.frombuffer(b''.join(bytes.fromhex(h) for h in fp.deps), dtype=np.uint8).astype(np.float64)}
+    for name, cols in tables.items():
+        n = len(next(iter(cols.values())))
+        rows = np.arange(n) if n <= DUMP_ROWS else np.sort(np.random.default_rng(20240601).choice(n, DUMP_ROWS, replace=False))
+        out[name + '_row'] = rows.astype(np.float64)
+        for col, v in cols.items():
+            out['%s_%s' % (name, col)] = np.asarray(v)[rows].astype(np.float64)
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + '.npy'), a)
 
 
 def ptr_array_e2e(trace, lib, torch, local, steps):
@@ -319,6 +361,7 @@ def main():
     ap.add_argument('--workload', default='C3', choices=sorted(WORKLOADS))
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-extras', action='store_true', help='headline figures only (no other routes / workloads / pointer-array entry)')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the patch of the last timed step (rank 0) as DIR/<name>.npy')
     args = ap.parse_args()
     rank, world, local = int(os.environ.get('RANK', 0)), int(os.environ.get('WORLD_SIZE', 1)), int(os.environ.get('LOCAL_RANK', 0))
     if args.impl == 'reference':
@@ -349,14 +392,15 @@ def main():
     total_ops = trace.n_ops * world
     blob_ptr, offs = C.c_void_p(m['pinned'].data_ptr()), m['offs']
     extras = rank == 0 and not args.no_extras
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, m.pop('patch'))
 
     # decode roofline: re-run the decode kernels on the resident batch
     roofline = None
     if rank == 0:
         ms_sha, ms_parse, ms_dec, algo = C.c_float(), C.c_float(), C.c_float(), C.c_uint64()
         rc = L.amg_bench_decode(doc.h, 20, C.byref(ms_sha), C.byref(ms_parse), C.byref(ms_dec), C.byref(algo), C.byref(err))
-        peak, peak_src = read_peaks()
-        traffic, traffic_src = read_traffic()
+        peak, peak_src = HBM_PEAK_GBS
         if rc == 0:
             # the HBM-bound part of the decode: header parse + column expansion (one fused kernel). SHA-256 over the same
             # bytes is ALU-bound (64 rounds per 64-byte block) and is reported next to it, not folded into the HBM figure.
@@ -365,7 +409,7 @@ def main():
             ach = algo.value / t_dec / 1e9
             n_blocks = (trace.blob.size + 64 * trace.n_changes) / 64.0          # ~ message blocks incl. padding
             roofline = {'bound': 'hbm', 'kernel': kernel_name,
-                        'achieved': ach, 'peak': peak, 'unit': 'GB/s', 'frac': ach / peak, 'traffic': traffic, 'traffic_source': traffic_src, 'peak_source': peak_src,
+                        'achieved': ach, 'peak': peak, 'unit': 'GB/s', 'frac': ach / peak, 'peak_source': peak_src,
                         'algorithmic_bytes_per_launch': int(algo.value),
                         'ms': {'decode_tiles': ms_parse.value, 'decode_large_changes': ms_dec.value},
                         'sha256_kernel': {'bound': 'alu', 'ms': ms_sha.value, 'bytes_hashed': int(trace.blob.size),
@@ -374,7 +418,7 @@ def main():
                         'with_sha256_gbs': algo.value / ((ms_sha.value + ms_parse.value + ms_dec.value) / 1e3) / 1e9,
                         'with_sha256_frac': algo.value / ((ms_sha.value + ms_parse.value + ms_dec.value) / 1e3) / 1e9 / peak}
         else:
-            roofline = {'bound': 'hbm', 'achieved': None, 'peak': peak, 'unit': 'GB/s', 'frac': None, 'traffic': None, 'error': err.msg.decode()}
+            roofline = {'bound': 'hbm', 'achieved': None, 'peak': peak, 'unit': 'GB/s', 'frac': None, 'error': err.msg.decode()}
 
     # the other routes of SURVEY §8d, once each on rank 0 (wall clock through the C ABI): (ii) loadChanges + getPatch,
     # (iii) save, then load + getPatch of the saved document
@@ -432,7 +476,7 @@ def main():
             'ms_per_step': t_wall * 1e3, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': 'int64', 'data': 'synthetic',
             'config': {'workload': m['desc'],
                        'ops_per_gpu': trace.n_ops, 'changes_per_gpu': trace.n_changes, 'change_bytes_per_gpu': nbytes, 'parallelism': 'replicas x%d' % world, 'numa_node': numa,
-                       'l2': 'inputs (%.0f MB) + working tables exceed the 126 MB L2; document reset every step' % (nbytes / 1e6),
+                       'l2': 'inputs (%.0f MB) + working tables exceed the 50 MB L2; document reset every step' % (nbytes / 1e6),
                        'value_definition': 'change bytes resident in HBM (device pointer handed to amg_apply_changes_packed); CUDA events on the engine stream from the first to the last kernel of the call, patch copied to pinned host memory',
                        'e2e_definition': 'same call with the bytes in pinned HOST memory: wall clock around the synchronous call, H2D upload and patch D2H inside',
                        'device_ms_per_step': t_dev * 1e3, 'wall_ms_steps': [round(x * 1e3, 3) for x in m['wall_steps']], 'call_return_ms_last_step': round(m['call_ms'], 3), 'abi_call_ms_last_step': round(last_ph[23], 3), 'device_ms_steps': [round(x * 1e3, 3) for x in m['dev_steps']],

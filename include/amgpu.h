@@ -1,4 +1,4 @@
-/* amgpu — C ABI of the B200-native bulk change-replay engine for automerge-classic.
+/* amgpu — C ABI of the H100-native bulk change-replay engine for automerge-classic.
  *
  * This is the drop-in boundary: a backend module for `Automerge.setDefaultBackend()`
  * (reference src/automerge.js:147-149; function set in backend/index.js:1-8 and

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box with `-m gpu`): the CUDA engine, called through the C ABI
+"""GPU parity tests (run on an H100 with `-m gpu`): the CUDA engine, called through the C ABI
 (libamgpu.so via automerge_classic_b200.engine), against the CPU oracle on the same inputs.
 
   * every reference test extracted into tests/golden/ is replayed through the Backend facade on the

@@ -3,7 +3,7 @@ with -DAMG_EMU (tests/_emu/build.sh) and executed as serial loops, so the orches
 csrc/engine_impl.cuh and the per-item kernel logic can be checked against the oracle in this
 GPU-less build container. This is a development aid: the emulation library is never loaded by the
 product package, and none of these tests stands in for the `-m gpu` parity tests, which run the
-nvcc-built kernels through libamgpu.so on a B200.
+nvcc-built kernels through libamgpu.so on an H100.
 """
 import os
 import subprocess
