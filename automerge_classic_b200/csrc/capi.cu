@@ -110,14 +110,11 @@ amg_backend* amg_clone(amg_backend* src, amg_error* err) {
     sync(s.ctx); s.ensureHostMirror();
     d.hostArena.assign(s.hostArena); d.arenaLen = s.arenaLen; d.arena.ensure(c, s.arenaLen + 64); d2d(c, d.arena.p, s.arena.p, s.arenaLen);
     d.numApplied = s.numApplied; d.hashes.ensure(c, s.numApplied * 32 + 64); d2d(c, d.hashes.p, s.hashes.p, s.numApplied * 32);
-    d.numRows = s.numRows; d.doc.ensure(c, s.numRows + 1);
-    d2d(c, d.doc.id.p, s.doc.id.p, s.numRows * 8); d2d(c, d.doc.obj.p, s.doc.obj.p, s.numRows * 8); d2d(c, d.doc.key.p, s.doc.key.p, s.numRows * 8);
-    d2d(c, d.doc.keyStrOff.p, s.doc.keyStrOff.p, s.numRows * 4); d2d(c, d.doc.keyStrLen.p, s.doc.keyStrLen.p, s.numRows * 4); d2d(c, d.doc.flags.p, s.doc.flags.p, s.numRows * 4);
-    d2d(c, d.doc.valLen.p, s.doc.valLen.p, s.numRows * 4); d2d(c, d.doc.valOff.p, s.doc.valOff.p, s.numRows * 4); d2d(c, d.doc.time.p, s.doc.time.p, s.numRows * 4);
+    d.numRows = s.numRows; d.doc.copyFrom(c, s.doc, s.numRows);
     d.numSucc = s.numSucc; d.succOff.ensure(c, s.numRows + 2); d2d(c, d.succOff.p, s.succOff.p, (s.numRows + 1) * 4); d.succ.ensure(c, s.numSucc + 1); d2d(c, d.succ.p, s.succ.p, s.numSucc * 8);
-    d.actorIds = s.actorIds; d.actorRep = s.actorRep; d.clock = s.clock; d.heads = s.heads; d.headIdx = s.headIdx; d.changes = s.changes; d.deflatedOriginal = s.deflatedOriginal; d.loadedDoc = s.loadedDoc; d.numLoaded = s.numLoaded; for (int k = 0; k < 9; k++) d.loadedCols[k] = s.loadedCols[k];
-    d.unknownCols = s.unknownCols; d.queue = s.queue; d.queueOriginal = s.queueOriginal; d.maxOp = s.maxOp; d.haveHashGraph = s.haveHashGraph; d.historyRebuilt = s.historyRebuilt;
-    while (d.actorCap < 2 * (d.actorIds.size() + 16)) d.actorCap *= 2;
+    d.st = s.st; d.changes = s.changes; d.deflatedOriginal = s.deflatedOriginal; d.loadedDoc = s.loadedDoc; d.numLoaded = s.numLoaded; for (int k = 0; k < 9; k++) d.loadedCols[k] = s.loadedCols[k];
+    d.unknownCols = s.unknownCols; d.queue = s.queue; d.queueOriginal = s.queueOriginal; d.haveHashGraph = s.haveHashGraph; d.historyRebuilt = s.historyRebuilt;
+    while (d.actorCap < 2 * (d.st.actorIds.size() + 16)) d.actorCap *= 2;
     d.actorSlots.ensure(c, d.actorCap); d.rebuildActorTable();
     sync(c);
     return b;
@@ -131,7 +128,7 @@ int amg_apply_changes(amg_backend* b, const uint8_t* const* bufs, const size_t* 
 }
 int amg_apply_changes_packed(amg_backend* b, const uint8_t* blob, const uint64_t* offsets, size_t n, int is_local, int want_patch, amg_patch** out, amg_error* err) {
   AMG_GUARD(amg::HostClock whole; { PatchOut p; b->eng.applyChanges(nullptr, nullptr, n, blob, (const u64*)offsets, is_local != 0, want_patch != 0, p);
-            if (out) *out = want_patch ? serialize(p) : nullptr; } b->eng.lastPhaseMs[23] = whole.ms(); return 0;)   // [23]: the whole call as the ABI sees it
+            if (out) *out = want_patch ? serialize(p) : nullptr; } b->eng.trace.ms[23] = whole.ms(); return 0;)   // [23]: the whole call as the ABI sees it
 }
 int amg_get_patch(amg_backend* b, amg_patch** out, amg_error* err) {
   AMG_GUARD(PatchOut p; b->eng.getPatch(p); *out = serialize(p); return 0;)
@@ -152,7 +149,7 @@ void amg_buffers_free(amg_buffers* l) { delete l; }
 void amg_free_mem(void* p) { free(p); }
 
 int amg_get_heads(amg_backend* b, amg_buffers** out, amg_error* err) {
-  AMG_GUARD(auto* l = new amg_buffers(); for (auto& h : b->eng.heads) l->items.emplace_back((const char*)h.data(), 32); *out = l; return 0;)
+  AMG_GUARD(auto* l = new amg_buffers(); for (auto& h : b->eng.st.heads) l->items.emplace_back((const char*)h.data(), 32); *out = l; return 0;)
 }
 
 // new.js:2033-2055
@@ -180,7 +177,7 @@ int amg_get_changes(amg_backend* b, const uint8_t* have_deps, size_t n, amg_buff
       if (!all) break;
       auto& ds = g.dependents[h]; stack.insert(stack.end(), ds.begin(), ds.end());
     }
-    bool headsSeen = true; for (auto& h : b->eng.heads) if (!seen.count(h)) headsSeen = false;
+    bool headsSeen = true; for (auto& h : b->eng.st.heads) if (!seen.count(h)) headsSeen = false;
     if (stack.empty() && headsSeen) { for (auto& h : toReturn) l->items.push_back(b->changeBytes(g.indexByHash[h])); *out = guard.release(); return 0; }
     stack.clear(); for (size_t i = 0; i < n; i++) stack.push_back(toHash(have_deps + 32 * i)); seen.clear();
     while (!stack.empty()) {
@@ -197,7 +194,7 @@ int amg_get_changes(amg_backend* b, const uint8_t* have_deps, size_t n, amg_buff
 int amg_get_changes_added(amg_backend* bn, amg_backend* bo, amg_buffers** out, amg_error* err) {
   AMG_GUARD(
     bn->ensureGraph(); bo->ensureGraph(); HostGraph& g = bn->g; auto* l = new amg_buffers();
-    std::vector<Hash> stack = bn->eng.heads, toReturn; std::unordered_map<Hash, bool, HashHasher> seen;
+    std::vector<Hash> stack = bn->eng.st.heads, toReturn; std::unordered_map<Hash, bool, HashHasher> seen;
     while (!stack.empty()) {
       Hash h = stack.back(); stack.pop_back();
       if (!seen.count(h) && !bo->g.indexByHash.count(h)) { seen[h] = true; toReturn.push_back(h); auto& ds = g.deps[g.indexByHash[h]]; stack.insert(stack.end(), ds.begin(), ds.end()); }
@@ -233,16 +230,16 @@ int amg_get_missing_deps(amg_backend* b, const uint8_t* heads, size_t n, amg_buf
 }
 int amg_clock_of(amg_backend* b, const uint8_t* actor, size_t actor_len, uint64_t* seq_out, amg_error* err) {
   AMG_GUARD(std::string a((const char*)actor, actor_len); *seq_out = 0; Engine& e = b->eng;
-            for (size_t i = 0; i < e.actorIds.size(); i++) if (e.actorIds[i] == a) *seq_out = e.clock[i]; return 0;)
+            for (size_t i = 0; i < e.st.actorIds.size(); i++) if (e.st.actorIds[i] == a) *seq_out = e.st.clock[i]; return 0;)
 }
 int amg_hash_by_actor(amg_backend* b, const uint8_t* actor, size_t actor_len, uint64_t index, uint8_t hash_out[32], int* found, amg_error* err) {
   AMG_GUARD(b->ensureGraph(); *found = 0; auto it = b->g.hashesByActor.find(std::string((const char*)actor, actor_len));
             if (it != b->g.hashesByActor.end() && index < it->second.size()) { memcpy(hash_out, it->second[index].data(), 32); *found = 1; } return 0;)
 }
 
-int amg_last_timings(amg_backend* b, float* ms_out, int n) { for (int i = 0; i < n && i < 24; i++) ms_out[i] = b->eng.lastPhaseMs[i]; return 0; }
+int amg_last_timings(amg_backend* b, float* ms_out, int n) { for (int i = 0; i < n && i < 24; i++) ms_out[i] = b->eng.trace.ms[i]; return 0; }
 size_t amg_debug_marks(amg_backend* b, char* buf, size_t cap) {
-  std::string s; for (auto& m : b->eng.dbgMarks) { char t[96]; snprintf(t, sizeof t, "%s=%.3f ", m.first, m.second); s += t; }
+  std::string s; for (auto& m : b->eng.trace.marks) { char t[96]; snprintf(t, sizeof t, "%s=%.3f ", m.first, m.second); s += t; }
   if (cap) { snprintf(buf, cap, "%s", s.c_str()); } return s.size();
 }
 uint64_t amg_kernel_launches(amg_backend* b) { return b->eng.ctx.launches; }

@@ -52,7 +52,6 @@ struct Ctx {
   cudaEvent_t evFork = nullptr, evJoin = nullptr;
   cudaStream_t copy = nullptr;        // third stream: device -> host copy of the uploaded change bytes into the host mirror
   cudaEvent_t evUp = nullptr, evMirror = nullptr; bool copyPending = false; std::vector<cudaEvent_t> pieceEv; size_t pieceNext = 0;
-  cudaEvent_t phaseEv[13]; bool phaseEvReady = false;   // phase timing of the last call (PhaseTimer)
   // small device -> host reads go through a kernel that stores into pinned (device-visible) host memory, not through the
   // copy engine: a read of 4 bytes must not queue behind a 100 MB transfer (see d2h / sync)
   struct Peek { void* dst; size_t off, bytes; };
@@ -262,6 +261,7 @@ template <class T> struct DBuf {
     dev_free(p); p = np_; cap = ncap;
   }
   T* get() { return p; }
+  void swap(DBuf& o) { std::swap(p, o.p); std::swap(cap, o.cap); }
 };
 
 // Pinned host staging buffer

@@ -11,12 +11,15 @@
 #pragma once
 #include <algorithm>
 #include <array>
-#include <functional>
 #include <initializer_list>
 #include <map>
 #include <memory>
 #include <thread>
+#include <chrono>
 #include <zlib.h>
+#ifndef AMG_EMU
+#include <nvtx3/nvToolsExt.h>
+#endif
 #include "patch.cuh"
 #include "inflate.cuh"
 #include "encode.cuh"
@@ -30,17 +33,60 @@ namespace amg {
 
 struct DocBufs {
   DBuf<u64> id, obj, key; DBuf<u32> keyStrOff, keyStrLen, flags, valLen, valOff, time;
-  void ensure(Ctx& c, size_t n, size_t keep = 0) {
-    id.ensure(c, n, keep); obj.ensure(c, n, keep); key.ensure(c, n, keep); keyStrOff.ensure(c, n, keep); keyStrLen.ensure(c, n, keep);
-    flags.ensure(c, n, keep); valLen.ensure(c, n, keep); valOff.ensure(c, n, keep); time.ensure(c, n, keep);
-  }
+  template <class F> void each(DocBufs& o, F f) { f(id, o.id); f(obj, o.obj); f(key, o.key); f(keyStrOff, o.keyStrOff); f(keyStrLen, o.keyStrLen); f(flags, o.flags); f(valLen, o.valLen); f(valOff, o.valOff); f(time, o.time); }
+  void ensure(Ctx& c, size_t n, size_t keep = 0) { each(*this, [&](auto& x, auto&) { x.ensure(c, n, keep); }); }
   DocRows view() { return DocRows{id.p, obj.p, key.p, keyStrOff.p, keyStrLen.p, flags.p, valLen.p, valOff.p, time.p}; }
-  void swap(DocBufs& o) {
-    std::swap(id.p, o.id.p); std::swap(id.cap, o.id.cap); std::swap(obj.p, o.obj.p); std::swap(obj.cap, o.obj.cap); std::swap(key.p, o.key.p); std::swap(key.cap, o.key.cap);
-    std::swap(keyStrOff.p, o.keyStrOff.p); std::swap(keyStrOff.cap, o.keyStrOff.cap); std::swap(keyStrLen.p, o.keyStrLen.p); std::swap(keyStrLen.cap, o.keyStrLen.cap);
-    std::swap(flags.p, o.flags.p); std::swap(flags.cap, o.flags.cap); std::swap(valLen.p, o.valLen.p); std::swap(valLen.cap, o.valLen.cap);
-    std::swap(valOff.p, o.valOff.p); std::swap(valOff.cap, o.valOff.cap); std::swap(time.p, o.time.p); std::swap(time.cap, o.time.cap);
+  void swap(DocBufs& o) { each(o, [](auto& x, auto& y) { x.swap(y); }); }
+  void copyFrom(Ctx& c, DocBufs& o, size_t n) { ensure(c, n + 1); each(o, [&](auto& x, auto& y) { d2d(c, x.p, y.p, n * sizeof(*x.p)); }); }   // rows [0, n) of `o`
+};
+
+// Host state of the document. An applyChanges call works on a copy and commits it by assignment; load, reset and clone set it whole.
+struct DocState {
+  std::vector<std::string> actorIds;           // raw bytes, index = document actor number
+  std::vector<std::pair<u32, u32>> actorRep;   // arena (offset, length) of each actor's id bytes
+  std::vector<u64> clock;                      // per actor number
+  u64 maxOp = 0;
+  std::vector<std::array<u8, 32>> heads; std::vector<u32> headIdx;   // heads (sorted by hash) and their application indices
+};
+
+struct HostClock {
+  std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
+  float ms() const { return std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count(); }
+};
+
+// Timing of the last applyChanges call, and the development trace. phase(name) ends the running pipeline phase and
+// starts the next one (nullptr: ends the last): a CUDA event on the main stream, a host clock mark and an NVTX range
+// (nsys timelines; SURVEY.md section 5). mark(label) records a labelled host mark (amg_debug_marks). Both do nothing
+// outside a call. With AMG_TRACE set (read when a call starts), the marks are printed to stderr as they happen (to see
+// where a call is stuck), and load, save and the history reconstruction print theirs too, after a sync.
+struct Trace {
+  float ms[24] = {0};   // [0..11] CUDA-event phases, [12..23] host clock marks (ms since the call started), [23] the whole ABI call
+  std::vector<std::pair<const char*, float>> marks; bool live = false;
+  static bool enabled() { return getenv("AMG_TRACE") != nullptr; }
+  explicit Trace(Ctx& c) : ctx(c) {}
+  void begin(const char* first) { nEv = 0; record(); clk = HostClock(); for (auto& x : ms) x = 0; marks.clear(); nHost = 12; active = true; live = enabled(); nvtx(first); }
+  void phase(const char* next) { if (!active) return; record(); if (nHost < 24) ms[nHost++] = clk.ms(); nvtx(next); }
+  void mark(const char* label) {
+    if (!active) return;
+    marks.emplace_back(label, clk.ms());
+    if (live) { fprintf(stderr, "amgpu mark %-28s %9.3f ms\n", label, clk.ms()); fflush(stderr); }
   }
+  void end() { nvtx(nullptr); active = false; }
+  // load / save / history reconstruction: host marks since `t0`, printed only with AMG_TRACE (after a sync, so they include the device work)
+  void print(const char* what, const char* label, const HostClock& t0) { if (enabled()) { sync(ctx); fprintf(stderr, "amgpu %s: %-28s %9.2f ms\n", what, label, t0.ms()); } }
+#ifndef AMG_EMU
+  ~Trace() { if (evReady) for (auto& e : ev) cudaEventDestroy(e); }
+  void collect() { cudaEventSynchronize(ev[nEv - 1]); for (int i = 0; i + 1 < nEv && i < 12; i++) cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]); }   // device intervals into ms[0..11]
+ private:
+  cudaEvent_t ev[13]; bool evReady = false, nvtxOpen = false;   // the events are created once: 13 new timing events per call cost more than a phase
+  void record() { if (!evReady) { for (auto& e : ev) cudaEventCreate(&e); evReady = true; } if (nEv < 13) cudaEventRecord(ev[nEv++], ctx.stream); }
+  void nvtx(const char* name) { if (nvtxOpen) nvtxRangePop(); nvtxOpen = name != nullptr; if (name) nvtxRangePushA(name); }
+#else
+  void collect() {}
+ private:
+  void record() {} void nvtx(const char*) {}
+#endif
+  Ctx& ctx; HostClock clk; bool active = false; int nEv = 0, nHost = 12;
 };
 
 struct PatchOut {   // flat patch, written straight into the engine's pinned output buffer (layout: include/amgpu.h)
@@ -63,6 +109,19 @@ struct HostArena {
   void assign(const HostArena& o) { resize(o.len); if (o.len) memcpy(buf.p, o.buf.p, o.len); }
 };
 
+inline std::string inflateRawBytes(const u8* p, size_t n) {
+  z_stream zs; memset(&zs, 0, sizeof(zs));
+  if (inflateInit2(&zs, -15) != Z_OK) throw Error(AMG_ERR_INTERNAL, "inflateInit failed");
+  std::string out; out.resize(std::max<size_t>(n * 6, 1024)); zs.next_in = (Bytef*)p; zs.avail_in = (uInt)n; size_t produced = 0;
+  while (true) {
+    zs.next_out = (Bytef*)out.data() + produced; zs.avail_out = (uInt)(out.size() - produced);
+    int rc = inflate(&zs, Z_NO_FLUSH); produced = out.size() - zs.avail_out;
+    if (rc == Z_STREAM_END) break;
+    if (rc != Z_OK && rc != Z_BUF_ERROR) { inflateEnd(&zs); throw Error(AMG_ERR_RANGE, "invalid deflate data"); }
+    if (zs.avail_out == 0) out.resize(out.size() * 2); else if (zs.avail_in == 0) { inflateEnd(&zs); throw Error(AMG_ERR_RANGE, "unexpected end of deflate data"); }
+  }
+  inflateEnd(&zs); out.resize(produced); return out;
+}
 inline std::string hex_of(const u8* p, size_t n) { static const char* d = "0123456789abcdef"; std::string s; for (size_t i = 0; i < n; i++) { s.push_back(d[p[i] >> 4]); s.push_back(d[p[i] & 15]); } return s; }
 
 class Engine {
@@ -75,12 +134,8 @@ class Engine {
   DBuf<ActorSlot> actorSlots; size_t actorCap = 0;
   DBuf<u32> actorRank;
   // ---- persistent host state
-  std::vector<std::string> actorIds;   // raw bytes, index = document actor number
-  std::vector<u64> clock;              // per actor number
-  std::vector<std::array<u8, 32>> heads; std::vector<u32> headIdx;   // heads (sorted by hash) and their application indices
-  std::vector<std::pair<u32, u32>> actorRep;   // arena (offset, length) of each actor's id bytes
+  DocState st;
   std::vector<HostChange> changes;     // applied, in application order
-  std::vector<std::array<u8, 32>> changeHashes;   // host copy of applied hashes (filled lazily)
   struct OrigRange { u32 idx; HostChange range; };
   std::vector<OrigRange> deflatedOriginal;        // (applied change index, arena range of the original DEFLATEd bytes), ascending index
   const HostChange* originalOf(u32 idx) const {
@@ -88,10 +143,7 @@ class Engine {
     return it != deflatedOriginal.end() && it->idx == idx ? &it->range : nullptr;
   }
   std::vector<HostChange> queue, queueOriginal;   // not yet causally ready (+ original range, len 0 = not deflated)
-  u64 maxOp = 0;
-  float lastPhaseMs[24] = {0};   // [0..11] CUDA-event phases, [12..23] host wall-clock markers (ms since call start)
-  struct PhaseTimer* curTimer = nullptr; std::function<void()> curHostMark;
-  std::vector<std::pair<const char*, float>> dbgMarks; std::function<void(const char*)> dbgMark = [](const char*) {};
+  Trace trace{ctx};
   HBuf<u8> patchBuf;   // pinned: patch records are copied device -> host directly into their final place
   // ---- scratch (grow-only)
   DBuf<u32> chOff, chLen, nOps, nPreds, nDeps, nActors, colOff, colLen, depBase, depIdx, primary, pass, flagWord, appRank, opBase, predBase, timeBase, amapBase, amap, authorSlot, newSlots;
@@ -112,8 +164,8 @@ class Engine {
   DBuf<u32> isObjHead, objIdx, objStart, elemVis, elemVisScan, rowEmit, firstVis, state, nItems, itemBase, qIndex, zero, wzero, zscan, wscan, editObjKey;
   DBuf<DomItem> items, items2; DBuf<PropRec> propOut; DBuf<EditRec> editOut, editOut2; DBuf<u64> editElem, editElem2;
   std::unique_ptr<ColumnEncoder> encoder; DBuf<long long> saveVals; DBuf<u32> saveStrOff, saveStrLen; std::string loadedDoc; size_t numLoaded = 0; HostChange loadedCols[9] = {}; DBuf<u64> counterTotal; DBuf<int> domW, domW2; DBuf<u32> elemMinT, editRowPos, editRowPos2, editObjKey2, rowClass, firstBare, counterOwner, newSuccTime, counterLast, runHeadFlag, runScan, runStart, elemFollower, domTw, domTw2, oldVisScan, inflLen, inflOff, groupHasChild, gCount, gElem, gT1, gQOrd, gBase, nQ, elemHasRecs, listLinkTime, editElemPos, editElemPos2, editKind, editPred, editDead, editMerge, editMulti, editLive;
-  DBuf<u32> seqSlot, actorCnt, actorBaseD, clockD, changeActor, editTime; DBuf<u8> hashTmp; DBuf<u32> headsPack, headsOut; bool batchInOrder = true;
-  DBuf<u32> finalTime, gFailed, memberFinal, opAt, runHead, opGroupHead; DBuf<u64> gBound; DocRows workView{}; DBuf<HostChange> chPairs; DBuf<u32> largeFlag, largeSlot, largeList; size_t lastNumLarge = 0; DBuf<u64> zwScan; DBuf<u32> deflList, patchTriples;
+  DBuf<u32> seqSlot, actorCnt, actorBaseD, clockD, changeActor, editTime; DBuf<u8> hashTmp; DBuf<u32> headsPack, headsOut;
+  DBuf<u32> finalTime, gFailed, memberFinal, opAt, runHead, opGroupHead; DBuf<u64> gBound; DBuf<HostChange> chPairs; DBuf<u32> largeFlag, largeSlot, largeList; size_t lastNumLarge = 0; DBuf<u64> zwScan; DBuf<u32> deflList, patchTriples;
 
   explicit Engine(int device) {
     ctx.device = device;
@@ -132,7 +184,7 @@ class Engine {
     ShaConsts k; memcpy(k.k, SHA_K, sizeof(SHA_K)); CUDA_CHECK(cudaMemcpyToSymbol(c_sha, &k, sizeof(k)));
 #endif
     errWord.ensure(ctx, 4); flagWord.ensure(ctx, 16);
-    actorCap = 64; actorSlots.ensure(ctx, actorCap); resetActorSlots(0, actorCap);
+    actorCap = 64; actorSlots.ensure(ctx, actorCap); rebuildActorTable();
     succOff.ensure(ctx, 1); dev_memset(ctx, succOff.p, 0, 4);
   }
   ~Engine() {
@@ -142,7 +194,6 @@ class Engine {
     if (ctx.side) cudaStreamDestroy(ctx.side);
     if (ctx.copy) cudaStreamDestroy(ctx.copy);
     if (ctx.peekBuf) cudaFreeHost(ctx.peekBuf);
-    if (ctx.phaseEvReady) for (auto& e : ctx.phaseEv) cudaEventDestroy(e);
     if (last_peek_ctx() == &ctx) last_peek_ctx() = nullptr;
     if (ctx.evUp) cudaEventDestroy(ctx.evUp);
     if (ctx.evMirror) cudaEventDestroy(ctx.evMirror);
@@ -154,16 +205,12 @@ class Engine {
   // (re)builds the device actor table from the host's actor list (after growth, rollback or commit)
   void rebuildActorTable() {
     std::vector<ActorSlot> t(actorCap); for (auto& s : t) { s.hash = 0; s.first = ~0ULL; s.actorNum = EMPTY32; s.repOff = 0; s.repLen = 0; s.pad = 0; }
-    for (size_t a = 0; a < actorIds.size(); a++) {
-      const u64 h = fnv1a64((const u8*)actorIds[a].data(), (u32)actorIds[a].size()); u64 s = mix64(h) & (actorCap - 1);
+    for (size_t a = 0; a < st.actorIds.size(); a++) {
+      const u64 h = fnv1a64((const u8*)st.actorIds[a].data(), (u32)st.actorIds[a].size()); u64 s = mix64(h) & (actorCap - 1);
       while (t[s].hash != 0) s = (s + 1) & (actorCap - 1);
-      t[s].hash = h; t[s].first = 0; t[s].actorNum = (u32)a; t[s].repOff = actorRep[a].first; t[s].repLen = actorRep[a].second;
+      t[s].hash = h; t[s].first = 0; t[s].actorNum = (u32)a; t[s].repOff = st.actorRep[a].first; t[s].repLen = st.actorRep[a].second;
     }
     h2d(ctx, actorSlots.p, t.data(), actorCap * sizeof(ActorSlot)); sync(ctx);
-  }
-  void resetActorSlots(size_t from, size_t to) {
-    std::vector<ActorSlot> init(to - from); for (auto& s : init) { s.hash = 0; s.first = ~0ULL; s.actorNum = EMPTY32; s.repOff = 0; s.repLen = 0; s.pad = 0; }
-    h2d(ctx, actorSlots.p + from, init.data(), init.size() * sizeof(ActorSlot)); sync(ctx);
   }
 
   // ---------------------------------------------------------------- error plumbing
@@ -187,12 +234,12 @@ class Engine {
     errSnapshot = w[k]; errSnapLaunches = launchesNow;
   }
   u64 fetchErr() { if (errSnapLaunches != ctx.launches) { void* none[1] = {nullptr}; readWords({}, none); } return errSnapshot; }
-  std::string opIdText(u64 id) const {
+  static std::string opIdText(u64 id, const std::vector<std::string>& actors) {
     const u32 a = id_actor(id);
-    return std::to_string(id_ctr(id)) + "@" + (a < actorIds.size() ? hex_of((const u8*)actorIds[a].data(), actorIds[a].size()) : std::string("?"));
+    return std::to_string(id_ctr(id)) + "@" + (a < actors.size() ? hex_of((const u8*)actors[a].data(), actors[a].size()) : std::string("?"));
   }
-  [[noreturn]] void throwKernelError(u64 w, const std::vector<std::string>& actorsNow, const u64* predIdHost = nullptr) {
-    const u32 code = (u32)(w & 0xff); const u64 item = w >> 8; (void)item; (void)actorsNow; (void)predIdHost;
+  [[noreturn]] static void throwKernelError(u64 w) {
+    const u32 code = (u32)(w & 0xff);
     switch (code) {
       case KE_MAGIC: throw Error(AMG_ERR_RANGE, "Data does not begin with magic bytes 85 6f 4a 83");
       case KE_CHECKSUM: throw Error(AMG_ERR_RANGE, "checksum does not match data");
@@ -230,7 +277,7 @@ class Engine {
       default: throw Error(AMG_ERR_INTERNAL, "amgpu: kernel error " + std::to_string(code));
     }
   }
-  void checkErr(const std::vector<std::string>& actorsNow) { u64 w = fetchErr(); if (w) throwKernelError(w, actorsNow); }
+  void checkErr() { u64 w = fetchErr(); if (w) throwKernelError(w); }
 
   // ---------------------------------------------------------------- helpers
   DBuf<u64> gateBest;   // causal gate with several copies of a waiting change: best (pass, position) per hash
@@ -244,39 +291,53 @@ class Engine {
   // sort `perm` (row ids) by successive 64-bit fields produced by keyFn(field) ; stable LSD over fields
   void sortPairs(DBuf<u64>& keys, DBuf<u32>& vals, size_t n, int bits) { radix_sort_pairs(ctx, sortTmp, keys, vals, n, 0, bits); }
 
-  // reference columnar.js:813-823 (pako.inflateRaw -> zlib raw inflate); magic + checksum are kept. `zs` may be a reusable,
-  // already initialised stream (inflateInit2(.., -15)); it is reset, not re-allocated.
-  static std::string inflateChange(const u8* buf, size_t len, z_stream* reuse = nullptr) {
+  // reference columnar.js:813-823 (pako.inflateRaw -> zlib raw inflate); magic + checksum are kept
+  static std::string inflateChange(const u8* buf, size_t len) {
     ByteReader r(buf, 9, (u32)len); const u64 clen = r.uleb();
     if (r.err || r.pos + clen > len) throw Error(AMG_ERR_RANGE, "buffer ended with incomplete number");
-    z_stream local; z_stream* zs = reuse;
-    if (!zs) { memset(&local, 0, sizeof(local)); if (inflateInit2(&local, -15) != Z_OK) throw Error(AMG_ERR_INTERNAL, "inflateInit failed"); zs = &local; }
-    else inflateReset(zs);
-    struct End { z_stream* z; bool own; ~End() { if (own) inflateEnd(z); } } end{zs, !reuse};
-    std::string out; out.resize(std::max<size_t>(clen * 4, 512));
-    zs->next_in = (Bytef*)(buf + r.pos); zs->avail_in = (uInt)clen; size_t produced = 0;
-    while (true) {
-      zs->next_out = (Bytef*)out.data() + produced; zs->avail_out = (uInt)(out.size() - produced);
-      int rc = inflate(zs, Z_NO_FLUSH); produced = out.size() - zs->avail_out;
-      if (rc == Z_STREAM_END) break;
-      if (rc != Z_OK && rc != Z_BUF_ERROR) throw Error(AMG_ERR_RANGE, "invalid deflate data");
-      if (zs->avail_out == 0) out.resize(out.size() * 2); else if (zs->avail_in == 0) throw Error(AMG_ERR_RANGE, "unexpected end of deflate data");
-    }
+    const std::string body = inflateRawBytes(buf + r.pos, clen);
     // header: magic + checksum (8 bytes), chunk type 1, LEB128 length, then the inflated body
-    u8 hdr[24]; memcpy(hdr, buf, 8); hdr[8] = 1; size_t hl = 9; u64 v = produced; do { u8 b = v & 0x7f; v >>= 7; if (v) b |= 0x80; hdr[hl++] = b; } while (v);
-    std::string res; res.reserve(hl + produced); res.append((const char*)hdr, hl); res.append(out.data(), produced);
-    return res;
+    u8 hdr[24]; memcpy(hdr, buf, 8); hdr[8] = 1; size_t hl = 9; u64 v = body.size(); do { u8 b = v & 0x7f; v >>= 7; if (v) b |= 0x80; hdr[hl++] = b; } while (v);
+    return std::string((const char*)hdr, hl) + body;
   }
 
   // ---------------------------------------------------------------- applyChanges
-  struct ApplyResult { PatchOut patch; };
-
-  void applyChanges(const u8* const* bufs, const size_t* lens, size_t n, const u8* blob, const u64* offsets, bool isLocal, bool wantPatch, PatchOut& out, bool hostScan = false);
-  void applyChangesOnce(const u8* const* bufs, const size_t* lens, size_t n, const u8* blob, const u64* offsets, bool isLocal, bool wantPatch, PatchOut& out, bool hostScan = false);
+  // What one call's phases hand to each other (engine_impl.cuh). Device scratch stays in the engine: grow-only, reused.
+  struct ApplyCall {
+    const u8* const* bufs; const size_t* lens; size_t n; const u8* blob; const u64* offsets; bool isLocal, wantPatch;   // pointer array or packed blob
+    enum { SRC_PINNED, SRC_DEVICE, SRC_PAGEABLE } srcKind = SRC_PAGEABLE; bool offsetsByDma = false, copiesFirst = false;
+    size_t total = 0, arenaLen0 = 0, cur = 0, Bq = 0, B = 0;   // batch: n new changes, then Bq queued ones; bytes arena[arenaLen0, cur)
+    struct Piece { size_t byteEnd, changeEnd, mark; }; std::vector<Piece> pieces;
+    HostChange* pairs = nullptr; u8* hashOut = nullptr; DecodeTilesArgs dargs{};   // pairs: pinned (offset, length) table of the batch
+    // DEFLATEd changes: originals of queue entries (batchOriginal, dense) and of the ones inflated now (inflOrig, parallel to deflIdx)
+    std::vector<HostChange> batchOriginal, inflOrig; std::vector<u32> deflIdx; size_t inflNd = 0, inflExtraStart = 0, inflExtra = 0; bool inflPending = false;
+    void finishInflate(Engine& e); HostChange originalOf(size_t b) const;
+    u32 decTot[4] = {0, 0, 0, 0};   // decode totals: ops, preds, overflow, flags (1: large changes, 2: unknown columns)
+    size_t G = 0, numNew = 0; bool inOrder = true;   // gate: G = applied before + batch
+    std::vector<u8> appliedH; std::vector<u32> primaryH, appRankH; std::vector<HostChange> newQueue, newQueueOriginal;   // host copies: only when an entry waits or the order differs
+    DocState now;   // the document's host state as this call leaves it
+    size_t M = 0, P = 0, N = 0, numPairs = 0; OpRows ops{}; IdTable idt{nullptr, nullptr, 0}; Ord ord{}; DocRows w{};   // w: rows before the sort
+    std::vector<std::pair<u64, UnknownRow>> unknownRows; std::set<u32> unknownIds;
+    std::thread fill;   // fills the host's list of the batch entries; needBatch() joins it before the list is first read
+    void needBatch() { if (fill.joinable()) fill.join(); }
+    ~ApplyCall() { needBatch(); }
+  };
+  void applyChanges(const u8* const* bufs, const size_t* lens, size_t n, const u8* blob, const u64* offsets, bool isLocal, bool wantPatch, PatchOut& out);
+  void applyChangesOnce(ApplyCall& a, PatchOut& out);   // the phases, in order:
+  void stageBatch(ApplyCall& a), inflateBatch(ApplyCall& a), runGate(ApplyCall& a), internActors(ApplyCall& a), checkSequence(ApplyCall& a), finalizeOps(ApplyCall& a),
+       orderOpSet(ApplyCall& a), computeHeads(ApplyCall& a), commit(ApplyCall& a);
+  void queueCopy(ApplyCall& a, ApplyCall::Piece& pc, size_t byte0, size_t ch0); void fillPairs(ApplyCall& a);
+  // error messages of the rare paths
+  [[noreturn]] void throwActorError(u64 ew, const std::vector<std::string>& actors); [[noreturn]] void throwSequenceError(ApplyCall& a);
+  [[noreturn]] void throwOpError(u64 ew, const std::vector<std::string>& actors); [[noreturn]] void throwPatchValueError(u64 ew, size_t numProps);
   void getPatch(PatchOut& out);
   void saveDocument(std::string& result);
-  void buildPatch(DocRows d, size_t N, bool wholeDoc, const OpRows* ops, size_t numOps, const IdTable* idt, const u32* rowOfOpD, const u32* posD,
-                  const std::vector<std::string>& actorsNow, PatchOut& out, const u32* succOffD, const u64* succD);
+  struct PatchInputs {   // everything buildPatch reads: the rows in document order, their succ CSR and counts; incremental: the batch and the op-set tables
+    DocRows d; size_t N; bool wholeDoc; const u32* succOff; const u64* succ; const u32* succCnt; Ord ord;
+    const OpRows* ops = nullptr; size_t numOps = 0; const IdTable* idt = nullptr; const u32 *rowOfOp = nullptr, *pos = nullptr;
+    const u32 *newSuccCnt = nullptr, *firstNewSucc = nullptr, *newSuccTime = nullptr, *objPos = nullptr, *pass = nullptr; DocRows unsorted{};   // rows before the sort
+  };
+  void buildPatch(const PatchInputs& in, PatchOut& out);
   void fillPatchHeader(PatchOut& out);
   void finishPatch(PatchOut& out);
   void reset();
@@ -290,7 +351,8 @@ class Engine {
   void collectUnknownColumns(size_t B, std::vector<std::pair<u64, UnknownRow>>& out, std::set<u32>& ids);
   void appendUnknownDocColumns(std::vector<std::pair<u32, std::string>>& cols);   // save(): their document columns
   RawRows rawRows();
-  u32 decodeHugeChanges(const RawRows& raw, size_t numLarge); DBuf<u32> hugeDone;
+  const HostChange& loadedCol(u32 id) const { static const u32 IDS[9] = {0x01, 0x03, 0x13, 0x23, 0x35, 0x40, 0x43, 0x56, 0x57}; for (int k = 0; k < 9; k++) if (IDS[k] == id) return loadedCols[k]; return loadedCols[0]; }   // a loaded document's change column
+  void decodeHugeChanges(const RawRows& raw, size_t numLarge); DBuf<u32> hugeDone;
   void runDecodeTiles(const u8* arenaP, size_t B, size_t batchBytes, const u32* deflListP = nullptr, size_t numDefl = 0, size_t deflStart = 0);
   DecodeTilesArgs decodeArgs(const u8* arenaP, size_t B, size_t batchBytes);
   // Host mirror of the arena, filled on demand: hostArena holds arena[0, hostArena.size()); whatever is missing is fetched

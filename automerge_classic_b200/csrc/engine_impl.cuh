@@ -1,9 +1,5 @@
 // amgpu — Engine::applyChanges / getPatch pipeline (see engine.cuh for the state layout).
 #pragma once
-#include <chrono>
-#ifndef AMG_EMU
-#include <nvtx3/nvToolsExt.h>
-#endif
 #include "engine.cuh"
 #include "misc.cuh"
 
@@ -15,32 +11,6 @@ namespace amg {
 #define CUDA_CHECK_EMU(x) CUDA_CHECK(x)
 #endif
 static const size_t PATCH_HDR_WORDS = 20;
-// NVTX range per pipeline phase: next() closes the running range and opens the named one (nullptr: just closes)
-struct NvtxPhases {
-#ifndef AMG_EMU
-  bool open = false;
-  void next(const char* name) { if (open) nvtxRangePop(); open = name != nullptr; if (name) nvtxRangePushA(name); }
-  ~NvtxPhases() { if (open) nvtxRangePop(); }
-#else
-  void next(const char*) {}
-#endif
-};
-struct HostClock {
-  std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
-  float ms() const { return std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count(); }
-};
-struct PhaseTimer {
-#ifndef AMG_EMU
-  cudaEvent_t* ev; int n = 0; Ctx* c;   // the events live in the context: creating and destroying 13 timing events per call cost more than a pipeline phase
-  explicit PhaseTimer(Ctx& ctx) : ev(ctx.phaseEv), c(&ctx) { if (!ctx.phaseEvReady) { for (int i = 0; i < 13; i++) cudaEventCreate(&ev[i]); ctx.phaseEvReady = true; } mark(); }
-  void mark() { if (n < 13) cudaEventRecord(ev[n++], c->stream); }
-  void collect(float* out, int maxN) { cudaEventSynchronize(ev[n - 1]); for (int i = 0; i + 1 < n && i < maxN; i++) cudaEventElapsedTime(&out[i], ev[i], ev[i + 1]); }
-#else
-  explicit PhaseTimer(Ctx&) {}
-  void mark() {}
-  void collect(float*, int) {}
-#endif
-};
 
 inline void parallel_copy(u8* dst, const u8* src, size_t n) {
   if (n < (4u << 20)) { memcpy(dst, src, n); return; }
@@ -72,9 +42,9 @@ inline void parallel_gather(u8* dst, const u8* const* bufs, const size_t* lens, 
 }
 
 inline void Engine::fillPatchHeader(PatchOut& out) {
-  out.maxOp = maxOp; out.pendingChanges = queue.size();
-  out.clock.clear(); for (size_t a = 0; a < clock.size(); a++) if (clock[a] > 0) out.clock.emplace_back((u32)a, clock[a]);
-  out.deps = heads; out.actors = actorIds;
+  out.maxOp = st.maxOp; out.pendingChanges = queue.size();
+  out.clock.clear(); for (size_t a = 0; a < st.clock.size(); a++) if (st.clock[a] > 0) out.clock.emplace_back((u32)a, st.clock[a]);
+  out.deps = st.heads; out.actors = st.actorIds;
 }
 
 // writes the header and the small sections (actor, actors, clock, deps) after the big record sections
@@ -100,96 +70,88 @@ inline void Engine::finishPatch(PatchOut& out) {
 inline void Engine::reset() {
   sync(ctx); headIndexesUnknown = false; unknownCols.clear();
   arenaLen = 0; hostArena.len = 0; numApplied = 0; numRows = 0; numSucc = 0; dev_memset(ctx, succOff.p, 0, 4);
-  actorIds.clear(); actorRep.clear(); clock.clear(); heads.clear(); headIdx.clear(); changes.clear(); changeHashes.clear(); deflatedOriginal.clear(); loadedDoc.clear(); numLoaded = 0; historyRebuilt = 0; haveHashGraph = true;
-  queue.clear(); queueOriginal.clear(); maxOp = 0; rebuildActorTable();
+  st = DocState(); changes.clear(); deflatedOriginal.clear(); loadedDoc.clear(); numLoaded = 0; historyRebuilt = 0; haveHashGraph = true;
+  queue.clear(); queueOriginal.clear(); rebuildActorTable();
 }
 
 // After Backend.load the hashes of the loaded changes are unknown until computeHashGraph has run. Like the reference
 // (new.js:1833-1840) the first attempt goes without them; if a change then stays unapplied (or looks out of sequence)
 // because it refers to history, the hash graph is computed and the call starts over. Nothing was committed by then.
 struct NeedHistory {};
-inline void Engine::applyChanges(const u8* const* bufs, const size_t* lens, size_t n, const u8* blob, const u64* offsets, bool isLocal, bool wantPatch, PatchOut& out, bool hostScan) {
-  if (haveHashGraph) { applyChangesOnce(bufs, lens, n, blob, offsets, isLocal, wantPatch, out, hostScan); return; }
-  bool retry = false;
-  try { applyChangesOnce(bufs, lens, n, blob, offsets, isLocal, wantPatch, out, hostScan); }
-  catch (NeedHistory&) { retry = true; }
-  catch (Error& e) { if (e.code != AMG_ERR_RANGE) throw; retry = true; }
-  if (!retry) return;
+inline void Engine::applyChanges(const u8* const* bufs, const size_t* lens, size_t n, const u8* blob, const u64* offsets, bool isLocal, bool wantPatch, PatchOut& out) {
+  auto once = [&]() { ApplyCall a{bufs, lens, n, blob, offsets, isLocal, wantPatch}; applyChangesOnce(a, out); };
+  try { once(); return; }
+  catch (NeedHistory&) {}
+  catch (Error& e) { if (haveHashGraph || e.code != AMG_ERR_RANGE) throw; }
   drop_peeks(ctx);
   computeHashGraph();
   out = PatchOut();
-  applyChangesOnce(bufs, lens, n, blob, offsets, isLocal, wantPatch, out, hostScan);
+  once();
 }
-inline void Engine::applyChangesOnce(const u8* const* bufs, const size_t* lens, size_t n, const u8* blob, const u64* offsets, bool isLocal, bool wantPatch, PatchOut& out, bool hostScan) {
-  PhaseTimer timer(ctx); HostClock hclk; int hmark = 12;
-  NvtxPhases nvtx; nvtx.next("upload+hash+decode");   // NVTX ranges per pipeline phase (nsys / ncu timelines; SURVEY.md section 5)
-  for (auto& x : lastPhaseMs) x = 0;
-  auto hostMark = [&]() { if (hmark < 24) lastPhaseMs[hmark++] = hclk.ms(); };
-  curTimer = &timer; curHostMark = hostMark;
-  static const bool liveMarks = getenv("AMG_DEBUG_LIVE") != nullptr;   // development aid: marks go to stderr as they happen (to see where a call is stuck)
-  dbgMarks.clear(); dbgMark = [this, &hclk](const char* l) { dbgMarks.emplace_back(l, hclk.ms()); if (liveMarks) { fprintf(stderr, "amgpu mark %-28s %9.3f ms\n", l, hclk.ms()); fflush(stderr); } };
-  struct SideJoinAll { Ctx& c; ~SideJoinAll() { side_join(c); } } sideJoinAll{ctx};   // whatever this call put on the side stream is ordered before the next call
-  struct ClearTimer { Engine* e; ~ClearTimer() { e->curTimer = nullptr; e->curHostMark = nullptr; e->dbgMark = [](const char*) {}; } } clearTimer{this};
-  // ------------------------------------------------------------ 0. stage the batch in the arena; hash and decode it piece by piece
-  // The change bytes go to the device in pieces on the copy stream; as soon as a piece has landed, its changes are hashed
-  // (side stream) and decoded (main stream) while the next piece is still crossing PCIe - both kernels read the piece
-  // while it is hot in L2. The host keeps NO copy of bytes that came from a pinned or device buffer of the caller: the
-  // mirror (hostArena) is filled lazily when something asks for it (getChanges, amg_arena ...; ensureHostMirror). Bytes
-  // that have to be staged through pinned memory anyway (pageable caller buffers, pointer arrays) are staged through the
-  // mirror itself, which then stays complete for free.
-  const size_t arenaLen0 = arenaLen; const size_t hostLen0 = hostArena.size();
-  std::vector<HostChange>& batch = batchStore; batch.clear();   // member: the 8 MB of a 1M-change batch keep their pages across calls
-  std::vector<HostChange> batchOriginal, inflOrig;   // originals of DEFLATEd changes: batchOriginal (dense, queue entries) / inflOrig (sparse, parallel to deflIdx)
-  std::vector<u32> deflIdx;
-  size_t inflNd = 0, inflExtraStart = 0, inflExtra = 0; bool inflPending = false;
-  // Host side of the device inflate: which batch entries moved where. Not on the critical path: runs when the information
-  // is first needed (queue hand-over, commit).
-  auto finishInflate = [&]() {
-    if (!inflPending) return;
-    inflPending = false; const size_t nd = inflNd;
-    u32* origOff = patchTriples.p; u32* origLen = patchTriples.p + nd;
-    pinnedScratch.ensure(5 * nd + 16); u32* ps = pinnedScratch.p;   // pinned: the five small copies queue up and complete with one sync
-    d2h(ctx, ps, deflList.p, nd * 4); d2h(ctx, ps + nd, inflLen.p, nd * 4); d2h(ctx, ps + 2 * nd, inflOff.p, nd * 4);
-    d2h(ctx, ps + 3 * nd, origOff, nd * 4); d2h(ctx, ps + 4 * nd, origLen, nd * 4);
-    if (hostArena.size() == inflExtraStart) {   // the mirror is complete up to here: keep it complete
-      hostArena.resize(inflExtraStart + inflExtra);
-      d2h(ctx, hostArena.data() + inflExtraStart, arena.p + inflExtraStart, inflExtra);
+
+// One attempt at a batch: the pipeline phases of DESIGN.md section 3, in order. The kernels write scratch only; nothing
+// persistent changes before commit(), and the guards restore the host side when a phase throws.
+inline void Engine::applyChangesOnce(ApplyCall& a, PatchOut& out) {
+  trace.begin("upload+hash+decode");
+  struct EndTrace { Trace& t; ~EndTrace() { t.end(); } } endTrace{trace};
+  a.arenaLen0 = a.cur = arenaLen; a.Bq = queue.size(); a.B = a.n + a.Bq;
+  if (a.blob && a.n > 0) a.total = a.offsets[a.n] - a.offsets[0]; else for (size_t i = 0; i < a.n; i++) a.total += a.lens[i];
+  if ((u64)a.arenaLen0 + a.total + 64 >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: change arena limited to 4 GiB per document");
+  struct Rollback { Engine* e; size_t len; bool armed = true; ~Rollback() { if (armed) { if (e->hostArena.size() > len) e->hostArena.resize(len); e->rebuildActorTable(); } } } rb{this, hostArena.size()};
+  struct CopyJoin { Ctx& c; ~CopyJoin() { copy_join(c); } } copyJoin{ctx};   // nothing of this call is left on the copy stream, also on the error paths
+  struct SideJoin { Ctx& c; ~SideJoin() { side_join(c); } } sideJoin{ctx};   // whatever this call put on the side stream is ordered before the next call
+  if (a.B == 0) { rb.armed = false; fillPatchHeader(out); finishPatch(out); return; }
+  stageBatch(a);   trace.phase("inflate+decode-finish");
+  inflateBatch(a); trace.phase("gate");
+  runGate(a);      trace.phase("actors+seq+finalize");
+  if (a.numNew > 0) {
+    internActors(a); checkSequence(a); finalizeOps(a); trace.phase("opset");
+    orderOpSet(a);                                      trace.phase("patch");
+    if (a.wantPatch) {   // incremental patch
+      objPos.ensure(ctx, a.N + 1);
+      foreach(ctx, a.N, ObjPosKernel{perm.p, objRow.p, pos.p, objPos.p});
+      buildPatch(PatchInputs{sorted.view(), a.N, false, newSuccOff.p, newSucc.p, succCnt.p, a.ord, &a.ops, a.M, &a.idt, rowOfOp.p, pos.p,
+                             newSuccCnt.p, firstNewSucc.p, newSuccTime.p, objPos.p, pass.p, a.w}, out);
     }
-    sync(ctx);
-    deflIdx.assign(ps, ps + nd); inflOrig.resize(nd);   // deflIdx is ascending: (batch index, original range), looked up by binary search
-    for (size_t k = 0; k < nd; k++) { const u32 bi = ps[k]; inflOrig[k] = HostChange{ps[3 * nd + k], ps[4 * nd + k]}; batch[bi] = HostChange{(u32)inflExtraStart + ps[2 * nd + k], ps[nd + k]}; }
-  };
-  auto originalOf = [&](size_t b) -> HostChange {
-    if (!batchOriginal.empty() && batchOriginal[b].len) return batchOriginal[b];
-    auto it = std::lower_bound(deflIdx.begin(), deflIdx.end(), (u32)b);
-    return it != deflIdx.end() && *it == (u32)b ? inflOrig[it - deflIdx.begin()] : HostChange{0, 0};
-  };
-  struct Rollback { Engine* e; size_t len; bool armed = true; ~Rollback() { if (armed) { if (e->hostArena.size() > len) e->hostArena.resize(len); e->rebuildActorTable(); } } };
-  size_t total = 0;
-  if (blob && n > 0) total = offsets[n] - offsets[0]; else for (size_t i = 0; i < n; i++) total += lens[i];
-  if ((u64)arenaLen0 + total + 64 >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: change arena limited to 4 GiB per document");
-  Rollback rb{this, hostLen0};
-  struct CopyJoin { Engine* e; ~CopyJoin() { copy_join(e->ctx); } } copyJoin{this};   // nothing of this call is left on the copy stream, also on the error paths
-  size_t cur = arenaLen0;
-  const size_t Bq = queue.size(); const size_t B = n + Bq;
-  if (B == 0) { rb.armed = false; fillPatchHeader(out); finishPatch(out); return; }
-  enum { SRC_PINNED, SRC_DEVICE, SRC_PAGEABLE } srcKind = SRC_PAGEABLE;
+    checkErr();                                         trace.phase("heads+commit");
+    computeHeads(a);
+  }
+  commit(a); rb.armed = false;
+  side_join(ctx); sync(ctx); trace.phase(nullptr);
+  fillPatchHeader(out);
+  if (a.isLocal && a.n == 1) {   // new.js:1874-1877
+    std::vector<ChangeHot> m0(1); d2h(ctx, m0.data(), hot.p, sizeof(ChangeHot)); sync(ctx);
+    out.hasActorSeq = true; out.actor.assign(m0[0].actorLen, '\0'); out.seq = m0[0].seq;
+    if (m0[0].actorLen) { d2h(ctx, &out.actor[0], arena.p + m0[0].actorOff, m0[0].actorLen); sync(ctx); }
+  }
+  trace.mark("commit:end");
+  lastB = a.B; lastM = a.M; lastP = a.P; lastBytes = a.cur - a.arenaLen0;
+  finishPatch(out); trace.mark("call:patch-finished");
+  trace.collect(); trace.mark("call:timers-collected");
+}
+
+// ------------------------------------------------------------ 1. stage the batch in the arena; hash and decode it piece by piece
+// The change bytes go to the device in pieces on the copy stream; as soon as a piece has landed, its changes are hashed
+// (side stream) and decoded (main stream) while the next piece is still crossing PCIe - both kernels read the piece
+// while it is hot in L2. The host keeps NO copy of bytes that came from a pinned or device buffer of the caller: the
+// mirror (hostArena) is filled lazily when something asks for it (getChanges, amg_arena ...; ensureHostMirror). Bytes
+// that have to be staged through pinned memory anyway (pageable caller buffers, pointer arrays) are staged through the
+// mirror itself, which then stays complete for free.
+inline void Engine::stageBatch(ApplyCall& a) {
+  const size_t n = a.n, B = a.B, Bq = a.Bq, arenaLen0 = a.arenaLen0, total = a.total; const u64* offsets = a.offsets;
 #ifndef AMG_EMU
-  if (blob && n > 0) { cudaPointerAttributes at; if (cudaPointerGetAttributes(&at, blob) == cudaSuccess) { if (at.type == cudaMemoryTypeHost) srcKind = SRC_PINNED; else if (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) srcKind = SRC_DEVICE; } else cudaGetLastError(); }
+  if (a.blob && n > 0) { cudaPointerAttributes at; if (cudaPointerGetAttributes(&at, a.blob) == cudaSuccess) { if (at.type == cudaMemoryTypeHost) a.srcKind = a.SRC_PINNED; else if (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) a.srcKind = a.SRC_DEVICE; } else cudaGetLastError(); }
 #endif
-  const bool throughMirror = srcKind == SRC_PAGEABLE && total > 0;
-  if (throughMirror) { ensureHostMirror(); hostArena.resize(arenaLen0 + total); }
+  if (a.srcKind == a.SRC_PAGEABLE && total > 0) { ensureHostMirror(); hostArena.resize(arenaLen0 + total); }
   arena.ensure(ctx, arenaLen0 + total + 64, arenaLen0);
-  dbgMark("stage:begin");
-  batch.clear();
+  trace.mark("stage:begin");
+  batchStore.clear();   // member: the 8 MB of a 1M-change batch keep their pages across calls
   // Pieces end on change boundaries. The copies of a pinned / device buffer are queued first (they need nothing but byte
   // ranges); the (offset, length) table of the changes is built and uploaded while they run; then every piece's kernels
   // are queued behind its copy. Pageable input is staged piece by piece, each piece's kernels right behind it.
   const size_t kPiece = 16u << 20;
-  struct Piece { size_t byteEnd, changeEnd, mark; };
-  std::vector<Piece> pieces;
-  pairStage.ensure(B + 1); HostChange* pairs = pairStage.p;   // pinned: the table goes up by DMA while the host carries on
-  if (blob && n > 0) {
+  pairStage.ensure(B + 1); HostChange* pairs = a.pairs = pairStage.p;   // pinned: the table goes up by DMA while the host carries on
+  if (a.blob && n > 0) {
     const size_t base = offsets[0];
     // cut points: every kPiece bytes, the tail halved three more times - what is left to hash and decode once the last byte
     // has arrived is a piece of a few MB, not a whole one
@@ -200,165 +162,185 @@ inline void Engine::applyChangesOnce(const u8* const* bufs, const size_t* lens, 
     for (size_t c : cuts) {
       const size_t ce = (size_t)(std::upper_bound(offsets, offsets + n + 1, (u64)(base + c)) - offsets) - 1;   // changes that end inside the first c bytes
       if (ce <= lastCe || ce >= n) continue;
-      pieces.push_back({(size_t)(offsets[ce] - base), ce, 0}); lastCe = ce;
+      a.pieces.push_back({(size_t)(offsets[ce] - base), ce, 0}); lastCe = ce;
     }
-    pieces.push_back({total, n, 0});
+    a.pieces.push_back({total, n, 0});
   } else {
     size_t at = 0, nextCut = kPiece;
     for (size_t i = 0; i < n; i++) {
-      pairs[i] = HostChange{(u32)(arenaLen0 + at), (u32)lens[i]}; at += lens[i];
-      if (at >= nextCut && i + 1 < n) { pieces.push_back({at, i + 1, 0}); nextCut = at + kPiece; }
+      pairs[i] = HostChange{(u32)(arenaLen0 + at), (u32)a.lens[i]}; at += a.lens[i];
+      if (at >= nextCut && i + 1 < n) { a.pieces.push_back({at, i + 1, 0}); nextCut = at + kPiece; }
     }
-    pieces.push_back({at, n, 0});
+    a.pieces.push_back({at, n, 0});
   }
-  cur = arenaLen0 + total;
+  a.cur = arenaLen0 + total;
   copy_fork(ctx);   // the copy stream starts behind what is queued on the main stream so far (arena growth)
-  const bool copiesFirst = srcKind != SRC_PAGEABLE;
-  auto queueCopy = [&](Piece& pc, size_t byte0, size_t ch0) {
-    const size_t m = pc.byteEnd - byte0;
-    if (m > 0) {
-      u8* dst = arena.p + arenaLen0 + byte0;
-      if (srcKind == SRC_PINNED) h2d_copy(ctx, dst, blob + offsets[0] + byte0, m);
-      else if (srcKind == SRC_DEVICE) d2d_copy(ctx, dst, blob + offsets[0] + byte0, m);
-      else {
-        u8* stage = hostArena.data() + arenaLen0 + byte0;
-        if (blob) parallel_copy(stage, blob + offsets[0] + byte0, m);
-        else parallel_gather(stage, bufs, lens, ch0, pc.changeEnd);
-        h2d_copy(ctx, dst, stage, m);
-      }
-    }
-    pc.mark = copy_piece_record(ctx);
-  };
-  if (copiesFirst) { size_t byte0 = 0, ch0 = 0; for (Piece& pc : pieces) { queueCopy(pc, byte0, ch0); byte0 = pc.byteEnd; ch0 = pc.changeEnd; } }
-  dbgMark("stage:copies-queued");
+  a.copiesFirst = a.srcKind != a.SRC_PAGEABLE;
+  if (a.copiesFirst) { size_t byte0 = 0, ch0 = 0; for (auto& pc : a.pieces) { queueCopy(a, pc, byte0, ch0); byte0 = pc.byteEnd; ch0 = pc.changeEnd; } }
+  trace.mark("stage:copies-queued");
   // The (offset, length) table of the changes. Packed batch whose offsets array is pinned or device memory: the array goes
   // up by DMA and a kernel derives the table (the host's own copy is filled later, in the shadow of the device work).
-  // Otherwise the host fills a pinned table (a few threads for 1M entries) and uploads that.
-  auto fillPairs = [&]() {
-    if (!(blob && n > 0)) return;
-    const size_t base = offsets[0]; const u32 shift = (u32)(arenaLen0 - base);
-    auto fill = [&](size_t a, size_t b) { for (size_t i = a; i < b; i++) { pairs[i].off = (u32)offsets[i] + shift; pairs[i].len = (u32)(offsets[i + 1] - offsets[i]); } };
-    const unsigned nt = n < (1u << 16) ? 1u : std::min<unsigned>(4, std::max(1u, std::thread::hardware_concurrency()));
-    if (nt == 1) fill(0, n);
-    else { std::vector<std::thread> ts; const size_t per = (n + nt - 1) / nt; for (unsigned t = 0; t < nt; t++) { const size_t a = t * per, b = std::min(n, a + per); if (a < b) ts.emplace_back(fill, a, b); } for (auto& t : ts) t.join(); }
-  };
-  bool offsetsByDma = false;
+  // Otherwise the host fills a pinned table and uploads that.
 #ifndef AMG_EMU
-  if (blob && n >= 4096) { cudaPointerAttributes at; if (cudaPointerGetAttributes(&at, offsets) == cudaSuccess) offsetsByDma = at.type == cudaMemoryTypeHost || at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged; else cudaGetLastError(); }
+  if (a.blob && n >= 4096) { cudaPointerAttributes at; if (cudaPointerGetAttributes(&at, offsets) == cudaSuccess) a.offsetsByDma = at.type == cudaMemoryTypeHost || at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged; else cudaGetLastError(); }
 #endif
   for (size_t i = 0; i < Bq; i++) pairs[n + i] = queue[i];
   chPairs.ensure(ctx, B); chOff.ensure(ctx, B); chLen.ensure(ctx, B);
-  if (offsetsByDma) {
+  if (a.offsetsByDma) {
     DBuf<u64>& offsD = offsDev; offsD.ensure(ctx, n + 2);
     CUDA_CHECK_EMU(cudaMemcpyAsync(offsD.p, offsets, (n + 1) * 8, cudaMemcpyDefault, ctx.stream));
     foreach(ctx, n, OffsetsToRangesKernel{offsD.p, (u32)(arenaLen0 - offsets[0]), chOff.p, chLen.p});
     if (Bq > 0) { h2d(ctx, chPairs.p + n, pairs + n, Bq * sizeof(HostChange)); foreach(ctx, Bq, SplitPairsKernel{chPairs.p + n, chOff.p + n, chLen.p + n}); }
   } else {
-    fillPairs();
+    fillPairs(a);
     h2d(ctx, chPairs.p, pairs, B * sizeof(HostChange));
     foreach(ctx, B, SplitPairsKernel{chPairs.p, chOff.p, chLen.p});
   }
-  dev_memset(ctx, arena.p + cur, 0, 64);
+  dev_memset(ctx, arena.p + a.cur, 0, 64);
   dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
   hashes.ensure(ctx, (numApplied + B) * 32 + 64, numApplied * 32);
   deflList.ensure(ctx, B + 1);
-  u8* hashOut = hashes.p + numApplied * 32;
-  const DecodeTilesArgs dargs = decodeArgs(arena.p, B, cur - arenaLen0);
-  decode_tiles_begin(ctx, dargs);
-  struct SideJoin { Ctx& c; ~SideJoin() { side_join(c); } } sideJoin{ctx};   // also on the error paths: nothing of this call outlives it on the side stream
-  dbgMark("stage:tables");
+  a.hashOut = hashes.p + numApplied * 32;
+  a.dargs = decodeArgs(arena.p, B, a.cur - arenaLen0);
+  decode_tiles_begin(ctx, a.dargs);
+  trace.mark("stage:tables");
   // changes [c0, c1) are on the device once the copy stream has passed the piece's mark: hash on the side stream, decode on the main one
   auto processRange = [&](size_t c0, size_t c1, bool waitCopy, size_t mark) {
     if (c1 <= c0) return;
     if (waitCopy) copy_piece_wait(ctx, mark);   // both streams wait for the piece
     else side_fork(ctx);
-    sha_range(ctx, ShaTilesArgs{arena.p, chOff.p, chLen.p, hashOut, errWord.p, deflList.p, (u32)c0, (u32)c1}, true);
-    decode_tiles_range(ctx, dargs, (u32)c0, (u32)c1);
+    sha_range(ctx, ShaTilesArgs{arena.p, chOff.p, chLen.p, a.hashOut, errWord.p, deflList.p, (u32)c0, (u32)c1}, true);
+    decode_tiles_range(ctx, a.dargs, (u32)c0, (u32)c1);
   };
   side_fork(ctx);   // the side stream is ordered behind the tables
   if (Bq > 0) processRange(n, B, false, 0);   // queue entries: their bytes are on the device already
-  {
-    size_t byte0 = 0, ch0 = 0;
-    for (Piece& pc : pieces) {
-      if (!copiesFirst) queueCopy(pc, byte0, ch0);
-      processRange(ch0, pc.changeEnd, true, pc.mark);
-      byte0 = pc.byteEnd; ch0 = pc.changeEnd;
+  size_t byte0 = 0, ch0 = 0;
+  for (auto& pc : a.pieces) {
+    if (!a.copiesFirst) queueCopy(a, pc, byte0, ch0);
+    processRange(ch0, pc.changeEnd, true, pc.mark);
+    byte0 = pc.byteEnd; ch0 = pc.changeEnd;
+  }
+  trace.mark("stage:enqueued");
+  // the host's own list of the batch entries (bookkeeping at commit, queue hand-over): a helper thread fills it while this
+  // one keeps the device fed
+  auto fillBatch = [this, &a]() {
+    if (a.offsetsByDma) fillPairs(a);
+    batchStore.assign(a.pairs, a.pairs + a.B);
+    if (a.Bq > 0) { a.batchOriginal.assign(a.B, HostChange{0, 0}); for (size_t i = 0; i < a.Bq; i++) a.batchOriginal[a.n + i] = queueOriginal[i]; }
+  };
+  if (B >= (1u << 15)) a.fill = std::thread(fillBatch); else fillBatch();
+}
+inline void Engine::queueCopy(ApplyCall& a, ApplyCall::Piece& pc, size_t byte0, size_t ch0) {
+  const size_t m = pc.byteEnd - byte0;
+  if (m > 0) {
+    u8* dst = arena.p + a.arenaLen0 + byte0; const u8* src = a.blob ? a.blob + a.offsets[0] + byte0 : nullptr;
+    if (a.srcKind == a.SRC_PINNED) h2d_copy(ctx, dst, src, m);
+    else if (a.srcKind == a.SRC_DEVICE) d2d_copy(ctx, dst, src, m);
+    else {
+      u8* stage = hostArena.data() + a.arenaLen0 + byte0;
+      if (a.blob) parallel_copy(stage, src, m);
+      else parallel_gather(stage, a.bufs, a.lens, ch0, pc.changeEnd);
+      h2d_copy(ctx, dst, stage, m);
     }
   }
-  dbgMark("stage:enqueued");
-  timer.mark(); hostMark();
-  // The host's own list of the batch entries (bookkeeping at commit, queue hand-over) is filled by a helper thread while
-  // this one keeps the device fed; needBatch() joins it before the list is first read.
-  struct BatchFill { std::thread t; void join() { if (t.joinable()) t.join(); } ~BatchFill() { join(); } } batchFill;
-  auto fillBatch = [&, pairs, B, n, Bq]() {
-    if (offsetsByDma) fillPairs();
-    batch.assign(pairs, pairs + B);
-    if (Bq > 0) { batchOriginal.assign(B, HostChange{0, 0}); for (size_t i = 0; i < Bq; i++) batchOriginal[n + i] = queueOriginal[i]; }
-  };
-  if (B >= (1u << 15)) batchFill.t = std::thread(fillBatch); else fillBatch();
-  auto needBatch = [&]() { batchFill.join(); };
-  nvtx.next("inflate+decode-finish");
-  // ------------------------------------------------------------ 1. DEFLATEd changes
-  {
-    // Which changes of the batch are DEFLATEd (columnar.js:742)? Those are inflated on the device, behind the batch:
-    // flag -> scan -> ordered list -> k_inflate (decode into scratch, sizes) -> scan -> k_inflate (assemble in place); the originals stay.
-    // The hash / decode kernels above skipped them; they are hashed and decoded here, from the inflated bytes.
-    emit.ensure(ctx, B + 1); slot.ensure(ctx, B + 2);
-    dev_memset(ctx, flagWord.p + 8, 0, 4);
-    foreach(ctx, B, DeflateFlagKernel{arena.p, chOff.p, chLen.p, emit.p, flagWord.p + 8});
-    scan_exclusive(ctx, scanTmp, emit.p, slot.p, B);
-    u32 nd32 = 0, deflBytes = 0; readU32x2(slot.p + B, flagWord.p + 8, &nd32, &deflBytes);
-    const size_t nd = nd32;
-    dbgMark("sha:deflate-scanned");
-    if (nd > 0) {
-      // every stream is decoded once, into scratch (capacity: a few times its compressed size); the sizes give the places
-      // behind the batch, a second kernel assembles the changes there (copy; the rare stream that did not fit is decoded again)
-      foreach(ctx, B, CompactKernel{emit.p, slot.p, deflList.p});
-      inflLen.ensure(ctx, nd + 1); inflOff.ensure(ctx, nd + 2); patchTriples.ensure(ctx, 2 * nd + 2); inflCap.ensure(ctx, nd + 2); inflCapOff.ensure(ctx, nd + 2); inflOvf.ensure(ctx, nd + 1);
-      u32* origOff = patchTriples.p; u32* origLen = patchTriples.p + nd;
-      u32 factor = 4; while (factor > 1 && (u64)factor * deflBytes + 1024ull * nd >= 0xf0000000ULL) factor--;
-      const size_t scratchBytes = (size_t)factor * deflBytes + 1024 * nd + 64;
-      inflScratch.ensure(ctx, scratchBytes);
-      foreach(ctx, nd, InflateCapKernel{deflList.p, chLen.p, factor, inflCap.p});
-      scan_exclusive(ctx, scanTmp, inflCap.p, inflCapOff.p, nd);
-      InflateArgs ia{arena.p, chOff.p, chLen.p, deflList.p, nd, inflLen.p, nullptr, 0u, origOff, origLen, inflScratch.p, inflCapOff.p, inflOvf.p, errWord.p};
-      inflate_changes(ctx, INFL_SPECULATE, ia);
-      scan_exclusive(ctx, scanTmp, inflLen.p, inflOff.p, nd);
-      const size_t extra = readU32(inflOff.p + nd);
-      if (errSnapshot) throwKernelError(errSnapshot, actorIds);   // (the error word travels with every small read)
-      if ((u64)cur + extra + 64 >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: change arena limited to 4 GiB per document");
-      const size_t extraStart = cur; cur += extra;
-      side_join(ctx);   // the arena may move: nothing may still be reading it
-      arena.ensure(ctx, cur + 64, extraStart);
-      ia.arena = arena.p; ia.outOff = inflOff.p; ia.extraStart = (u32)extraStart;
-      inflate_changes(ctx, INFL_PLACE, ia);
-      dev_memset(ctx, arena.p + cur, 0, 64);
-      foreach(ctx, nd, InflatePatchKernel{deflList.p, inflLen.p, inflOff.p, (u32)extraStart, chOff.p, chLen.p});
-      foreach(ctx, nd, ShaKernel{arena.p, chOff.p, chLen.p, hashOut, errWord.p, deflList.p, nullptr});
-      inflNd = nd; inflExtraStart = extraStart; inflExtra = extra; inflPending = true;   // host bookkeeping happens in finishInflate()
-      dbgMark("sha:inflated");
-    }
+  pc.mark = copy_piece_record(ctx);
+}
+// the (offset, length) table of a packed batch, filled on the host (a few threads for 1M entries)
+inline void Engine::fillPairs(ApplyCall& a) {
+  if (!(a.blob && a.n > 0)) return;
+  const size_t n = a.n; const u64* offsets = a.offsets; HostChange* pairs = a.pairs; const u32 shift = (u32)(a.arenaLen0 - offsets[0]);
+  auto fill = [=](size_t lo, size_t hi) { for (size_t i = lo; i < hi; i++) { pairs[i].off = (u32)offsets[i] + shift; pairs[i].len = (u32)(offsets[i + 1] - offsets[i]); } };
+  const unsigned nt = n < (1u << 16) ? 1u : std::min<unsigned>(4, std::max(1u, std::thread::hardware_concurrency()));
+  if (nt == 1) fill(0, n);
+  else { std::vector<std::thread> ts; const size_t per = (n + nt - 1) / nt; for (unsigned t = 0; t < nt; t++) { const size_t lo = t * per, hi = std::min(n, lo + per); if (lo < hi) ts.emplace_back(fill, lo, hi); } for (auto& t : ts) t.join(); }
+}
+
+// ------------------------------------------------------------ 2. DEFLATEd changes
+// Which changes of the batch are DEFLATEd (columnar.js:742)? Those are inflated on the device, behind the batch:
+// flag -> scan -> ordered list -> k_inflate (decode into scratch, sizes) -> scan -> k_inflate (assemble in place); the originals stay.
+// The hash / decode kernels of the staging phase skipped them; they are hashed and decoded here, from the inflated bytes.
+inline void Engine::inflateBatch(ApplyCall& a) {
+  const size_t B = a.B;
+  emit.ensure(ctx, B + 1); slot.ensure(ctx, B + 2);
+  dev_memset(ctx, flagWord.p + 8, 0, 4);
+  foreach(ctx, B, DeflateFlagKernel{arena.p, chOff.p, chLen.p, emit.p, flagWord.p + 8});
+  scan_exclusive(ctx, scanTmp, emit.p, slot.p, B);
+  u32 nd32 = 0, deflBytes = 0; readU32x2(slot.p + B, flagWord.p + 8, &nd32, &deflBytes);
+  const size_t nd = nd32;
+  trace.mark("sha:deflate-scanned");
+  if (nd > 0) {
+    // every stream is decoded once, into scratch (capacity: a few times its compressed size); the sizes give the places
+    // behind the batch, a second kernel assembles the changes there (copy; the rare stream that did not fit is decoded again)
+    foreach(ctx, B, CompactKernel{emit.p, slot.p, deflList.p});
+    inflLen.ensure(ctx, nd + 1); inflOff.ensure(ctx, nd + 2); patchTriples.ensure(ctx, 2 * nd + 2); inflCap.ensure(ctx, nd + 2); inflCapOff.ensure(ctx, nd + 2); inflOvf.ensure(ctx, nd + 1);
+    u32* origOff = patchTriples.p; u32* origLen = patchTriples.p + nd;
+    u32 factor = 4; while (factor > 1 && (u64)factor * deflBytes + 1024ull * nd >= 0xf0000000ULL) factor--;
+    const size_t scratchBytes = (size_t)factor * deflBytes + 1024 * nd + 64;
+    inflScratch.ensure(ctx, scratchBytes);
+    foreach(ctx, nd, InflateCapKernel{deflList.p, chLen.p, factor, inflCap.p});
+    scan_exclusive(ctx, scanTmp, inflCap.p, inflCapOff.p, nd);
+    InflateArgs ia{arena.p, chOff.p, chLen.p, deflList.p, nd, inflLen.p, nullptr, 0u, origOff, origLen, inflScratch.p, inflCapOff.p, inflOvf.p, errWord.p};
+    inflate_changes(ctx, INFL_SPECULATE, ia);
+    scan_exclusive(ctx, scanTmp, inflLen.p, inflOff.p, nd);
+    const size_t extra = readU32(inflOff.p + nd);
+    if (errSnapshot) throwKernelError(errSnapshot);   // (the error word travels with every small read)
+    if ((u64)a.cur + extra + 64 >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: change arena limited to 4 GiB per document");
+    const size_t extraStart = a.cur; a.cur += extra;
+    side_join(ctx);   // the arena may move: nothing may still be reading it
+    arena.ensure(ctx, a.cur + 64, extraStart);
+    ia.arena = arena.p; ia.outOff = inflOff.p; ia.extraStart = (u32)extraStart;
+    inflate_changes(ctx, INFL_PLACE, ia);
+    dev_memset(ctx, arena.p + a.cur, 0, 64);
+    foreach(ctx, nd, InflatePatchKernel{deflList.p, inflLen.p, inflOff.p, (u32)extraStart, chOff.p, chLen.p});
+    foreach(ctx, nd, ShaKernel{arena.p, chOff.p, chLen.p, a.hashOut, errWord.p, deflList.p, nullptr});
+    a.inflNd = nd; a.inflExtraStart = extraStart; a.inflExtra = extra; a.inflPending = true;   // host bookkeeping happens in finishInflate()
+    trace.mark("sha:inflated");
   }
   // changes the tile kernel passed on (inflated ones, changes outside their tile's window), then the totals
-  { DecodeTilesArgs fin = dargs; fin.arena = arena.p; decode_tiles_list(ctx, fin, deflList.p, (u32)inflNd); decode_tiles_finish(ctx, fin, B); }
-  lastDeflCount = inflNd; lastDeflStart = inflExtraStart;
-  dbgMark("decode:finish-enqueued");
+  { DecodeTilesArgs fin = a.dargs; fin.arena = arena.p; decode_tiles_list(ctx, fin, deflList.p, (u32)a.inflNd); decode_tiles_finish(ctx, fin, B); }
+  lastDeflCount = a.inflNd; lastDeflStart = a.inflExtraStart;
+  trace.mark("decode:finish-enqueued");
   side_join(ctx);
-  timer.mark(); hostMark(); nvtx.next("gate");
-  // (parse errors surface with the first host round trip of the gate: the error word travels with every small read, and a
-  //  change that failed to parse has zero deps / ops so the kernels in between have nothing to walk)
-  // ------------------------------------------------------------ 2. causal gate
+}
+// Host side of the device inflate: which batch entries moved where. Not on the critical path: runs when the information
+// is first needed (queue hand-over, commit).
+inline void Engine::ApplyCall::finishInflate(Engine& e) {
+  if (!inflPending) return;
+  inflPending = false; const size_t nd = inflNd; Ctx& ctx = e.ctx;
+  u32* origOff = e.patchTriples.p; u32* origLen = e.patchTriples.p + nd;
+  e.pinnedScratch.ensure(5 * nd + 16); u32* ps = e.pinnedScratch.p;   // pinned: the five small copies queue up and complete with one sync
+  d2h(ctx, ps, e.deflList.p, nd * 4); d2h(ctx, ps + nd, e.inflLen.p, nd * 4); d2h(ctx, ps + 2 * nd, e.inflOff.p, nd * 4);
+  d2h(ctx, ps + 3 * nd, origOff, nd * 4); d2h(ctx, ps + 4 * nd, origLen, nd * 4);
+  if (e.hostArena.size() == inflExtraStart) {   // the mirror is complete up to here: keep it complete
+    e.hostArena.resize(inflExtraStart + inflExtra);
+    d2h(ctx, e.hostArena.data() + inflExtraStart, e.arena.p + inflExtraStart, inflExtra);
+  }
+  sync(ctx);
+  deflIdx.assign(ps, ps + nd); inflOrig.resize(nd);   // deflIdx is ascending: (batch index, original range), looked up by binary search
+  for (size_t k = 0; k < nd; k++) { const u32 bi = ps[k]; inflOrig[k] = HostChange{ps[3 * nd + k], ps[4 * nd + k]}; e.batchStore[bi] = HostChange{(u32)inflExtraStart + ps[2 * nd + k], ps[nd + k]}; }
+}
+inline HostChange Engine::ApplyCall::originalOf(size_t b) const {
+  if (!batchOriginal.empty() && batchOriginal[b].len) return batchOriginal[b];
+  auto it = std::lower_bound(deflIdx.begin(), deflIdx.end(), (u32)b);
+  return it != deflIdx.end() && *it == (u32)b ? inflOrig[it - deflIdx.begin()] : HostChange{0, 0};
+}
+
+// ------------------------------------------------------------ 3. causal gate
+// (parse errors surface with the first host round trip of the gate: the error word travels with every small read, and a
+//  change that failed to parse has zero deps / ops so the kernels in between have nothing to walk)
+inline void Engine::runGate(ApplyCall& a) {
+  const size_t B = a.B;
   depBase.ensure(ctx, B + 1); scan_exclusive(ctx, scanTmp, nDeps.p, depBase.p, B);
-  const size_t depBound = (cur - arenaLen0) / 32 + B + 1;   // every dependency occupies 32 bytes of its change: no need to read the exact total
+  const size_t depBound = (a.cur - a.arenaLen0) / 32 + B + 1;   // every dependency occupies 32 bytes of its change: no need to read the exact total
   depIdx.ensure(ctx, depBound + 1); primary.ensure(ctx, B); pass.ensure(ctx, B);
-  const size_t G = numApplied + B; const size_t tcap = pow2_at_least(2 * G + 2);
+  a.G = numApplied + B; const size_t tcap = pow2_at_least(2 * a.G + 2);
   hashTable.ensure(ctx, tcap); dev_memset(ctx, hashTable.p, 0xff, tcap * 4);
-  foreach(ctx, G, HashInsertKernel{hashes.p, hashTable.p, (u64)tcap - 1});
+  foreach(ctx, a.G, HashInsertKernel{hashes.p, hashTable.p, (u64)tcap - 1});
   foreach(ctx, B, ResolveDepsKernel{arena.p, hashes.p, hashTable.p, (u64)tcap - 1, hot.p, nDeps.p, numApplied, depBase.p, depIdx.p, primary.p});
   fill32(pass.p, 1, B);
   dev_memset(ctx, flagWord.p + 12, 0, 4);
   foreach(ctx, B, GateDupFlagKernel{primary.p, numApplied, flagWord.p + 12});
-  bool copiesChecked = false, haveCopies = false; u32 decTot[4] = {0, 0, 0, 0};
+  bool copiesChecked = false, haveCopies = false; u32* decTot = a.decTot;
   for (size_t iter = 0; iter <= B + 1; iter += 2) {   // two sweeps per host round trip: the common batch settles in the first
     if (haveCopies) break;
     foreach(ctx, B, RelaxKernel{depBase.p, depIdx.p, nDeps.p, primary.p, numApplied, pass.p, flagWord.p, (u32)B + 1});
@@ -367,9 +349,9 @@ inline void Engine::applyChangesOnce(const u8* const* bufs, const size_t* lens, 
     u32 again = 0, copies = 0;
     { void* dst[6] = {&again, &copies, &decTot[0], &decTot[1], &decTot[2], &decTot[3]};
       readWords({{flagWord.p, 4}, {flagWord.p + 12, 4}, {decTotalsPtr(), 4}, {decTotalsPtr() + 1, 4}, {decTotalsPtr() + 2, 4}, {decTotalsPtr() + 3, 4}}, dst); }
-    checkErr(actorIds);   // free: the error word came with the read
+    checkErr();   // free: the error word came with the read
     if (iter == 0 && decodeOverflowed(decTot)) {   // the raw row tables were too small for this batch: grown, decoded again (same results otherwise)
-      runDecodeTiles(arena.p, B, cur - arenaLen0, deflList.p, inflNd, inflExtraStart);   // the whole batch is resident by now (inflated changes re-pointed)
+      runDecodeTiles(arena.p, B, a.cur - a.arenaLen0, deflList.p, a.inflNd, a.inflExtraStart);   // the whole batch is resident by now (inflated changes re-pointed)
       void* d2[4] = {&decTot[0], &decTot[1], &decTot[2], &decTot[3]};
       readWords({{decTotalsPtr(), 4}, {decTotalsPtr() + 1, 4}, {decTotalsPtr() + 2, 4}, {decTotalsPtr() + 3, 4}}, d2);
       if (decTot[2]) throw Error(AMG_ERR_INTERNAL, "amgpu: decode row tables overflowed twice");
@@ -384,7 +366,7 @@ inline void Engine::applyChangesOnce(const u8* const* bufs, const size_t* lens, 
       foreach(ctx, B, GateBestKernel{primary.p, pass.p, numApplied, gateBest.p});
       foreach(ctx, B, RelaxCopiesKernel{depBase.p, depIdx.p, nDeps.p, primary.p, numApplied, gateBest.p, pass.p, flagWord.p, (u32)B + 1});
       const u32 again = readU32(flagWord.p);
-      checkErr(actorIds);
+      checkErr();
       if (!again) break;
     }
     dev_memset(ctx, gateBest.p, 0xff, B * 8);
@@ -393,399 +375,383 @@ inline void Engine::applyChangesOnce(const u8* const* bufs, const size_t* lens, 
     if (depTotal) foreach(ctx, depTotal, GateDepWinnerKernel{gateBest.p, numApplied, depIdx.p});
     foreach(ctx, B, GateWinnerKernel{gateBest.p, numApplied, primary.p});
   }
-  dbgMark("gate:settled");
+  trace.mark("gate:settled");
   applied.ensure(ctx, B); appRank.ensure(ctx, B + 1); isRow.ensure(ctx, B + 1);
   dev_memset(ctx, flagWord.p, 0, 8);
   foreach(ctx, B, AppliedFlagKernel{primary.p, pass.p, numApplied, applied.p, isRow.p, flagWord.p});
   u32 stats[2]; readU32x2(flagWord.p, flagWord.p + 1, &stats[0], &stats[1]);
-  const size_t numNew = stats[0]; const bool inOrder = stats[1] <= 1; batchInOrder = inOrder;
-  std::vector<u8> appliedH; std::vector<u32> primaryH, appRankH;
-  if (inOrder) scan_exclusive(ctx, scanTmp, isRow.p, appRank.p, B);
+  a.numNew = stats[0]; a.inOrder = stats[1] <= 1;
+  if (a.inOrder) scan_exclusive(ctx, scanTmp, isRow.p, appRank.p, B);
   else {
     sortKeys.ensure(ctx, B); sortVals.ensure(ctx, B);
     foreach(ctx, B, PassKeyKernel{pass.p, applied.p, sortKeys.p, sortVals.p});
     sortPairs(sortKeys, sortVals, B, 32);
-    foreach(ctx, B, RankFromOrderKernel{sortVals.p, appRank.p, numNew});
+    foreach(ctx, B, RankFromOrderKernel{sortVals.p, appRank.p, a.numNew});
   }
-  if (numNew < B || !inOrder) {
-    appliedH.resize(B); primaryH.resize(B); appRankH.resize(B);
-    d2h(ctx, appliedH.data(), applied.p, B); d2h(ctx, primaryH.data(), primary.p, B * 4); d2h(ctx, appRankH.data(), appRank.p, B * 4); sync(ctx);
+  if (a.numNew < B || !a.inOrder) {
+    a.appliedH.resize(B); a.primaryH.resize(B); a.appRankH.resize(B);
+    d2h(ctx, a.appliedH.data(), applied.p, B); d2h(ctx, a.primaryH.data(), primary.p, B * 4); d2h(ctx, a.appRankH.data(), appRank.p, B * 4); sync(ctx);
   }
-  if (!haveHashGraph && numNew < B) throw NeedHistory{};   // a change waits for (or repeats) something older than the loaded heads
+  if (!haveHashGraph && a.numNew < B) throw NeedHistory{};   // a change waits for (or repeats) something older than the loaded heads
   // the queue after this call: every batch entry whose hash is still not applied (new.js:1569-1570, 1832)
-  std::vector<HostChange> newQueue, newQueueOriginal;
-  if (numNew < B) { needBatch(); finishInflate(); }
-  if (numNew < B) for (size_t b = 0; b < B; b++) {
-    const u32 pr = primaryH[b];
-    const bool hashApplied = pr < numApplied || appliedH[pr - numApplied];
-    if (!hashApplied) { newQueue.push_back(batch[b]); newQueueOriginal.push_back(originalOf(b)); }
+  if (a.numNew < B) {
+    a.needBatch(); a.finishInflate(*this);
+    for (size_t b = 0; b < B; b++) {
+      const u32 pr = a.primaryH[b];
+      const bool hashApplied = pr < numApplied || a.appliedH[pr - numApplied];
+      if (!hashApplied) { a.newQueue.push_back(batchStore[b]); a.newQueueOriginal.push_back(a.originalOf(b)); }
+    }
   }
-  timer.mark(); hostMark(); nvtx.next("actors+seq+finalize");
-  std::vector<std::string> actorsNow = actorIds; std::vector<u64> clockNow = clock; std::vector<u32> actorCntH; std::vector<std::pair<u32, u32>> actorRepNow = actorRep;
-  size_t M = 0, P = 0, N = numRows, numPairs = numSucc; u64 maxOpNow = maxOp; bool hasUnknownColsCall = false;
-  IdTable idt{nullptr, nullptr, 0};
-  std::vector<std::array<u8, 32>> headsNow = heads; std::vector<u32> headIdxNow;
-  if (numNew > 0) {
-    // ---------------------------------------------------------- 3. actors
-    authorSlot.ensure(ctx, B); newSlots.ensure(ctx, B + 1); u32 fresh = 0;
-    while (true) {   // grow the table until the distinct authors fit at load factor <= 1/2
-      dev_memset(ctx, flagWord.p, 0, 8);
-      foreach(ctx, B, ActorInternKernel{arena.p, hot.p, applied.p, appRank.p, actorSlots.p, (u64)actorCap - 1, authorSlot.p, flagWord.p + 1});
-      foreach(ctx, B, NewActorKernel{hot.p, applied.p, authorSlot.p, actorSlots.p, newSlots.p, flagWord.p});
-      u32 full = 0; readU32x2(flagWord.p, flagWord.p + 1, &fresh, &full);
-      if (!full && (actorIds.size() + fresh) * 2 <= actorCap) break;
-      actorCap *= 4; actorSlots.ensure(ctx, actorCap); rebuildActorTable();
-    }
-    if (fresh > 0) {
-    dbgMark("actors:interned");
-      // slot numbers, slot records and id bytes of the new actors in ONE round trip (gathered into a staging buffer)
-      static const u32 ACTOR_STAGE = 64;
-      hashTmp.ensure(ctx, (size_t)fresh * (4 + sizeof(ActorSlot) + ACTOR_STAGE) + 64);
-      u8* stageD = hashTmp.p; const size_t recsAt = ((size_t)fresh * 4 + 15) & ~(size_t)15, bytesAt = recsAt + (size_t)fresh * sizeof(ActorSlot), stageLen = bytesAt + (size_t)fresh * ACTOR_STAGE;
-      foreach(ctx, fresh, GatherNewActorsKernel{arena.p, actorSlots.p, newSlots.p, reinterpret_cast<u32*>(stageD), reinterpret_cast<ActorSlot*>(stageD + recsAt), stageD + bytesAt, ACTOR_STAGE});
-      std::vector<u8> stageH(stageLen); d2h(ctx, stageH.data(), stageD, stageLen); sync(ctx);
-      std::vector<u32> slotsH(fresh); memcpy(slotsH.data(), stageH.data(), (size_t)fresh * 4);
-      std::vector<ActorSlot> recs(fresh); memcpy(recs.data(), stageH.data() + recsAt, (size_t)fresh * sizeof(ActorSlot));
-      std::vector<u32> order(fresh); for (u32 i = 0; i < fresh; i++) order[i] = i;
-      std::sort(order.begin(), order.end(), [&](u32 a, u32 b) { return recs[a].first < recs[b].first; });
-      std::vector<u32> ids(fresh), nums(fresh); actorsNow.reserve(actorsNow.size() + fresh);   // async copies target the strings: no reallocation below
-      bool longIds = false;
-      for (u32 k = 0; k < fresh; k++) {
-        const ActorSlot& r = recs[order[k]]; ids[k] = slotsH[order[k]]; nums[k] = (u32)actorsNow.size();
-        actorsNow.emplace_back(r.repLen, '\0');
-        if (r.repLen <= ACTOR_STAGE) memcpy(&actorsNow.back()[0], stageH.data() + bytesAt + (size_t)order[k] * ACTOR_STAGE, r.repLen);
-        else { d2h(ctx, &actorsNow.back()[0], arena.p + r.repOff, r.repLen); longIds = true; }   // from the device copy: the host mirror may still be filling
-        actorRepNow.emplace_back(r.repOff, r.repLen);
-      }
-      if (longIds) sync(ctx);
-      if (actorsNow.size() > 65535) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: more than 65535 actors in one document");
-      sortVals.ensure(ctx, 2 * fresh); h2d(ctx, sortVals.p, ids.data(), fresh * 4); h2d(ctx, sortVals.p + fresh, nums.data(), fresh * 4);
-      foreach(ctx, fresh, SetActorNumKernel{actorSlots.p, sortVals.p, sortVals.p + fresh});
-    }
-    const size_t A = actorsNow.size(); clockNow.resize(A, 0);
-    {   // rank of every actor in hex-string order (== byte order of the raw ids; new.js:64-65, 1180, 1198)
-      std::vector<u32> order(A), rank(A); for (size_t i = 0; i < A; i++) order[i] = (u32)i;
-      std::sort(order.begin(), order.end(), [&](u32 a, u32 b) { return actorsNow[a] < actorsNow[b]; });
-      for (size_t i = 0; i < A; i++) rank[order[i]] = (u32)i;
-      actorRank.ensure(ctx, A + 1); h2d(ctx, actorRank.p, rank.data(), A * 4);
-    }
-    const int rb = bits_for(A > 1 ? A - 1 : 1);
-    dbgMark("actors:numbered");
-    Ord ord{actorRank.p, rb};
-    amapBase.ensure(ctx, B + 1); rowSlot.ensure(ctx, B + 1);
-    foreach(ctx, B, MaskedCountKernel{nActors.p, applied.p, rowSlot.p});
-    scan_exclusive(ctx, scanTmp, rowSlot.p, amapBase.p, B);
-    amap.ensure(ctx, B + (cur - arenaLen0) / 2 + 2);   // author + one entry per other-actor table entry (>= 2 bytes each): bound instead of a round trip
-    foreach(ctx, B, ActorMapKernel{arena.p, hot.p, nActors.p, applied.p, appRank.p, actorSlots.p, (u64)actorCap - 1, amapBase.p, amap.p, errWord.p});
-    dbgMark("actors:mapped");
-    // ---------------------------------------------------------- 4. sequence numbers
-    changeActor.ensure(ctx, B); actorCnt.ensure(ctx, A + 1); actorBaseD.ensure(ctx, A + 1); seqSlot.ensure(ctx, numNew + 1);
-    dev_memset(ctx, actorCnt.p, 0, (A + 1) * 4);
-    foreach(ctx, B, ChangeActorKernel{amapBase.p, amap.p, applied.p, changeActor.p, actorCnt.p});
-    {
-      const u64 ew = fetchErr();
-      if ((ew & 0xff) == KE_UNKNOWN_ACTOR) {   // name the actor like the reference does (new.js:1446): re-read that change's actor table
-        const size_t b = (size_t)(ew >> 8); ChangeHot m0; u32 na0 = 1; d2h(ctx, &m0, hot.p + b, sizeof(ChangeHot)); d2h(ctx, &na0, nActors.p + b, 4); sync(ctx);
-        std::vector<u8> bytes(m0.len); d2h(ctx, bytes.data(), arena.p + m0.off, m0.len); sync(ctx);
-        ByteReader r(bytes.data(), m0.otherOff - m0.off, m0.len); std::string culprit;
-        for (u32 k = 0; k < na0 && !r.err; k++) {
-          u32 off, len; if (k == 0) { off = m0.actorOff - m0.off; len = m0.actorLen; } else { len = (u32)r.uleb(); off = r.pos; r.skip(len); }
-          if (r.err) break;
-          const std::string id((const char*)bytes.data() + off, len);
-          if (std::find(actorsNow.begin(), actorsNow.end(), id) == actorsNow.end()) { culprit = id; break; }
-        }
-        if (!culprit.empty()) throw Error(AMG_ERR_RANGE, "actorId " + hex_of((const u8*)culprit.data(), culprit.size()) + " is not known to document");
-      }
-      if (ew) throwKernelError(ew, actorsNow);
-    }
-    scan_exclusive(ctx, scanTmp, actorCnt.p, actorBaseD.p, A);
-    DBuf<u64>& clockDev = pairKey;   // scratch reuse before the succ phase
-    clockDev.ensure(ctx, A + 1); h2d(ctx, clockDev.p, clockNow.data(), A * 8);
-    dev_memset(ctx, seqSlot.p, 0xff, (numNew + 1) * 4); dev_memset(ctx, flagWord.p, 0, 4);
-    foreach(ctx, B, SeqScatterKernel{hot.p, applied.p, changeActor.p, appRank.p, actorBaseD.p, actorCnt.p, clockDev.p, seqSlot.p, flagWord.p});
-    foreach(ctx, B, SeqMonoKernel{hot.p, applied.p, changeActor.p, actorBaseD.p, actorCnt.p, clockDev.p, seqSlot.p, flagWord.p});
-    actorCntH.resize(A); d2h(ctx, actorCntH.data(), actorCnt.p, A * 4);
-    if (readU32(flagWord.p)) {
-      // error path: replay the sequence check in application order on the host to produce the reference's message
-      std::vector<ChangeHot> mh(B); std::vector<u32> ca(B), ar(B); std::vector<u8> ap(B);
-      d2h(ctx, mh.data(), hot.p, B * sizeof(ChangeHot)); d2h(ctx, ca.data(), changeActor.p, B * 4); d2h(ctx, ar.data(), appRank.p, B * 4); d2h(ctx, ap.data(), applied.p, B); sync(ctx);
-      std::vector<u32> byRank(numNew, 0); for (size_t b = 0; b < B; b++) if (ap[b]) byRank[ar[b]] = (u32)b;
-      std::vector<u64> clk = clockNow;
-      for (size_t k = 0; k < numNew; k++) {
-        const u32 b = byRank[k]; const u64 expected = clk[ca[b]] + 1; const std::string actorHex = hex_of((const u8*)actorsNow[ca[b]].data(), actorsNow[ca[b]].size());
-        if (mh[b].seq < expected) throw Error(AMG_ERR_RANGE, "Reuse of sequence number " + std::to_string(mh[b].seq) + " for actor " + actorHex);
-        if (mh[b].seq > expected) throw Error(AMG_ERR_RANGE, "Skipped sequence number " + std::to_string(expected) + " for actor " + actorHex);
-        clk[ca[b]] = mh[b].seq;
-      }
-      throw Error(AMG_ERR_INTERNAL, "amgpu: sequence check disagreement");
-    }
-    for (size_t a = 0; a < A; a++) clockNow[a] += actorCntH[a];
-    dbgMark("seq:checked");
-    // ---------------------------------------------------------- 5. ops of the applied changes
-    // The rows were decoded with the headers (step 1), in batch order. When every change of the batch is applied the
-    // op / pred ranges of the changes are the raw ones; otherwise they are the scans over the applied changes only.
-    timeBase.ensure(ctx, B + 1);
-    const bool allApplied = numNew == B;
-    opBase.ensure(ctx, B + 1); predBase.ensure(ctx, B + 1); u32* opBaseP = opBase.p; u32* predBaseP = predBase.p;
-    const u32 anyLarge = decTot[3] & 1u; hasUnknownColsCall = (decTot[3] & 2u) != 0;
-    // first op / pred of every applied change in batch order (the raw rows themselves lie in tile arrival order, rawBase)
-    if (allApplied) { scan_exclusive(ctx, scanTmp, nOps.p, opBase.p, B); scan_exclusive(ctx, scanTmp, nPreds.p, predBase.p, B); M = decTot[0]; P = decTot[1]; }
-    else {
-      foreach(ctx, B, MaskedCountKernel{nOps.p, applied.p, rowSlot.p}); scan_exclusive(ctx, scanTmp, rowSlot.p, opBase.p, B);
-      foreach(ctx, B, MaskedCountKernel{nPreds.p, applied.p, rowSlot.p}); scan_exclusive(ctx, scanTmp, rowSlot.p, predBase.p, B);
-      u32 m32 = 0, p32 = 0; void* dst[2] = {&m32, &p32}; readWords({{opBase.p + B, 4}, {predBase.p + B, 4}}, dst); M = m32; P = p32;
-    }
-    if (decTot[0] >= 0x7fffffffu || decTot[1] >= 0x7fffffffu) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: more than 2^31 operations in one call");
-    dbgMark("decode:counts");
-    if (!inOrder) {
-      perm.ensure(ctx, B + 1); dev_memset(ctx, perm.p, 0, (B + 1) * 4);
-      foreach(ctx, B, OpsInOrderKernel{nOps.p, applied.p, appRank.p, perm.p});
-      scan_exclusive(ctx, scanTmp, perm.p, perm.p, numNew);
-    }
-    foreach(ctx, B, TimeBaseKernel{perm.p, applied.p, appRank.p, opBaseP, inOrder ? 1 : 0, timeBase.p});
-    DBuf<u64>& maxOpD = pairSucc; maxOpD.ensure(ctx, 1); h2d(ctx, maxOpD.p, &maxOpNow, 8);
-    foreach(ctx, B, MaxOpKernel{hot.p, nOps.p, applied.p, decErr.p, maxOpD.p, errWord.p});
-    d2h(ctx, &maxOpNow, maxOpD.p, 8);
-    RawRows raw = rawRows();
-    lastNumLarge = 0;
-    if (anyLarge) {   // changes with more than SMALL_CHANGE_OPS ops: (column, change)-parallel expansion into their reserved rows
-      largeFlag.ensure(ctx, B + 1); largeSlot.ensure(ctx, B + 2); largeList.ensure(ctx, B + 1);
-      foreach(ctx, B, LargeFlagKernel{nOps.p, applied.p, largeFlag.p});
-      scan_exclusive(ctx, scanTmp, largeFlag.p, largeSlot.p, B);
-      lastNumLarge = readU32(largeSlot.p + B);
-      if (lastNumLarge > 0) {
-        foreach(ctx, B, CompactKernel{largeFlag.p, largeSlot.p, largeList.p});
-        // bulk changes (thousands of ops in one change): their columns are expanded in parallel by the token / record
-        // decoders of doccols.cuh, column by column; whatever those decline (non-canonical streams, columns that do not hold
-        // exactly the op count) and all other large changes go through DecodeColumnKernel (one thread per column)
-        u32 hugeMask = 0;
-        if (lastNumLarge <= 8) hugeMask = decodeHugeChanges(raw, lastNumLarge);
-        foreach(ctx, (size_t)NCOLS * lastNumLarge, DecodeColumnKernel{arena.p, largeList.p, lastNumLarge, hot.p, nOps.p, nPreds.p, rawBase.p, rawPredBase.p, applied.p, raw, errWord.p, hugeDone.p});
-        (void)hugeMask;
-      }
-    }
-    for (DBuf<u64>* b : {&o_id, &o_obj, &o_key}) b->ensure(ctx, M + 1);
-    o_predId.ensure(ctx, P + 1);
-    for (DBuf<u32>* b : {&o_keyStrOff, &o_keyStrLen, &o_flags, &o_valLen, &o_valOff, &o_predOff, &o_predNum, &o_change, &o_time}) b->ensure(ctx, M + 1);
-    OpRows ops{o_id.p, o_obj.p, o_key.p, o_keyStrOff.p, o_keyStrLen.p, o_flags.p, o_valLen.p, o_valOff.p, o_predOff.p, o_predNum.p, o_change.p, o_time.p, o_predId.p};
-    foreach(ctx, M, FinalizeOpsKernel{B, hot.p, nActors.p, opBaseP, predBaseP, rawBase.p, rawPredBase.p, timeBase.p, amapBase.p, amap.p, applied.p, raw, ops, errWord.p});
-    checkErr(actorsNow);
-    dbgMark("decode:finalized");
-    timer.mark(); hostMark(); nvtx.next("opset");
-    // ---------------------------------------------------------- 6. op set
-    if (maxOpNow >= (1ULL << 40)) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: op counters above 2^40");
-    const int ordBits = bits_for(maxOpNow) + rb;
-    isRow.ensure(ctx, M + 1); rowSlot.ensure(ctx, M + 1); rowOfOp.ensure(ctx, M + 1);
-    foreach(ctx, M, RowFlagKernel{o_flags.p, isRow.p}); scan_exclusive(ctx, scanTmp, isRow.p, rowSlot.p, M);
-    const size_t R = readU32(rowSlot.p + M); N = numRows + R;
-    if (N >= (1u << 29)) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: more than 2^29 document rows");
-    doc.ensure(ctx, N + 1, numRows);
-    DocRows w = doc.view();
-    foreach(ctx, M, AppendRowsKernel{ops, isRow.p, rowSlot.p, numRows, w, rowOfOp.p});
-    const size_t icap = pow2_at_least(2 * N + 2); idKeys.ensure(ctx, icap); idVals.ensure(ctx, icap); dev_memset(ctx, idKeys.p, 0, icap * 8);
-    idt = IdTable{idKeys.p, idVals.p, (u64)icap - 1};
-    foreach(ctx, N, IdInsertKernel{w.id, idt, errWord.p});
-    objRow.ensure(ctx, N + 1); elemRow.ensure(ctx, N + 1); parentRow.ensure(ctx, N + 1);
-    foreach(ctx, N, ResolveRowsKernel{w, idt, ord, numRows, objRow.p, elemRow.p, parentRow.p, errWord.p});
-    checkErr(actorsNow);
-    dbgMark("opset:resolved");
-    // map keys: intern, verify, rank distinct keys with an LSD string sort
-    const size_t kcap = pow2_at_least(2 * N + 2); keySlots.ensure(ctx, kcap); keySlot.ensure(ctx, N + 1); repList.ensure(ctx, N + 1); repCount.ensure(ctx, 4);
-    foreach(ctx, kcap, KeySlotInitKernel{keySlots.p});
-    foreach(ctx, N, KeyInternKernel{arena.p, w, keySlots.p, (u64)kcap - 1, keySlot.p});
-    dev_memset(ctx, repCount.p, 0, 16);
-    foreach(ctx, N, KeyVerifyKernel{arena.p, w, keySlots.p, keySlot.p, repList.p, repCount.p, errWord.p});
-    u32 rc[2]; readU32x2(repCount.p, repCount.p + 1, &rc[0], &rc[1]);
-    const size_t D = rc[0]; const u32 maxKeyLen = rc[1];
-    dbgMark("opset:keys-interned");
-    if (D > 0) {
-      sortKeys.ensure(ctx, D); sortVals.ensure(ctx, D);
-      d2d(ctx, sortVals.p, repList.p, D * 4);
-      const int chunks = (int)((maxKeyLen + 6) / 7);
-      for (int ch = std::max(chunks, 1) - 1; ch >= 0; ch--) {
-        foreach(ctx, D, KeyChunkKernel{arena.p, w, sortVals.p, (u32)ch * 7, sortKeys.p});
-        sortPairs(sortKeys, sortVals, D, 64);
-      }
-      foreach(ctx, D, KeyRankKernel{sortVals.p, keySlot.p, keySlots.p});
-    }
-    // RGA order of every list: sibling sort, Euler tour, pointer jumping
-    listPos.ensure(ctx, N + 1); insItems.ensure(ctx, N + 1); emit.ensure(ctx, N + 1); slot.ensure(ctx, N + 2);
-    foreach(ctx, N, InsertFlagKernel{w, emit.p}); scan_exclusive(ctx, scanTmp, emit.p, slot.p, N);
-    const size_t I = readU32(slot.p + N);
-    dbgMark("opset:inserts-counted");
-    if (I > 0) {
-      const int parentBits = bits_for(N) + 1;
-      if (ordBits + parentBits > 64) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: opId range x document size exceeds the 64-bit sibling sort key");
-      foreach(ctx, N, CompactKernel{emit.p, slot.p, insItems.p});
-      sortKeys.ensure(ctx, I); sortVals.ensure(ctx, I);
-      foreach(ctx, I, SiblingKeyKernel{w, insItems.p, parentRow.p, objRow.p, ord, ordBits, sortKeys.p, errWord.p});
-      d2d(ctx, sortVals.p, insItems.p, I * 4);
-      sortPairs(sortKeys, sortVals, I, ordBits + parentBits);
-      checkErr(actorsNow);
-      itemIdx.ensure(ctx, N + 1); objSlot.ensure(ctx, N + 2);
-      foreach(ctx, I, ItemIndexKernel{sortVals.p, itemIdx.p});
-      foreach(ctx, N, ListObjFlagKernel{w, emit.p}); scan_exclusive(ctx, scanTmp, emit.p, objSlot.p, N);
-      const size_t Lo = readU32(objSlot.p + N);
-      const size_t S = 2 * I + 2 * Lo; eNext.ensure(ctx, S + 1); eRank.ensure(ctx, S + 1); ePacked.ensure(ctx, S + 1); ePacked2.ensure(ctx, S + 1);
-      foreach(ctx, S, EulerInitKernel{eNext.p, eRank.p});
-      foreach(ctx, I, EulerLinkKernel{sortKeys.p, ordBits, itemIdx.p, objSlot.p, eNext.p, eRank.p, I});
-      foreach(ctx, S, ListRankPackKernel{eNext.p, eRank.p, ePacked.p});
-      const int rounds = bits_for(S);
-      for (int k = 0; k < rounds; k++) {
-        foreach(ctx, S, ListRankPackedKernel{ePacked.p, ePacked2.p});
-        std::swap(ePacked.p, ePacked2.p); std::swap(ePacked.cap, ePacked2.cap);
-      }
-      foreach(ctx, S, ListRankUnpackKernel{ePacked.p, eRank.p});
-      foreach(ctx, N, ListPosKernel{eRank.p, elemRow.p, objRow.p, itemIdx.p, objSlot.p, (u32)I, listPos.p});
-    } else dev_memset(ctx, listPos.p, 0, (N + 1) * 4);
-    checkErr(actorsNow);
-    dbgMark("opset:list-ranked");
-    // document order: stable LSD over (object, key rank | list position, opId within the key / element)
-    perm.ensure(ctx, N + 1); pos.ensure(ctx, N + 1); sortKeys.ensure(ctx, N);
-    foreach(ctx, N, IotaKernel{perm.p});
-    const int fieldBits[3] = {ordBits + 1, bits_for(N), ordBits + 1};
-    for (int f = 0; f < 3; f++) {
-      foreach(ctx, N, DocKeyKernel{f, w, perm.p, listPos.p, keySlots.p, keySlot.p, ord, sortKeys.p});
-      sortPairs(sortKeys, perm, N, fieldBits[f]);
-    }
-    foreach(ctx, N, InversePermKernel{perm.p, pos.p});
-    dbgMark("opset:doc-ordered(enqueued)");
-    // succ lists
-    numPairs = numSucc + P;
-    pairKey.ensure(ctx, numPairs + 1); pairSucc.ensure(ctx, numPairs + 1); pairIdx.ensure(ctx, numPairs + 1); pairPos.ensure(ctx, numPairs + 1); pairTime.ensure(ctx, numPairs + 1);
-    foreach(ctx, M, DelElemCheckKernel{ops, idt, w, errWord.p});
-    checkErr(actorsNow);
-    foreach(ctx, numRows, OldPairsKernel{succOff.p, succ.p, pos.p, ord, pairKey.p, pairIdx.p, pairSucc.p, pairPos.p, pairTime.p});
-    foreach(ctx, M, PredPairsKernel{ops, idt, pos.p, rowOfOp.p, w, elemRow.p, keySlot.p, ord, pairKey.p, pairIdx.p, pairSucc.p, pairPos.p, pairTime.p, numSucc, errWord.p});
-    foreach(ctx, M, DelKeyCheckKernel{arena.p, ops, idt, w, errWord.p});
-    foreach(ctx, M, IncCheckKernel{ops, idt, w, arena.p, errWord.p});
-    {
-      const u64 w2 = fetchErr();
-      if (w2) {
-        if ((w2 & 0xff) == KE_PRED_MISSING) { u64 pid = 0; d2h(ctx, &pid, o_predId.p + (w2 >> 8), 8); sync(ctx); actorIds.swap(actorsNow); std::string t = opIdText(pid); actorIds.swap(actorsNow); throw Error(AMG_ERR_RANGE, "no matching operation for pred: " + t); }
-        if ((w2 & 0xff) == KE_UNKNOWN_COUNTER) { u64 oid = 0; d2h(ctx, &oid, o_id.p + (w2 >> 8), 8); sync(ctx); actorIds.swap(actorsNow); std::string t = opIdText(oid); actorIds.swap(actorsNow); throw Error(AMG_ERR_RANGE, "increment operation " + t + " for unknown counter"); }
-        throwKernelError(w2, actorsNow);
-      }
-    }
-    sortPairs(pairKey, pairIdx, numPairs, ordBits);
-    foreach(ctx, numPairs, PairPosKeyKernel{pairPos.p, pairIdx.p, pairKey.p});
-    sortPairs(pairKey, pairIdx, numPairs, bits_for(N));
-    succCnt.ensure(ctx, N + 2); newSuccCnt.ensure(ctx, N + 2); newSuccOff.ensure(ctx, N + 2); firstNewSucc.ensure(ctx, N + 2); newSucc.ensure(ctx, numPairs + 1);
-    dev_memset(ctx, succCnt.p, 0, (N + 2) * 4); dev_memset(ctx, newSuccCnt.p, 0, (N + 2) * 4); dev_memset(ctx, firstNewSucc.p, 0xff, (N + 2) * 4);
-    foreach(ctx, numPairs, CountSuccKernel{pairPos.p, succCnt.p});
-    foreach(ctx, numPairs, NewSuccFlagKernel{pairPos.p, pairTime.p, newSuccCnt.p});
-    foreach(ctx, numPairs, FirstSuccTimeKernel{pairPos.p, pairTime.p, firstNewSucc.p});
-    scan_exclusive(ctx, scanTmp, succCnt.p, newSuccOff.p, N);
-    newSuccTime.ensure(ctx, numPairs + 1);
-    foreach(ctx, numPairs, WriteSuccKernel{pairIdx.p, pairSucc.p, newSucc.p, pairTime.p, newSuccTime.p});
-    sorted.ensure(ctx, N + 1);
-    foreach(ctx, N, GatherRowsKernel{w, sorted.view(), perm.p});
-    dbgMark("opset:succ+gather(enqueued)");
-    timer.mark(); hostMark(); nvtx.next("patch");
-    // ---------------------------------------------------------- 7. incremental patch
-    if (wantPatch) {
-      objPos.ensure(ctx, N + 1);
-      foreach(ctx, N, ObjPosKernel{perm.p, objRow.p, pos.p, objPos.p});
-      workView = w;
-      buildPatch(sorted.view(), N, false, &ops, M, &idt, rowOfOp.p, pos.p, actorsNow, out, newSuccOff.p, newSucc.p);
-    }
-    checkErr(actorsNow);
-    timer.mark(); hostMark(); nvtx.next("heads+commit");
-    // heads
-    dbgMark("commit:begin");
-    {
-      DBuf<u32>& isDep = groupLinked; isDep.ensure(ctx, G + 1); dev_memset(ctx, isDep.p, 0, (G + 1) * 4);
-      foreach(ctx, B, MarkDepsKernel{applied.p, nDeps.p, depBase.p, depIdx.p, isDep.p});
-      emit.ensure(ctx, B + 1); slot.ensure(ctx, B + 2); objStart.ensure(ctx, B + 1);
-      foreach(ctx, B, HeadFlag2Kernel{applied.p, isDep.p, numApplied, emit.p});
-      scan_exclusive(ctx, scanTmp, emit.p, slot.p, B);
-      foreach(ctx, B, CompactKernel{emit.p, slot.p, objStart.p});
-      // one round trip for the whole answer (HeadsPackKernel); a second one only if the call leaves more heads than the block holds
-      const u32 nOld = (u32)headIdx.size(); u32 cap = 64, nh = 0; std::vector<u32> pack;
-      headsPack.ensure(ctx, nOld + 1);
-      if (nOld) h2d(ctx, headsPack.p, headIdx.data(), nOld * 4);
-      for (;;) {
-        const size_t words = 1 + (size_t)nOld + 9 * (size_t)cap;
-        headsOut.ensure(ctx, words + 1); pack.resize(words);
-        foreach(ctx, std::max<size_t>(std::max<size_t>(nOld, cap), 1), HeadsPackKernel{slot.p + B, objStart.p, hashes.p + numApplied * 32, appRank.p, isDep.p, headsPack.p, nOld, cap, headsOut.p});
-        d2h(ctx, pack.data(), headsOut.p, words * 4); sync(ctx);
-        nh = pack[0];
-        if (nh <= cap) break;
-        cap = nh;
-      }
-      std::vector<std::array<u8, 32>> hs; std::vector<u32> hi;
-      for (u32 i = 0; i < nOld; i++) if (!pack[1 + i]) { hs.push_back(heads[i]); hi.push_back(headIdx[i]); }
-      for (u32 k = 0; k < nh; k++) { const u32* e = pack.data() + 1 + nOld + 9 * (size_t)k; std::array<u8, 32> h; memcpy(h.data(), e, 32); hs.push_back(h); hi.push_back((u32)(numApplied + e[8])); }
-      std::vector<size_t> o(hs.size()); for (size_t i = 0; i < o.size(); i++) o[i] = i;
-      std::sort(o.begin(), o.end(), [&](size_t a, size_t b) { return hs[a] < hs[b]; });
-      headsNow.clear(); headIdxNow.clear(); for (size_t i : o) { headsNow.push_back(hs[i]); headIdxNow.push_back(hi[i]); }
-    }
-  } else {
-    headIdxNow = headIdx;
+}
+
+// ------------------------------------------------------------ 4. actors
+inline void Engine::internActors(ApplyCall& a) {
+  const size_t B = a.B; a.now = st; std::vector<std::string>& actors = a.now.actorIds;
+  authorSlot.ensure(ctx, B); newSlots.ensure(ctx, B + 1); u32 fresh = 0;
+  while (true) {   // grow the table until the distinct authors fit at load factor <= 1/2
+    dev_memset(ctx, flagWord.p, 0, 8);
+    foreach(ctx, B, ActorInternKernel{arena.p, hot.p, applied.p, appRank.p, actorSlots.p, (u64)actorCap - 1, authorSlot.p, flagWord.p + 1});
+    foreach(ctx, B, NewActorKernel{hot.p, applied.p, authorSlot.p, actorSlots.p, newSlots.p, flagWord.p});
+    u32 full = 0; readU32x2(flagWord.p, flagWord.p + 1, &fresh, &full);
+    if (!full && (actors.size() + fresh) * 2 <= actorCap) break;
+    actorCap *= 4; actorSlots.ensure(ctx, actorCap); rebuildActorTable();
   }
-  dbgMark("commit:heads-done");
-  std::vector<std::pair<u64, UnknownRow>> unknownNow; std::set<u32> unknownIdsNow;
-  if (numNew > 0 && hasUnknownColsCall) collectUnknownColumns(B, unknownNow, unknownIdsNow);   // rare: columns written by a future version (unknowncols.hpp)
-  // ------------------------------------------------------------ 8. commit (nothing above mutated persistent state)
+  if (fresh > 0) {
+    trace.mark("actors:interned");
+    // slot numbers, slot records and id bytes of the new actors in ONE round trip (gathered into a staging buffer)
+    static const u32 ACTOR_STAGE = 64;
+    hashTmp.ensure(ctx, (size_t)fresh * (4 + sizeof(ActorSlot) + ACTOR_STAGE) + 64);
+    u8* stageD = hashTmp.p; const size_t recsAt = ((size_t)fresh * 4 + 15) & ~(size_t)15, bytesAt = recsAt + (size_t)fresh * sizeof(ActorSlot), stageLen = bytesAt + (size_t)fresh * ACTOR_STAGE;
+    foreach(ctx, fresh, GatherNewActorsKernel{arena.p, actorSlots.p, newSlots.p, reinterpret_cast<u32*>(stageD), reinterpret_cast<ActorSlot*>(stageD + recsAt), stageD + bytesAt, ACTOR_STAGE});
+    std::vector<u8> stageH(stageLen); d2h(ctx, stageH.data(), stageD, stageLen); sync(ctx);
+    std::vector<u32> slotsH(fresh); memcpy(slotsH.data(), stageH.data(), (size_t)fresh * 4);
+    std::vector<ActorSlot> recs(fresh); memcpy(recs.data(), stageH.data() + recsAt, (size_t)fresh * sizeof(ActorSlot));
+    std::vector<u32> order(fresh); for (u32 i = 0; i < fresh; i++) order[i] = i;
+    std::sort(order.begin(), order.end(), [&](u32 x, u32 y) { return recs[x].first < recs[y].first; });
+    std::vector<u32> ids(fresh), nums(fresh); actors.reserve(actors.size() + fresh);   // async copies target the strings: no reallocation below
+    bool longIds = false;
+    for (u32 k = 0; k < fresh; k++) {
+      const ActorSlot& r = recs[order[k]]; ids[k] = slotsH[order[k]]; nums[k] = (u32)actors.size();
+      actors.emplace_back(r.repLen, '\0');
+      if (r.repLen <= ACTOR_STAGE) memcpy(&actors.back()[0], stageH.data() + bytesAt + (size_t)order[k] * ACTOR_STAGE, r.repLen);
+      else { d2h(ctx, &actors.back()[0], arena.p + r.repOff, r.repLen); longIds = true; }   // from the device copy: the host mirror may still be filling
+      a.now.actorRep.emplace_back(r.repOff, r.repLen);
+    }
+    if (longIds) sync(ctx);
+    if (actors.size() > 65535) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: more than 65535 actors in one document");
+    sortVals.ensure(ctx, 2 * fresh); h2d(ctx, sortVals.p, ids.data(), fresh * 4); h2d(ctx, sortVals.p + fresh, nums.data(), fresh * 4);
+    foreach(ctx, fresh, SetActorNumKernel{actorSlots.p, sortVals.p, sortVals.p + fresh});
+  }
+  const size_t A = actors.size(); a.now.clock.resize(A, 0);
+  {   // rank of every actor in hex-string order (== byte order of the raw ids; new.js:64-65, 1180, 1198)
+    std::vector<u32> order(A), rank(A); for (size_t i = 0; i < A; i++) order[i] = (u32)i;
+    std::sort(order.begin(), order.end(), [&](u32 x, u32 y) { return actors[x] < actors[y]; });
+    for (size_t i = 0; i < A; i++) rank[order[i]] = (u32)i;
+    actorRank.ensure(ctx, A + 1); h2d(ctx, actorRank.p, rank.data(), A * 4);
+  }
+  a.ord = Ord{actorRank.p, bits_for(A > 1 ? A - 1 : 1)};
+  trace.mark("actors:numbered");
+  amapBase.ensure(ctx, B + 1); rowSlot.ensure(ctx, B + 1);
+  foreach(ctx, B, MaskedCountKernel{nActors.p, applied.p, rowSlot.p});
+  scan_exclusive(ctx, scanTmp, rowSlot.p, amapBase.p, B);
+  amap.ensure(ctx, B + (a.cur - a.arenaLen0) / 2 + 2);   // author + one entry per other-actor table entry (>= 2 bytes each): bound instead of a round trip
+  foreach(ctx, B, ActorMapKernel{arena.p, hot.p, nActors.p, applied.p, appRank.p, actorSlots.p, (u64)actorCap - 1, amapBase.p, amap.p, errWord.p});
+  trace.mark("actors:mapped");
+}
+
+// ------------------------------------------------------------ 5. sequence numbers
+inline void Engine::checkSequence(ApplyCall& a) {
+  const size_t B = a.B, A = a.now.actorIds.size();
+  changeActor.ensure(ctx, B); actorCnt.ensure(ctx, A + 1); actorBaseD.ensure(ctx, A + 1); seqSlot.ensure(ctx, a.numNew + 1);
+  dev_memset(ctx, actorCnt.p, 0, (A + 1) * 4);
+  foreach(ctx, B, ChangeActorKernel{amapBase.p, amap.p, applied.p, changeActor.p, actorCnt.p});
+  if (const u64 ew = fetchErr()) throwActorError(ew, a.now.actorIds);
+  scan_exclusive(ctx, scanTmp, actorCnt.p, actorBaseD.p, A);
+  DBuf<u64>& clockDev = pairKey;   // scratch reuse before the succ phase
+  clockDev.ensure(ctx, A + 1); h2d(ctx, clockDev.p, a.now.clock.data(), A * 8);
+  dev_memset(ctx, seqSlot.p, 0xff, (a.numNew + 1) * 4); dev_memset(ctx, flagWord.p, 0, 4);
+  foreach(ctx, B, SeqScatterKernel{hot.p, applied.p, changeActor.p, appRank.p, actorBaseD.p, actorCnt.p, clockDev.p, seqSlot.p, flagWord.p});
+  foreach(ctx, B, SeqMonoKernel{hot.p, applied.p, changeActor.p, actorBaseD.p, actorCnt.p, clockDev.p, seqSlot.p, flagWord.p});
+  std::vector<u32> actorCntH(A); d2h(ctx, actorCntH.data(), actorCnt.p, A * 4);
+  if (readU32(flagWord.p)) throwSequenceError(a);
+  for (size_t x = 0; x < A; x++) a.now.clock[x] += actorCntH[x];
+  trace.mark("seq:checked");
+}
+// an unknown actor is named like the reference does (new.js:1446): the actor table of the change the kernel reported is read again
+inline void Engine::throwActorError(u64 ew, const std::vector<std::string>& actors) {
+  if ((ew & 0xff) != KE_UNKNOWN_ACTOR) throwKernelError(ew);
+  const size_t b = (size_t)(ew >> 8); ChangeHot m0; u32 na0 = 1; d2h(ctx, &m0, hot.p + b, sizeof(ChangeHot)); d2h(ctx, &na0, nActors.p + b, 4); sync(ctx);
+  std::vector<u8> bytes(m0.len); d2h(ctx, bytes.data(), arena.p + m0.off, m0.len); sync(ctx);
+  ByteReader r(bytes.data(), m0.otherOff - m0.off, m0.len); std::string culprit;
+  for (u32 k = 0; k < na0 && !r.err; k++) {
+    u32 off, len; if (k == 0) { off = m0.actorOff - m0.off; len = m0.actorLen; } else { len = (u32)r.uleb(); off = r.pos; r.skip(len); }
+    if (r.err) break;
+    const std::string id((const char*)bytes.data() + off, len);
+    if (std::find(actors.begin(), actors.end(), id) == actors.end()) { culprit = id; break; }
+  }
+  if (!culprit.empty()) throw Error(AMG_ERR_RANGE, "actorId " + hex_of((const u8*)culprit.data(), culprit.size()) + " is not known to document");
+  throwKernelError(ew);
+}
+// the sequence check failed: replay it in application order on the host to produce the reference's message
+inline void Engine::throwSequenceError(ApplyCall& a) {
+  const size_t B = a.B; const std::vector<std::string>& actors = a.now.actorIds;
+  std::vector<ChangeHot> mh(B); std::vector<u32> ca(B), ar(B); std::vector<u8> ap(B);
+  d2h(ctx, mh.data(), hot.p, B * sizeof(ChangeHot)); d2h(ctx, ca.data(), changeActor.p, B * 4); d2h(ctx, ar.data(), appRank.p, B * 4); d2h(ctx, ap.data(), applied.p, B); sync(ctx);
+  std::vector<u32> byRank(a.numNew, 0); for (size_t b = 0; b < B; b++) if (ap[b]) byRank[ar[b]] = (u32)b;
+  std::vector<u64> clk = a.now.clock;
+  for (size_t k = 0; k < a.numNew; k++) {
+    const u32 b = byRank[k]; const u64 expected = clk[ca[b]] + 1; const std::string actorHex = hex_of((const u8*)actors[ca[b]].data(), actors[ca[b]].size());
+    if (mh[b].seq < expected) throw Error(AMG_ERR_RANGE, "Reuse of sequence number " + std::to_string(mh[b].seq) + " for actor " + actorHex);
+    if (mh[b].seq > expected) throw Error(AMG_ERR_RANGE, "Skipped sequence number " + std::to_string(expected) + " for actor " + actorHex);
+    clk[ca[b]] = mh[b].seq;
+  }
+  throw Error(AMG_ERR_INTERNAL, "amgpu: sequence check disagreement");
+}
+
+// ------------------------------------------------------------ 6. ops of the applied changes
+// The rows were decoded with the headers (staging phase), in batch order. When every change of the batch is applied the
+// op / pred ranges of the changes are the raw ones; otherwise they are the scans over the applied changes only.
+inline void Engine::finalizeOps(ApplyCall& a) {
+  const size_t B = a.B; const u32* decTot = a.decTot;
+  timeBase.ensure(ctx, B + 1);
+  opBase.ensure(ctx, B + 1); predBase.ensure(ctx, B + 1);
+  // first op / pred of every applied change in batch order (the raw rows themselves lie in tile arrival order, rawBase)
+  if (a.numNew == B) { scan_exclusive(ctx, scanTmp, nOps.p, opBase.p, B); scan_exclusive(ctx, scanTmp, nPreds.p, predBase.p, B); a.M = decTot[0]; a.P = decTot[1]; }
+  else {
+    foreach(ctx, B, MaskedCountKernel{nOps.p, applied.p, rowSlot.p}); scan_exclusive(ctx, scanTmp, rowSlot.p, opBase.p, B);
+    foreach(ctx, B, MaskedCountKernel{nPreds.p, applied.p, rowSlot.p}); scan_exclusive(ctx, scanTmp, rowSlot.p, predBase.p, B);
+    u32 m32 = 0, p32 = 0; void* dst[2] = {&m32, &p32}; readWords({{opBase.p + B, 4}, {predBase.p + B, 4}}, dst); a.M = m32; a.P = p32;
+  }
+  if (decTot[0] >= 0x7fffffffu || decTot[1] >= 0x7fffffffu) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: more than 2^31 operations in one call");
+  trace.mark("decode:counts");
+  if (!a.inOrder) {
+    perm.ensure(ctx, B + 1); dev_memset(ctx, perm.p, 0, (B + 1) * 4);
+    foreach(ctx, B, OpsInOrderKernel{nOps.p, applied.p, appRank.p, perm.p});
+    scan_exclusive(ctx, scanTmp, perm.p, perm.p, a.numNew);
+  }
+  foreach(ctx, B, TimeBaseKernel{perm.p, applied.p, appRank.p, opBase.p, a.inOrder ? 1 : 0, timeBase.p});
+  DBuf<u64>& maxOpD = pairSucc; maxOpD.ensure(ctx, 1); h2d(ctx, maxOpD.p, &a.now.maxOp, 8);
+  foreach(ctx, B, MaxOpKernel{hot.p, nOps.p, applied.p, decErr.p, maxOpD.p, errWord.p});
+  d2h(ctx, &a.now.maxOp, maxOpD.p, 8);
+  RawRows raw = rawRows();
+  lastNumLarge = 0;
+  if (decTot[3] & 1u) {   // changes with more than SMALL_CHANGE_OPS ops: (column, change)-parallel expansion into their reserved rows
+    largeFlag.ensure(ctx, B + 1); largeSlot.ensure(ctx, B + 2); largeList.ensure(ctx, B + 1);
+    foreach(ctx, B, LargeFlagKernel{nOps.p, applied.p, largeFlag.p});
+    scan_exclusive(ctx, scanTmp, largeFlag.p, largeSlot.p, B);
+    lastNumLarge = readU32(largeSlot.p + B);
+    if (lastNumLarge > 0) {
+      foreach(ctx, B, CompactKernel{largeFlag.p, largeSlot.p, largeList.p});
+      // bulk changes (thousands of ops in one change): their columns are expanded in parallel by the token / record
+      // decoders of doccols.cuh, column by column; whatever those decline (non-canonical streams, columns that do not hold
+      // exactly the op count) and all other large changes go through DecodeColumnKernel (one thread per column)
+      if (lastNumLarge <= 8) decodeHugeChanges(raw, lastNumLarge);
+      foreach(ctx, (size_t)NCOLS * lastNumLarge, DecodeColumnKernel{arena.p, largeList.p, lastNumLarge, hot.p, nOps.p, nPreds.p, rawBase.p, rawPredBase.p, applied.p, raw, errWord.p, hugeDone.p});
+    }
+  }
+  const size_t M = a.M;
+  for (DBuf<u64>* b : {&o_id, &o_obj, &o_key}) b->ensure(ctx, M + 1);
+  o_predId.ensure(ctx, a.P + 1);
+  for (DBuf<u32>* b : {&o_keyStrOff, &o_keyStrLen, &o_flags, &o_valLen, &o_valOff, &o_predOff, &o_predNum, &o_change, &o_time}) b->ensure(ctx, M + 1);
+  a.ops = OpRows{o_id.p, o_obj.p, o_key.p, o_keyStrOff.p, o_keyStrLen.p, o_flags.p, o_valLen.p, o_valOff.p, o_predOff.p, o_predNum.p, o_change.p, o_time.p, o_predId.p};
+  foreach(ctx, M, FinalizeOpsKernel{B, hot.p, nActors.p, opBase.p, predBase.p, rawBase.p, rawPredBase.p, timeBase.p, amapBase.p, amap.p, applied.p, raw, a.ops, errWord.p});
+  checkErr();
+  trace.mark("decode:finalized");
+}
+
+// ------------------------------------------------------------ 7. op set: the new rows, RGA list order, document order, succ lists
+inline void Engine::orderOpSet(ApplyCall& a) {
+  const size_t M = a.M; const Ord ord = a.ord;
+  if (a.now.maxOp >= (1ULL << 40)) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: op counters above 2^40");
+  const int ordBits = bits_for(a.now.maxOp) + ord.rb;
+  isRow.ensure(ctx, M + 1); rowSlot.ensure(ctx, M + 1); rowOfOp.ensure(ctx, M + 1);
+  foreach(ctx, M, RowFlagKernel{o_flags.p, isRow.p}); scan_exclusive(ctx, scanTmp, isRow.p, rowSlot.p, M);
+  const size_t R = readU32(rowSlot.p + M); const size_t N = a.N = numRows + R;
+  if (N >= (1u << 29)) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: more than 2^29 document rows");
+  doc.ensure(ctx, N + 1, numRows);
+  const DocRows w = a.w = doc.view();
+  foreach(ctx, M, AppendRowsKernel{a.ops, isRow.p, rowSlot.p, numRows, w, rowOfOp.p});
+  const size_t icap = pow2_at_least(2 * N + 2); idKeys.ensure(ctx, icap); idVals.ensure(ctx, icap); dev_memset(ctx, idKeys.p, 0, icap * 8);
+  a.idt = IdTable{idKeys.p, idVals.p, (u64)icap - 1};
+  foreach(ctx, N, IdInsertKernel{w.id, a.idt, errWord.p});
+  objRow.ensure(ctx, N + 1); elemRow.ensure(ctx, N + 1); parentRow.ensure(ctx, N + 1);
+  foreach(ctx, N, ResolveRowsKernel{w, a.idt, ord, numRows, objRow.p, elemRow.p, parentRow.p, errWord.p});
+  checkErr();
+  trace.mark("opset:resolved");
+  // map keys: intern, verify, rank distinct keys with an LSD string sort
+  const size_t kcap = pow2_at_least(2 * N + 2); keySlots.ensure(ctx, kcap); keySlot.ensure(ctx, N + 1); repList.ensure(ctx, N + 1); repCount.ensure(ctx, 4);
+  foreach(ctx, kcap, KeySlotInitKernel{keySlots.p});
+  foreach(ctx, N, KeyInternKernel{arena.p, w, keySlots.p, (u64)kcap - 1, keySlot.p});
+  dev_memset(ctx, repCount.p, 0, 16);
+  foreach(ctx, N, KeyVerifyKernel{arena.p, w, keySlots.p, keySlot.p, repList.p, repCount.p, errWord.p});
+  u32 rc[2]; readU32x2(repCount.p, repCount.p + 1, &rc[0], &rc[1]);
+  const size_t D = rc[0]; const u32 maxKeyLen = rc[1];
+  trace.mark("opset:keys-interned");
+  if (D > 0) {
+    sortKeys.ensure(ctx, D); sortVals.ensure(ctx, D);
+    d2d(ctx, sortVals.p, repList.p, D * 4);
+    const int chunks = (int)((maxKeyLen + 6) / 7);
+    for (int ch = std::max(chunks, 1) - 1; ch >= 0; ch--) {
+      foreach(ctx, D, KeyChunkKernel{arena.p, w, sortVals.p, (u32)ch * 7, sortKeys.p});
+      sortPairs(sortKeys, sortVals, D, 64);
+    }
+    foreach(ctx, D, KeyRankKernel{sortVals.p, keySlot.p, keySlots.p});
+  }
+  // RGA order of every list: sibling sort, Euler tour, pointer jumping
+  listPos.ensure(ctx, N + 1); insItems.ensure(ctx, N + 1); emit.ensure(ctx, N + 1); slot.ensure(ctx, N + 2);
+  foreach(ctx, N, InsertFlagKernel{w, emit.p}); scan_exclusive(ctx, scanTmp, emit.p, slot.p, N);
+  const size_t I = readU32(slot.p + N);
+  trace.mark("opset:inserts-counted");
+  if (I > 0) {
+    const int parentBits = bits_for(N) + 1;
+    if (ordBits + parentBits > 64) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: opId range x document size exceeds the 64-bit sibling sort key");
+    foreach(ctx, N, CompactKernel{emit.p, slot.p, insItems.p});
+    sortKeys.ensure(ctx, I); sortVals.ensure(ctx, I);
+    foreach(ctx, I, SiblingKeyKernel{w, insItems.p, parentRow.p, objRow.p, ord, ordBits, sortKeys.p, errWord.p});
+    d2d(ctx, sortVals.p, insItems.p, I * 4);
+    sortPairs(sortKeys, sortVals, I, ordBits + parentBits);
+    checkErr();
+    itemIdx.ensure(ctx, N + 1); objSlot.ensure(ctx, N + 2);
+    foreach(ctx, I, ItemIndexKernel{sortVals.p, itemIdx.p});
+    foreach(ctx, N, ListObjFlagKernel{w, emit.p}); scan_exclusive(ctx, scanTmp, emit.p, objSlot.p, N);
+    const size_t Lo = readU32(objSlot.p + N);
+    const size_t S = 2 * I + 2 * Lo; eNext.ensure(ctx, S + 1); eRank.ensure(ctx, S + 1); ePacked.ensure(ctx, S + 1); ePacked2.ensure(ctx, S + 1);
+    foreach(ctx, S, EulerInitKernel{eNext.p, eRank.p});
+    foreach(ctx, I, EulerLinkKernel{sortKeys.p, ordBits, itemIdx.p, objSlot.p, eNext.p, eRank.p, I});
+    foreach(ctx, S, ListRankPackKernel{eNext.p, eRank.p, ePacked.p});
+    const int rounds = bits_for(S);
+    for (int k = 0; k < rounds; k++) {
+      foreach(ctx, S, ListRankPackedKernel{ePacked.p, ePacked2.p});
+      ePacked.swap(ePacked2);
+    }
+    foreach(ctx, S, ListRankUnpackKernel{ePacked.p, eRank.p});
+    foreach(ctx, N, ListPosKernel{eRank.p, elemRow.p, objRow.p, itemIdx.p, objSlot.p, (u32)I, listPos.p});
+  } else dev_memset(ctx, listPos.p, 0, (N + 1) * 4);
+  checkErr();
+  trace.mark("opset:list-ranked");
+  // document order: stable LSD over (object, key rank | list position, opId within the key / element)
+  perm.ensure(ctx, N + 1); pos.ensure(ctx, N + 1); sortKeys.ensure(ctx, N);
+  foreach(ctx, N, IotaKernel{perm.p});
+  const int fieldBits[3] = {ordBits + 1, bits_for(N), ordBits + 1};
+  for (int f = 0; f < 3; f++) {
+    foreach(ctx, N, DocKeyKernel{f, w, perm.p, listPos.p, keySlots.p, keySlot.p, ord, sortKeys.p});
+    sortPairs(sortKeys, perm, N, fieldBits[f]);
+  }
+  foreach(ctx, N, InversePermKernel{perm.p, pos.p});
+  trace.mark("opset:doc-ordered(enqueued)");
+  // succ lists of the new document (old pairs re-keyed + the batch's preds), the checks on what the preds refer to, and the
+  // rows gathered into document order
+  const size_t numPairs = a.numPairs = numSucc + a.P;
+  pairKey.ensure(ctx, numPairs + 1); pairSucc.ensure(ctx, numPairs + 1); pairIdx.ensure(ctx, numPairs + 1); pairPos.ensure(ctx, numPairs + 1); pairTime.ensure(ctx, numPairs + 1);
+  foreach(ctx, M, DelElemCheckKernel{a.ops, a.idt, w, errWord.p});
+  checkErr();
+  foreach(ctx, numRows, OldPairsKernel{succOff.p, succ.p, pos.p, ord, pairKey.p, pairIdx.p, pairSucc.p, pairPos.p, pairTime.p});
+  foreach(ctx, M, PredPairsKernel{a.ops, a.idt, pos.p, rowOfOp.p, w, elemRow.p, keySlot.p, ord, pairKey.p, pairIdx.p, pairSucc.p, pairPos.p, pairTime.p, numSucc, errWord.p});
+  foreach(ctx, M, DelKeyCheckKernel{arena.p, a.ops, a.idt, w, errWord.p});
+  foreach(ctx, M, IncCheckKernel{a.ops, a.idt, w, arena.p, errWord.p});
+  if (const u64 ew = fetchErr()) throwOpError(ew, a.now.actorIds);
+  sortPairs(pairKey, pairIdx, numPairs, ordBits);
+  foreach(ctx, numPairs, PairPosKeyKernel{pairPos.p, pairIdx.p, pairKey.p});
+  sortPairs(pairKey, pairIdx, numPairs, bits_for(N));
+  succCnt.ensure(ctx, N + 2); newSuccCnt.ensure(ctx, N + 2); newSuccOff.ensure(ctx, N + 2); firstNewSucc.ensure(ctx, N + 2); newSucc.ensure(ctx, numPairs + 1);
+  dev_memset(ctx, succCnt.p, 0, (N + 2) * 4); dev_memset(ctx, newSuccCnt.p, 0, (N + 2) * 4); dev_memset(ctx, firstNewSucc.p, 0xff, (N + 2) * 4);
+  foreach(ctx, numPairs, CountSuccKernel{pairPos.p, succCnt.p});
+  foreach(ctx, numPairs, NewSuccFlagKernel{pairPos.p, pairTime.p, newSuccCnt.p});
+  foreach(ctx, numPairs, FirstSuccTimeKernel{pairPos.p, pairTime.p, firstNewSucc.p});
+  scan_exclusive(ctx, scanTmp, succCnt.p, newSuccOff.p, N);
+  newSuccTime.ensure(ctx, numPairs + 1);
+  foreach(ctx, numPairs, WriteSuccKernel{pairIdx.p, pairSucc.p, newSucc.p, pairTime.p, newSuccTime.p});
+  sorted.ensure(ctx, N + 1);
+  foreach(ctx, N, GatherRowsKernel{w, sorted.view(), perm.p});
+  trace.mark("opset:succ+gather(enqueued)");
+}
+
+// names the op of a missing pred or of an increment without a counter like the reference does
+inline void Engine::throwOpError(u64 ew, const std::vector<std::string>& actors) {
+  if ((ew & 0xff) == KE_PRED_MISSING) { u64 pid = 0; d2h(ctx, &pid, o_predId.p + (ew >> 8), 8); sync(ctx); throw Error(AMG_ERR_RANGE, "no matching operation for pred: " + opIdText(pid, actors)); }
+  if ((ew & 0xff) == KE_UNKNOWN_COUNTER) { u64 oid = 0; d2h(ctx, &oid, o_id.p + (ew >> 8), 8); sync(ctx); throw Error(AMG_ERR_RANGE, "increment operation " + opIdText(oid, actors) + " for unknown counter"); }
+  throwKernelError(ew);
+}
+
+// ------------------------------------------------------------ 9. heads
+inline void Engine::computeHeads(ApplyCall& a) {
+  const size_t B = a.B;
+  trace.mark("commit:begin");
+  DBuf<u32>& isDep = groupLinked; isDep.ensure(ctx, a.G + 1); dev_memset(ctx, isDep.p, 0, (a.G + 1) * 4);   // scratch reuse: the patch is done with it
+  foreach(ctx, B, MarkDepsKernel{applied.p, nDeps.p, depBase.p, depIdx.p, isDep.p});
+  emit.ensure(ctx, B + 1); slot.ensure(ctx, B + 2); objStart.ensure(ctx, B + 1);
+  foreach(ctx, B, HeadFlag2Kernel{applied.p, isDep.p, numApplied, emit.p});
+  scan_exclusive(ctx, scanTmp, emit.p, slot.p, B);
+  foreach(ctx, B, CompactKernel{emit.p, slot.p, objStart.p});
+  // one round trip for the whole answer (HeadsPackKernel); a second one only if the call leaves more heads than the block holds
+  const u32 nOld = (u32)st.headIdx.size(); u32 cap = 64, nh = 0; std::vector<u32> pack;
+  headsPack.ensure(ctx, nOld + 1);
+  if (nOld) h2d(ctx, headsPack.p, st.headIdx.data(), nOld * 4);
+  for (;;) {
+    const size_t words = 1 + (size_t)nOld + 9 * (size_t)cap;
+    headsOut.ensure(ctx, words + 1); pack.resize(words);
+    foreach(ctx, std::max<size_t>(std::max<size_t>(nOld, cap), 1), HeadsPackKernel{slot.p + B, objStart.p, hashes.p + numApplied * 32, appRank.p, isDep.p, headsPack.p, nOld, cap, headsOut.p});
+    d2h(ctx, pack.data(), headsOut.p, words * 4); sync(ctx);
+    nh = pack[0];
+    if (nh <= cap) break;
+    cap = nh;
+  }
+  std::vector<std::array<u8, 32>> hs; std::vector<u32> hi;
+  for (u32 i = 0; i < nOld; i++) if (!pack[1 + i]) { hs.push_back(st.heads[i]); hi.push_back(st.headIdx[i]); }
+  for (u32 k = 0; k < nh; k++) { const u32* e = pack.data() + 1 + nOld + 9 * (size_t)k; std::array<u8, 32> h; memcpy(h.data(), e, 32); hs.push_back(h); hi.push_back((u32)(numApplied + e[8])); }
+  std::vector<size_t> o(hs.size()); for (size_t i = 0; i < o.size(); i++) o[i] = i;
+  std::sort(o.begin(), o.end(), [&](size_t x, size_t y) { return hs[x] < hs[y]; });
+  a.now.heads.clear(); a.now.headIdx.clear(); for (size_t i : o) { a.now.heads.push_back(hs[i]); a.now.headIdx.push_back(hi[i]); }
+}
+
+// ------------------------------------------------------------ 10. commit (nothing before this mutated persistent state)
+inline void Engine::commit(ApplyCall& a) {
+  const size_t B = a.B, numNew = a.numNew;
+  trace.mark("commit:heads-done");
+  if (numNew > 0 && (a.decTot[3] & 2u)) collectUnknownColumns(B, a.unknownRows, a.unknownIds);   // rare: columns written by a future version (unknowncols.hpp)
   sync(ctx);
-  dbgMark("commit:synced");
-  needBatch(); finishInflate();
+  trace.mark("commit:synced");
+  a.needBatch(); a.finishInflate(*this);
   if (numNew > 0) {
-    if (!(inOrder && numNew == B)) {   // hashes of applied changes must be contiguous in application order
+    if (!(a.inOrder && numNew == B)) {   // hashes of applied changes must be contiguous in application order
       DBuf<u8>& tmp = hashTmp; tmp.ensure(ctx, numNew * 32 + 64);
       foreach(ctx, B, HashGatherKernel{hashes.p + numApplied * 32, applied.p, appRank.p, tmp.p});
       d2d(ctx, hashes.p + numApplied * 32, tmp.p, numNew * 32);
     }
-    if (appliedH.empty()) {   // all applied, in order
+    if (a.appliedH.empty()) {   // all applied, in order
       const u32 base0 = (u32)changes.size();
-      if (!batchOriginal.empty()) for (size_t b = 0; b < B; b++) { const HostChange o = originalOf(b); if (o.len) deflatedOriginal.push_back({base0 + (u32)b, o}); }
-      else { deflatedOriginal.reserve(deflatedOriginal.size() + deflIdx.size()); for (size_t k = 0; k < deflIdx.size(); k++) deflatedOriginal.push_back({base0 + deflIdx[k], inflOrig[k]}); }
-      if (changes.empty()) changes.swap(batch); else changes.insert(changes.end(), batch.begin(), batch.end());
-    }
-    else {
+      if (!a.batchOriginal.empty()) for (size_t b = 0; b < B; b++) { const HostChange o = a.originalOf(b); if (o.len) deflatedOriginal.push_back({base0 + (u32)b, o}); }
+      else { deflatedOriginal.reserve(deflatedOriginal.size() + a.deflIdx.size()); for (size_t k = 0; k < a.deflIdx.size(); k++) deflatedOriginal.push_back({base0 + a.deflIdx[k], a.inflOrig[k]}); }
+      if (changes.empty()) changes.swap(batchStore); else changes.insert(changes.end(), batchStore.begin(), batchStore.end());
+    } else {
       std::vector<u32> byRank(numNew);
-      if (appliedH.empty()) for (size_t b = 0; b < B; b++) byRank[b] = (u32)b; else for (size_t b = 0; b < B; b++) if (appliedH[b]) byRank[appRankH[b]] = (u32)b;
+      for (size_t b = 0; b < B; b++) if (a.appliedH[b]) byRank[a.appRankH[b]] = (u32)b;
       for (size_t k = 0; k < numNew; k++) {
         const u32 b = byRank[k];
-        { const HostChange o = originalOf(b); if (o.len) deflatedOriginal.push_back({(u32)changes.size(), o}); }
-        changes.push_back(batch[b]);
+        { const HostChange o = a.originalOf(b); if (o.len) deflatedOriginal.push_back({(u32)changes.size(), o}); }
+        changes.push_back(batchStore[b]);
       }
     }
-    dbgMark("commit:changes-recorded");
-    doc.swap(sorted); numRows = N;
-    std::swap(succOff.p, newSuccOff.p); std::swap(succOff.cap, newSuccOff.cap); std::swap(succ.p, newSucc.p); std::swap(succ.cap, newSucc.cap); numSucc = numPairs;
-    fill32(doc.time.p, 0, N);
-    for (auto& kv : unknownNow) unknownCols.byOp[kv.first] = std::move(kv.second);
-    unknownCols.colIds.insert(unknownIdsNow.begin(), unknownIdsNow.end());
-    loadedDoc.clear(); numApplied += numNew; actorRep = actorRepNow; actorIds = actorsNow; clock = clockNow; maxOp = maxOpNow; heads = headsNow; headIdx = headIdxNow;
-    dbgMark("commit:state-swapped");
+    trace.mark("commit:changes-recorded");
+    doc.swap(sorted); numRows = a.N;
+    succOff.swap(newSuccOff); succ.swap(newSucc); numSucc = a.numPairs;
+    fill32(doc.time.p, 0, a.N);
+    for (auto& kv : a.unknownRows) unknownCols.byOp[kv.first] = std::move(kv.second);
+    unknownCols.colIds.insert(a.unknownIds.begin(), a.unknownIds.end());
+    loadedDoc.clear(); numApplied += numNew; st = std::move(a.now);
+    trace.mark("commit:state-swapped");
     rebuildActorTable();   // slots of actors registered in this call become permanent (first = 0)
-    dbgMark("commit:actors-rebuilt");
+    trace.mark("commit:actors-rebuilt");
   }
-  arenaLen = cur; queue = newQueue; queueOriginal = newQueueOriginal; rb.armed = false;
-  side_join(ctx); sync(ctx);
-  timer.mark(); hostMark(); nvtx.next(nullptr);
-  fillPatchHeader(out);
-  if (isLocal && n == 1) {   // new.js:1874-1877
-    std::vector<ChangeHot> m0(1); d2h(ctx, m0.data(), hot.p, sizeof(ChangeHot)); sync(ctx);
-    out.hasActorSeq = true; out.actor.assign(m0[0].actorLen, '\0'); out.seq = m0[0].seq;
-    if (m0[0].actorLen) { d2h(ctx, &out.actor[0], arena.p + m0[0].actorOff, m0[0].actorLen); sync(ctx); }
-  }
-  dbgMark("commit:end");
-  lastB = B; lastM = M; lastP = P; lastBytes = cur - arenaLen0; for (auto& c : queue) lastBytes += 0 * c.len;
-  finishPatch(out); dbgMark("call:patch-finished");
-  timer.collect(lastPhaseMs, 12); dbgMark("call:timers-collected");
+  arenaLen = a.cur; queue = a.newQueue; queueOriginal = a.newQueueOriginal;
 }
 
-}  // namespace amg
 
-namespace amg {
-
-// Patch emission over a document table `d` in document order (N rows). wholeDoc = getPatch semantics
+// Patch emission over a document table `in.d` in document order (N rows). wholeDoc = getPatch semantics
 // (new.js:1604-1635), otherwise incremental semantics for the batch `ops` (new.js:884-1040, 1461-1528).
-// Uses succCnt (per position) and, in incremental mode, newSuccCnt / firstNewSucc / objPos.
-inline void Engine::buildPatch(DocRows d, size_t N, bool wholeDoc, const OpRows* ops, size_t numOps, const IdTable* idt, const u32* rowOfOpD, const u32* posD,
-                               const std::vector<std::string>& actorsNow, PatchOut& out, const u32* succOffD, const u64* succD) {
+inline void Engine::buildPatch(const PatchInputs& in, PatchOut& out) {
+  const DocRows d = in.d; const size_t N = in.N, numOps = in.numOps; const bool wholeDoc = in.wholeDoc; const OpRows* ops = in.ops;
+  const u32* succCntD = in.succCnt;
   out.numProps = out.numEdits = 0; out.bigEnd = 0;
   if (N == 0) return;
   // groups (map key / list element) and their visibility
@@ -798,11 +764,9 @@ inline void Engine::buildPatch(DocRows d, size_t N, bool wholeDoc, const OpRows*
   u32 numGroups32 = 0, numObjs32 = 0; readU32x2(headScan.p + N, objIdx.p + N, &numGroups32, &numObjs32);
   const size_t numGroups = numGroups32, numObjs = numObjs32;
   groupRows.ensure(ctx, numGroups + 1); groupVisible.ensure(ctx, numGroups + 1); groupFirst.ensure(ctx, numGroups + 1); groupTouched.ensure(ctx, numGroups + 1);
-  DBuf<u32>& groupLinkedB = linkDone;   // linkDone doubles as per-group linked flags storage below (separate buffers)
-  (void)groupLinkedB;
   dev_memset(ctx, groupRows.p, 0, (numGroups + 1) * 4); dev_memset(ctx, groupVisible.p, 0, (numGroups + 1) * 4); dev_memset(ctx, groupTouched.p, 0, (numGroups + 1) * 4);
   groupHasChild.ensure(ctx, numGroups + 1); dev_memset(ctx, groupHasChild.p, 0, (numGroups + 1) * 4);
-  foreach(ctx, N, GroupStatsKernel{headScan.p, head.p, succCnt.p, d, groupOf.p, groupRows.p, groupVisible.p, groupFirst.p, errWord.p, 0, groupHasChild.p});
+  foreach(ctx, N, GroupStatsKernel{headScan.p, head.p, succCntD, d, groupOf.p, groupRows.p, groupVisible.p, groupFirst.p, errWord.p, 0, groupHasChild.p});
   // objects in document order
   objStart.ensure(ctx, numObjs + 2);
   foreach(ctx, N, ObjStartKernel{isObjHead.p, objIdx.p, objStart.p, N});
@@ -810,12 +774,11 @@ inline void Engine::buildPatch(DocRows d, size_t N, bool wholeDoc, const OpRows*
   emit.ensure(ctx, N + 1); marker.ensure(ctx, N + 1); slot.ensure(ctx, N + 2);
   groupLinked.ensure(ctx, std::max(numGroups, numApplied + 1) + 2);
   dev_memset(ctx, groupLinked.p, 0, (numGroups + 1) * 4);
-  Ord ordNow{actorRank.p, bits_for(actorsNow.size() > 1 ? actorsNow.size() - 1 : 1)};
-  ListCtx lctx{d, succCnt.p, newSuccCnt.p, firstNewSucc.p, groupOf.p, groupFirst.p, groupRows.p, arena.p, succOffD, succD, newSuccTime.p};
-  MapGroupCtx mg{arena.p, ops ? *ops : OpRows{}, opAt.p, numOps, pass.p};
+  ListCtx lctx{d, succCntD, in.newSuccCnt, in.firstNewSucc, groupOf.p, groupFirst.p, groupRows.p, arena.p, in.succOff, in.succ, in.newSuccTime};
+  MapGroupCtx mg{arena.p, ops ? *ops : OpRows{}, opAt.p, numOps, in.pass};
   bool anyListLink = false;
   auto listGroups = [&](int pass) {
-    return ListGroupKernel{pass, mg, opGroupHead.p, *idt, rowOfOpD, posD, lctx, gCount.p, gElem.p, gT1.p, gQOrd.p, nQ.p, elemHasRecs.p, elemMinT.p,
+    return ListGroupKernel{pass, mg, opGroupHead.p, *in.idt, in.rowOfOp, in.pos, lctx, gCount.p, gElem.p, gT1.p, gQOrd.p, nQ.p, elemHasRecs.p, elemMinT.p,
                            itemBase.p, objIdx.p, objStart.p, items.p, domTw.p, domW.p, oldVisScan.p, runHeadFlag.p, runScan.p, runStart.p, gBase.p, qIndex.p, editOut.p, editElem.p, editObjKey.p, editElemPos.p, editRowPos.p, errWord.p};
   };
   if (!wholeDoc) {
@@ -840,10 +803,10 @@ inline void Engine::buildPatch(DocRows d, size_t N, bool wholeDoc, const OpRows*
     }
     objTouchedAt.ensure(ctx, N + 1); linkDone.ensure(ctx, N + 1);
     dev_memset(ctx, objTouchedAt.p, 0xff, (N + 1) * 4); dev_memset(ctx, linkDone.p, 0xff, (N + 1) * 4); dev_memset(ctx, flagWord.p, 0, 16);
-    foreach(ctx, N, TouchKernel{d, groupOf.p, firstNewSucc.p, groupTouched.p, objTouchedAt.p, objPos.p, flagWord.p + 2});
+    foreach(ctx, N, TouchKernel{d, groupOf.p, in.firstNewSucc, groupTouched.p, objTouchedAt.p, in.objPos, flagWord.p + 2});
     u32 linkChanged = 1, anyLink32 = 0;
     for (int iter = 0; iter < 1000 && linkChanged; iter++) {   // three sweeps per host round trip (object nesting is shallow)
-      LinkKernel lk{d, groupOf.p, groupHasChild.p, groupFirst.p, objPos.p, groupLinked.p, objTouchedAt.p, flagWord.p + 2, linkDone.p, flagWord.p, listLinkTime.p, flagWord.p + 3};
+      LinkKernel lk{d, groupOf.p, groupHasChild.p, groupFirst.p, in.objPos, groupLinked.p, objTouchedAt.p, flagWord.p + 2, linkDone.p, flagWord.p, listLinkTime.p, flagWord.p + 3};
       foreach(ctx, N, lk); foreach(ctx, N, lk);
       dev_memset(ctx, flagWord.p, 0, 4);
       foreach(ctx, N, lk);
@@ -859,26 +822,25 @@ inline void Engine::buildPatch(DocRows d, size_t N, bool wholeDoc, const OpRows*
   if (!wholeDoc && numOps > 0) {
     dev_memset(ctx, memberFinal.p, 0, (N + 1) * 4); dev_memset(ctx, gFailed.p, 0, (numGroups + 1) * 4);
     for (int pass = 0; pass < 2; pass++)
-      foreach(ctx, numOps, GroupFinalKernel{pass, mg, opGroupHead.p, *idt, rowOfOpD, posD, groupOf.p, workView, ordNow, finalTime.p, gBound.p, gFailed.p, memberFinal.p});
+      foreach(ctx, numOps, GroupFinalKernel{pass, mg, opGroupHead.p, *in.idt, in.rowOfOp, in.pos, groupOf.p, in.unsorted, in.ord, finalTime.p, gBound.p, gFailed.p, memberFinal.p});
   }
   counterLast.ensure(ctx, N + 1); counterTotal.ensure(ctx, N + 1); counterOwner.ensure(ctx, N + 1); dev_memset(ctx, counterOwner.p, 0xff, (N + 1) * 4);
-  foreach(ctx, N, CounterKernel{arena.p, d, succOffD, succD, groupOf.p, groupFirst.p, groupRows.p, counterLast.p, counterTotal.p, counterOwner.p});
-  foreach(ctx, N, PropFlagKernel{d, groupOf.p, groupTouched.p, groupLinked.p, succCnt.p, wholeDoc ? 1 : 0, finalTime.p, gBound.p, gFailed.p, memberFinal.p, ordNow, emit.p, groupEmitted.p, counterLast.p});
+  foreach(ctx, N, CounterKernel{arena.p, d, in.succOff, in.succ, groupOf.p, groupFirst.p, groupRows.p, counterLast.p, counterTotal.p, counterOwner.p});
+  foreach(ctx, N, PropFlagKernel{d, groupOf.p, groupTouched.p, groupLinked.p, succCntD, wholeDoc ? 1 : 0, finalTime.p, gBound.p, gFailed.p, memberFinal.p, in.ord, emit.p, groupEmitted.p, counterLast.p});
   foreach(ctx, N, PropMarkerKernel{d, groupOf.p, groupTouched.p, head.p, groupEmitted.p, wholeDoc ? 1 : 0, emit.p, marker.p});
   scan_exclusive(ctx, scanTmp, emit.p, slot.p, N);
   const size_t numProps = readU32(slot.p + N);
   propOut.ensure(ctx, numProps + 1);
   foreach(ctx, N, PropEmitKernel{d, emit.p, marker.p, slot.p, propOut.p, counterLast.p, counterTotal.p});
-  if (curTimer) { curTimer->mark(); curHostMark(); }
-  NvtxPhases nvtxPatch; nvtxPatch.next("patch:list-edits");
+  trace.phase("patch:list-index");
   // ---- list edits
   size_t numEdits = 0; bool shipElem = true;
   if (wholeDoc) {
     elemVis.ensure(ctx, N + 1); elemVisScan.ensure(ctx, N + 2); rowEmit.ensure(ctx, N + 1); firstVis.ensure(ctx, numGroups + 1);
     rowClass.ensure(ctx, N + 1); firstBare.ensure(ctx, numGroups + 1);
     dev_memset(ctx, firstVis.p, 0xff, (numGroups + 1) * 4); dev_memset(ctx, firstBare.p, 0xff, (numGroups + 1) * 4);
-    foreach(ctx, N, ListRowClassKernel{d, groupOf.p, succCnt.p, counterOwner.p, rowClass.p, firstVis.p, firstBare.p});
-    foreach(ctx, N, ListVisFlagKernel{d, groupOf.p, groupVisible.p, head.p, succCnt.p, elemVis.p, rowEmit.p, rowClass.p, firstVis.p, firstBare.p});
+    foreach(ctx, N, ListRowClassKernel{d, groupOf.p, succCntD, counterOwner.p, rowClass.p, firstVis.p, firstBare.p});
+    foreach(ctx, N, ListVisFlagKernel{d, groupOf.p, groupVisible.p, head.p, succCntD, elemVis.p, rowEmit.p, rowClass.p, firstVis.p, firstBare.p});
     scan_exclusive(ctx, scanTmp, elemVis.p, elemVisScan.p, N);
     scan_exclusive(ctx, scanTmp, rowEmit.p, slot.p, N);
     numEdits = readU32(slot.p + N);
@@ -915,7 +877,7 @@ inline void Engine::buildPatch(DocRows d, size_t N, bool wholeDoc, const OpRows*
       for (int bit = tbits - 1; bit >= localBits; bit--) {
         scan_exclusive64(ctx, scanTmp, DomScanInput{domTw.p, domW.p, bit}, zwScan.p, T);
         foreach(ctx, T, DomLevelKernel{items.p, items2.p, domTw2.p, domW2.p, zwScan.p, bit});
-        std::swap(items.p, items2.p); std::swap(items.cap, items2.cap); std::swap(domTw.p, domTw2.p); std::swap(domTw.cap, domTw2.cap); std::swap(domW.p, domW2.p); std::swap(domW.cap, domW2.cap);
+        items.swap(items2); domTw.swap(domTw2); domW.swap(domW2);
       }
 #ifdef AMG_EMU
       foreach(ctx, T, DomResultKernel{items.p, qIndex.p});
@@ -931,7 +893,7 @@ inline void Engine::buildPatch(DocRows d, size_t N, bool wholeDoc, const OpRows*
         CUDA_CHECK(cudaGetLastError()); ctx.launches++;
       }
 #endif
-      if (curTimer) { curTimer->mark(); curHostMark(); }
+      trace.phase("patch:edits+copy-out");
       ensureEdits(numGroupRecs);
       foreach(ctx, numOps, listGroups(2));
       // the records are in application order by construction: one stable sort by object gives the per-object edit lists
@@ -944,19 +906,19 @@ inline void Engine::buildPatch(DocRows d, size_t N, bool wholeDoc, const OpRows*
       foreach(ctx, numGroupRecs, EditFixKernel{editOut2.p, editElemPos2.p, editKind.p, editPred.p, editDead.p, numGroupRecs});
       foreach(ctx, numGroupRecs, EditMergeKernel{editOut2.p, editElem2.p, editKind.p, editPred.p, editMerge.p, editMulti.p});
       dev_memset(ctx, flagWord.p, 0, 4);
-      foreach(ctx, numGroupRecs, EditLiveKernel{editDead.p, editLive.p, editOut2.p, editElem2.p, editKind.p, flagWord.p, editElemPos2.p, elemHasLive.p, editRowPos2.p, succCnt.p, counterLast.p});
+      foreach(ctx, numGroupRecs, EditLiveKernel{editDead.p, editLive.p, editOut2.p, editElem2.p, editKind.p, flagWord.p, editElemPos2.p, elemHasLive.p, editRowPos2.p, succCntD, counterLast.p});
       DBuf<u32>& liveSlot = editPred;   // pred is consumed by now
       scan_exclusive(ctx, scanTmp, editLive.p, liveSlot.p, numGroupRecs);
       u32 numLive32 = 0, needElem32 = 0; readU32x2(liveSlot.p + numGroupRecs, flagWord.p, &numLive32, &needElem32);
       numLive = numLive32; shipElem = needElem32 != 0;
       foreach(ctx, numGroupRecs, EditCompactKernel{editOut2.p, editElem2.p, editDead.p, liveSlot.p, editKind.p, editMerge.p, editMulti.p, editOut.p, editElem.p, editObjKey2.p, editObjKey.p});
-    } else if (curTimer) { curTimer->mark(); curHostMark(); }
+    } else trace.phase("patch:edits+copy-out");
     // ---- B. setupPatches link edits on list parents: only for elements that did not keep an edit of their own; appended
     //         behind the object's other edits in the order the child objects were first touched
     if (anyListLink) {
       DBuf<u32>& linkCount = rowEmit; DBuf<u32>& linkBase = slot;
       elemVis.ensure(ctx, N + 1); elemVisScan.ensure(ctx, N + 2); linkCount.ensure(ctx, N + 1); linkBase.ensure(ctx, N + 2);
-      foreach(ctx, N, ListVisFlagKernel{d, groupOf.p, groupVisible.p, head.p, succCnt.p, elemVis.p, linkCount.p, nullptr, nullptr, nullptr});
+      foreach(ctx, N, ListVisFlagKernel{d, groupOf.p, groupVisible.p, head.p, succCntD, elemVis.p, linkCount.p, nullptr, nullptr, nullptr});
       scan_exclusive(ctx, scanTmp, elemVis.p, elemVisScan.p, N);   // index of a linked element = visible elements before it once the whole batch is applied
       foreach(ctx, N, ListLinkKernel{0, lctx, listLinkTime.p, elemVisScan.p, objIdx.p, objStart.p, linkCount.p, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, elemHasLive.p});
       scan_exclusive(ctx, scanTmp, linkCount.p, linkBase.p, N);
@@ -976,7 +938,7 @@ inline void Engine::buildPatch(DocRows d, size_t N, bool wholeDoc, const OpRows*
         foreach(ctx, total, GatherToU64Kernel{editObjKey.p, sortVals.p, sortKeys.p});
         sortPairs(sortKeys, sortVals, total, bits_for(numObjs));
         foreach(ctx, total, EditGatherKernel{editOut.p, editElem.p, nullptr, nullptr, sortVals.p, editOut2.p, editElem2.p, nullptr, nullptr});
-        std::swap(editOut.p, editOut2.p); std::swap(editOut.cap, editOut2.cap); std::swap(editElem.p, editElem2.p); std::swap(editElem.cap, editElem2.cap);
+        editOut.swap(editOut2); editElem.swap(editElem2);
       }
     }
     numEdits = numLive + numLink;
@@ -998,11 +960,7 @@ inline void Engine::buildPatch(DocRows d, size_t N, bool wholeDoc, const OpRows*
     if ((u64)end + nBytes >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: patch larger than 4 GiB");
     patchBytesD.ensure(ctx, nBytes + 8);
     foreach(ctx, nRec, PatchBytesGatherKernel{arena.p, propOut.p, numProps, editOut.p, patchByteOff.p, (u32)out.valBytesOff, patchBytesD.p, errWord.p});
-    {   // a value that the reference's decodeValue refuses (it decodes every value that reaches a patch, columnar.js:300-329)
-      const u64 ew = fetchErr();
-      if ((ew & 0xff) == KE_FLOAT_LEN) { u32 l = 0; d2h(ctx, &l, patchByteLen.p + (ew >> 8), 4); sync(ctx); const size_t i = (size_t)(ew >> 8); u32 keyLen = 0; if (i < numProps) { PropRec r; d2h(ctx, &r, propOut.p + i, sizeof(PropRec)); sync(ctx); keyLen = r.keyLen == 0xffffffffu ? 0 : r.keyLen; } throw Error(AMG_ERR_RANGE, "Invalid length for floating point number: " + std::to_string(l - keyLen)); }
-      if (ew) throwKernelError(ew, actorsNow);
-    }
+    if (const u64 ew = fetchErr()) throwPatchValueError(ew, numProps);
   }
   out.valBytesLen = nBytes; out.bigEnd = (out.valBytesOff + nBytes + 7) & ~(size_t)7;
   patchBuf.ensure(out.bigEnd + 4096);
@@ -1013,21 +971,24 @@ inline void Engine::buildPatch(DocRows d, size_t N, bool wholeDoc, const OpRows*
   if (nBytes > 0) d2h_side(ctx, patchBuf.p + out.valBytesOff, patchBytesD.p, nBytes);
 }
 
+// a value that the reference's decodeValue refuses (it decodes every value that reaches a patch, columnar.js:300-329)
+inline void Engine::throwPatchValueError(u64 ew, size_t numProps) {
+  if ((ew & 0xff) == KE_FLOAT_LEN) { u32 l = 0; d2h(ctx, &l, patchByteLen.p + (ew >> 8), 4); sync(ctx); const size_t i = (size_t)(ew >> 8); u32 keyLen = 0; if (i < numProps) { PropRec r; d2h(ctx, &r, propOut.p + i, sizeof(PropRec)); sync(ctx); keyLen = r.keyLen == 0xffffffffu ? 0 : r.keyLen; } throw Error(AMG_ERR_RANGE, "Invalid length for floating point number: " + std::to_string(l - keyLen)); }
+  throwKernelError(ew);
+}
+
 inline void Engine::getPatch(PatchOut& out) {
   dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
   succCnt.ensure(ctx, numRows + 2);
   foreach(ctx, numRows, SuccCntFromOffKernel{succOff.p, succCnt.p});
   struct SideJoin { Ctx& c; ~SideJoin() { side_join(c); } } sideJoin{ctx};
-  buildPatch(doc.view(), numRows, true, nullptr, 0, nullptr, nullptr, nullptr, actorIds, out, succOff.p, succ.p);
+  buildPatch(PatchInputs{doc.view(), numRows, true, succOff.p, succ.p, succCnt.p, Ord{actorRank.p, bits_for(std::max<size_t>(st.actorIds.size(), 2) - 1)}}, out);
   side_join(ctx); sync(ctx);
-  checkErr(actorIds);
+  checkErr();
   fillPatchHeader(out);
   finishPatch(out);
 }
 
-}  // namespace amg
-
-namespace amg {
 
 inline RawRows Engine::rawRows() {
   return RawRows{r_objActor.p, r_objCtr.p, r_keyActor.p, r_keyCtr.p, r_keyStrOff.p, r_keyStrLen.p, r_insert.p, r_action.p, r_valLen.p, r_valOff.p, r_predNum.p, r_predOff.p, r_predActor.p, r_predCtr.p};
@@ -1088,7 +1049,7 @@ inline void Engine::collectUnknownColumns(size_t B, std::vector<std::pair<u64, U
       out.emplace_back(pack_id(h.startOp + i, author), row);
     });
     if (e == KE_UNSUPPORTED_OP) throw Error(AMG_ERR_RANGE, "unexpected VALUE_RAW column");
-    if (e) throwKernelError(((u64)b << 8) | e, actorIds);
+    if (e) throwKernelError(((u64)b << 8) | e);
   }
 }
 
@@ -1114,7 +1075,7 @@ inline void Engine::appendUnknownDocColumns(std::vector<std::pair<u32, std::stri
 
 // Columns of bulk changes (>= HUGE_CHANGE_OPS ops) through the parallel column decoders. largeList holds the large changes of
 // the batch (at most 8 here). hugeDone[k * NCOLS + col] = 1 tells DecodeColumnKernel that column `col` of large change k is done.
-inline u32 Engine::decodeHugeChanges(const RawRows& raw, size_t numLarge) {
+inline void Engine::decodeHugeChanges(const RawRows& raw, size_t numLarge) {
   static const u32 HUGE_CHANGE_OPS = 4096;
   hugeDone.ensure(ctx, numLarge * NCOLS + 1); dev_memset(ctx, hugeDone.p, 0, (numLarge * NCOLS + 1) * 4);
   std::vector<u32> list(numLarge); d2h(ctx, list.data(), largeList.p, numLarge * 4); sync(ctx);
@@ -1147,9 +1108,8 @@ inline u32 Engine::decodeHugeChanges(const RawRows& raw, size_t numLarge) {
       if (ok) { done[pl.col] = 1; any |= 1u << pl.col; }
     }
     h2d(ctx, hugeDone.p + k * NCOLS, done.data(), NCOLS * 4); sync(ctx);
-    if (getenv("AMG_PAR_DOC_TRACE")) fprintf(stderr, "amgpu decode: bulk change %u (%u ops, %u preds): columns expanded in parallel: mask %04x\n", c, n, np, any);
+    if (trace.live) fprintf(stderr, "amgpu decode: bulk change %u (%u ops, %u preds): columns expanded in parallel: mask %04x\n", c, n, np, any);
   }
-  return any;
 }
 
 // Re-runs the decode kernels over the last applied batch (bytes resident in HBM) and times them with CUDA events.
@@ -1188,15 +1148,13 @@ inline void Engine::benchDecode(int iters, float* msSha, float* msParse, float* 
 inline void Engine::computeHashGraph() {
   if (haveHashGraph) return;
   if (!unknownCols.empty()) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: the change history of a loaded document that holds columns with unknown ids cannot be reconstructed");
-  const size_t L = numLoaded, N = numRows, S = numSucc, A = actorIds.size();
+  const size_t L = numLoaded, N = numRows, S = numSucc, A = st.actorIds.size();
   if (L == 0) { haveHashGraph = true; return; }
   if (L >= (1u << 29) || N + S >= (1u << 30)) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: document too large for history reconstruction");
   DocRows d = doc.view();
-  HostClock hclk; const bool htrace = getenv("AMG_PAR_DOC_TRACE") != nullptr;
-  auto hmark = [&](const char* what) { if (htrace) { sync(ctx); fprintf(stderr, "amgpu history: %-26s %9.2f ms\n", what, hclk.ms()); } };
+  HostClock t0; auto hmark = [&](const char* what) { trace.print("history", what, t0); };
   dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
   // ---- 1. change metadata columns (the same decoders as save() after load())
-  auto loadedCol = [&](u32 id) -> const HostChange& { static const u32 IDS[9] = {0x01, 0x03, 0x13, 0x23, 0x35, 0x40, 0x43, 0x56, 0x57}; for (int k = 0; k < 9; k++) if (IDS[k] == id) return loadedCols[k]; return loadedCols[0]; };
   DBuf<long long> cActor, cSeq, cMaxOp, cTime, cDepsNum, cExtra, depIdxV, scratchV; DBuf<u32> msgOff, msgLen, extraOff, extraLen, tmpOff, tmpLen, depsNum32, depBase, depIdx;
   for (DBuf<long long>* b : {&cActor, &cSeq, &cMaxOp, &cTime, &cDepsNum, &cExtra, &scratchV}) b->ensure(ctx, L + 1);
   for (DBuf<u32>* b : {&msgOff, &msgLen, &extraOff, &extraLen, &tmpOff, &tmpLen, &depsNum32}) b->ensure(ctx, L + 2);
@@ -1227,13 +1185,13 @@ inline void Engine::computeHashGraph() {
   if (D) foreach(ctx, D, HistI64ToU32Kernel{depIdxV.p, depIdx.p});
   // ---- 2. actor order (hex string order = byte order), representatives
   std::vector<u32> order(A), rankH(A), repOffH(A), repLenH(A);
-  for (size_t a = 0; a < A; a++) { order[a] = (u32)a; repOffH[a] = actorRep[a].first; repLenH[a] = actorRep[a].second; }
-  std::sort(order.begin(), order.end(), [&](u32 x, u32 y) { return actorIds[x] < actorIds[y]; });
+  for (size_t a = 0; a < A; a++) { order[a] = (u32)a; repOffH[a] = st.actorRep[a].first; repLenH[a] = st.actorRep[a].second; }
+  std::sort(order.begin(), order.end(), [&](u32 x, u32 y) { return st.actorIds[x] < st.actorIds[y]; });
   for (size_t i = 0; i < A; i++) rankH[order[i]] = (u32)i;
   DBuf<u32> rankD, actorOfRank, repOff, repLen;
   for (DBuf<u32>* b : {&rankD, &actorOfRank, &repOff, &repLen}) b->ensure(ctx, A + 1);
   h2d(ctx, rankD.p, rankH.data(), A * 4); h2d(ctx, actorOfRank.p, order.data(), A * 4); h2d(ctx, repOff.p, repOffH.data(), A * 4); h2d(ctx, repLen.p, repLenH.data(), A * 4);
-  const int ctrBits = bits_for(maxOp + 1), idBits = std::min(64, ctrBits + 16);
+  const int ctrBits = bits_for(st.maxOp + 1), idBits = std::min(64, ctrBits + 16);
   hmark("change columns decoded");
   // ---- 3. (successor, predecessor) pairs -> pred lists and deletions
   DBuf<u64> predKey, succKey, keyA, keyB, groupId, opId; DBuf<u32> pairRow, valA, pairRowSorted, head, groupIdx, groupStart, groupRow, isDel, delSlot, idRows;
@@ -1285,7 +1243,7 @@ inline void Engine::computeHashGraph() {
     scan_exclusive(ctx, scanTmp, predNumSorted.p, opPredBase.p, M);
   } else dev_memset(ctx, opPredBase.p, 0, 8);
   const size_t P = M ? readU32(opPredBase.p + M) : 0;
-  checkErr(actorIds);
+  checkErr();
   hmark("ops assigned to changes");
   // ---- 5. the other actors of every change
   HistOpView view{d, opId.p, opSrc.p, opPredStart.p, opPredNum.p, opOrder.p, pairRowSorted.p, (u32)N};
@@ -1325,7 +1283,7 @@ inline void Engine::computeHashGraph() {
   enc.pass = 1; enc.arena = arena.p; enc.outArena = arena.p; enc.outBase = (u32)arenaLen;
   foreach(ctx, L, enc);
   foreach(ctx, L, HistChOffKernel{outOff.p, (u32)arenaLen, chOffD.p});
-  checkErr(actorIds);
+  checkErr();
   hmark("changes encoded");
   // ---- 7. dependency levels (host: one pass over the dependency indexes), hashes level by level
   std::vector<u32> depsNumH(L), depBaseH(L + 1), depIdxH(D), level(L), list(L);
@@ -1360,28 +1318,28 @@ inline void Engine::computeHashGraph() {
     sync(ctx);   // levelStartD is a local
 #endif
   }
-  checkErr(actorIds);
+  checkErr();
   hmark("hashes (all levels)");
   // ---- 8. heads: the changes nobody depends on must be exactly the document's heads (columnar.js:968-980)
   {
     size_t nHeads = 0; for (size_t k = 0; k < L; k++) if (!isDep[k]) nHeads++;
-    bool ok = numApplied != L || nHeads == heads.size();   // (changes applied after the load have moved the heads)
-    std::vector<std::array<u8, 32>> got(heads.size());
+    bool ok = numApplied != L || nHeads == st.heads.size();   // (changes applied after the load have moved the heads)
+    std::vector<std::array<u8, 32>> got(st.heads.size());
     if (headIndexesUnknown) {   // loaded without head indexes: the heads are the changes nobody depends on, matched by hash
       if (numApplied != L) throw Error(AMG_ERR_INTERNAL, "amgpu: head indexes must be resolved right after the load");
       std::vector<u32> cand; for (size_t k = 0; k < L; k++) if (!isDep[k]) cand.push_back((u32)k);
-      ok = cand.size() == heads.size();
+      ok = cand.size() == st.heads.size();
       std::vector<std::array<u8, 32>> ch(cand.size());
       if (ok) { for (size_t i = 0; i < cand.size(); i++) d2h(ctx, ch[i].data(), newHashes.p + (size_t)cand[i] * 32, 32); sync(ctx); }
-      for (size_t i = 0; i < heads.size() && ok; i++) {
-        size_t j = 0; while (j < cand.size() && ch[j] != heads[i]) j++;
-        if (j == cand.size()) ok = false; else headIdx[i] = cand[j];
+      for (size_t i = 0; i < st.heads.size() && ok; i++) {
+        size_t j = 0; while (j < cand.size() && ch[j] != st.heads[i]) j++;
+        if (j == cand.size()) ok = false; else st.headIdx[i] = cand[j];
       }
       if (ok) headIndexesUnknown = false;
     } else if (numApplied == L) {
-      for (size_t i = 0; i < heads.size(); i++) d2h(ctx, got[i].data(), newHashes.p + (size_t)headIdx[i] * 32, 32);
+      for (size_t i = 0; i < st.heads.size(); i++) d2h(ctx, got[i].data(), newHashes.p + (size_t)st.headIdx[i] * 32, 32);
       sync(ctx);
-      for (size_t i = 0; i < heads.size() && ok; i++) if (isDep[headIdx[i]] || got[i] != heads[i]) ok = false;
+      for (size_t i = 0; i < st.heads.size() && ok; i++) if (isDep[st.headIdx[i]] || got[i] != st.heads[i]) ok = false;
     }
     if (!ok) throw Error(AMG_ERR_RANGE, "Mismatched heads hashes: the document's heads are not the hashes of its reconstructed changes");
   }
@@ -1414,7 +1372,7 @@ inline int Engine::debugDecodeColumn(const u8* bytes, size_t len, int kind, size
   } else {
     dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
     foreach_warp(ctx, 1, DebugColumnKernel{kind, colBytes.p, (u32)len, (u32)n, outD.p, tmp.p, errWord.p});
-    checkErr(actorIds);
+    checkErr();
   }
   if (n) d2h(ctx, out, outD.p, n * 8);
   sync(ctx);
@@ -1439,7 +1397,7 @@ inline void Engine::decodeRaw(const u8* blob, const u64* offsets, size_t n, u8* 
   runDecodeTiles(ar.p, n, staged.size());
   readWords({{decTotalsPtr(), 4}, {decTotalsPtr() + 1, 4}, {decTotalsPtr() + 2, 4}, {decTotalsPtr() + 3, 4}}, dst);
   if (decodeOverflowed(tot)) { runDecodeTiles(ar.p, n, staged.size()); readWords({{decTotalsPtr(), 4}, {decTotalsPtr() + 1, 4}, {decTotalsPtr() + 2, 4}, {decTotalsPtr() + 3, 4}}, dst); }
-  checkErr(actorIds);
+  checkErr();
   const size_t M = tot[0];
   DBuf<u32>* cols[12] = {&r_objActor, &r_objCtr, &r_keyActor, &r_keyCtr, &r_keyStrOff, &r_keyStrLen, &r_insert, &r_action, &r_valLen, &r_valOff, &r_predNum, &r_predOff};
   RawRows raw = rawRows();
@@ -1454,7 +1412,7 @@ inline void Engine::decodeRaw(const u8* blob, const u64* offsets, size_t n, u8* 
     }
   }
   foreach(ctx, n, RaiseDecErrKernel{decErr.p, errWord.p});
-  checkErr(actorIds);
+  checkErr();
   d2h(ctx, hashesOut, hashTmp.p, n * 32); d2h(ctx, nOpsOut, nOps.p, n * 4);
   const size_t P = tot[1];
   opBase.ensure(ctx, n + 1); predBase.ensure(ctx, n + 1);
@@ -1467,25 +1425,9 @@ inline void Engine::decodeRaw(const u8* blob, const u64* offsets, size_t n, u8* 
   sync(ctx); *rowsOut = rows; *totalOps = M; lastB = 0;
 }
 
-}  // namespace amg
-
-namespace amg {
 
 extern "C" void amg_host_sha256(const uint8_t* data, size_t len, uint8_t out[32]);   // hostsha.cc (x86 SHA extensions when present)
 inline void host_sha256(const u8* data, size_t len, u8 out[32]) { amg_host_sha256(data, len, out); }
-inline std::string inflateRawBytes(const u8* p, size_t n) {
-  z_stream zs; memset(&zs, 0, sizeof(zs));
-  if (inflateInit2(&zs, -15) != Z_OK) throw Error(AMG_ERR_INTERNAL, "inflateInit failed");
-  std::string out; out.resize(std::max<size_t>(n * 6, 1024)); zs.next_in = (Bytef*)p; zs.avail_in = (uInt)n; size_t produced = 0;
-  while (true) {
-    zs.next_out = (Bytef*)out.data() + produced; zs.avail_out = (uInt)(out.size() - produced);
-    int rc = inflate(&zs, Z_NO_FLUSH); produced = out.size() - zs.avail_out;
-    if (rc == Z_STREAM_END) break;
-    if (rc != Z_OK && rc != Z_BUF_ERROR) { inflateEnd(&zs); throw Error(AMG_ERR_RANGE, "invalid deflate data"); }
-    if (zs.avail_out == 0) out.resize(out.size() * 2); else if (zs.avail_in == 0) { inflateEnd(&zs); throw Error(AMG_ERR_RANGE, "unexpected end of deflate data"); }
-  }
-  inflateEnd(&zs); out.resize(produced); return out;
-}
 
 // Backend.save() (reference new.js:2033-2055, columnar.js:983-1004): change metadata columns (re-derived from the change
 // headers that live in the arena) and the 16 document op columns (from the document table and its succ lists), encoded
@@ -1495,8 +1437,7 @@ inline void Engine::saveDocument(std::string& result) {
   if (!loadedDoc.empty()) { result = loadedDoc; return; }   // unchanged since Backend.load (new.js:2034)
   if (!encoder) encoder.reset(new ColumnEncoder(ctx, scanTmp));
   ColumnEncoder& enc = *encoder; enc.outLen = 0;
-  HostClock sclk; const bool strace = getenv("AMG_PAR_DOC_TRACE") != nullptr;
-  auto smark = [&](const char* what) { if (strace) { sync(ctx); fprintf(stderr, "amgpu save: %-28s %8.2f ms\n", what, sclk.ms()); } };
+  HostClock t0; auto smark = [&](const char* what) { trace.print("save", what, t0); };
   struct Col { u32 id; size_t off, len; };
   std::vector<Col> changeCols, opCols;
   auto add = [&](std::vector<Col>& cols, u32 id, size_t len) { cols.push_back({id, enc.outLen - len, len}); };
@@ -1521,7 +1462,6 @@ inline void Engine::saveDocument(std::string& result) {
       foreach(ctx, C, HashInsertKernel{hashes.p, hashTable.p, (u64)tcap - 1});
       foreach(ctx, K, ResolveDepsKernelT<ChangeMeta>{arena.p, hashes.p, hashTable.p, (u64)tcap - 1, meta.p, nDeps.p, L, depBase.p, depIdx.p, primary.p});
     }
-    auto loadedCol = [&](u32 id) -> const HostChange& { static const u32 IDS[9] = {0x01, 0x03, 0x13, 0x23, 0x35, 0x40, 0x43, 0x56, 0x57}; for (int k = 0; k < 9; k++) if (IDS[k] == id) return loadedCols[k]; return loadedCols[0]; };
     if (L > 0) {   // number of dependency indexes the loaded changes carry
       DBuf<u64>& sumD = pairSucc; sumD.ensure(ctx, 1);
       const HostChange& dn = loadedCol(0x40);
@@ -1557,7 +1497,7 @@ inline void Engine::saveDocument(std::string& result) {
                                        add(changeCols, 0x43, enc.deltaNum(saveVals.p, (size_t)loadedDeps + totalDeps));
     loadedVal(LC_EXTRA_LEN, 0x56, (u32)L); changeVal(SM_EXTRA_LEN); add(changeCols, 0x56, enc.rleNum(saveVals.p, C, false));
                                        add(changeCols, 0x57, enc.raw(arena.p, saveStrOff.p, saveStrLen.p, C));
-    checkErr(actorIds);
+    checkErr();
   }
   // ---- document ops (columnar.js:60-82)
   if (N > 0) {
@@ -1614,12 +1554,12 @@ inline void Engine::saveDocument(std::string& result) {
   smark("columns deflated (host)");
   std::string body;
   auto uleb = [&](u64 v) { do { u8 b = v & 0x7f; v >>= 7; if (v) b |= 0x80; body.push_back((char)b); } while (v); };
-  uleb(actorIds.size()); for (auto& a : actorIds) { uleb(a.size()); body += a; }
-  uleb(heads.size()); for (auto& h : heads) body.append((const char*)h.data(), 32);
+  uleb(st.actorIds.size()); for (auto& a : st.actorIds) { uleb(a.size()); body += a; }
+  uleb(st.heads.size()); for (auto& h : st.heads) body.append((const char*)h.data(), 32);
   uleb(numChangeCols); for (size_t k = 0; k < numChangeCols; k++) { uleb(packed[k].id); uleb(packed[k].data.size()); }
   uleb(packed.size() - numChangeCols); for (size_t k = numChangeCols; k < packed.size(); k++) { uleb(packed[k].id); uleb(packed[k].data.size()); }
   for (auto& p : packed) body += p.data;
-  for (u32 i : headIdx) uleb(i);
+  for (u32 i : st.headIdx) uleb(i);
   std::string head; head.push_back(0); { u64 v = body.size(); do { u8 b = v & 0x7f; v >>= 7; if (v) b |= 0x80; head.push_back((char)b); } while (v); }
   std::string hashed = head + body; u8 digest[32]; host_sha256((const u8*)hashed.data(), hashed.size(), digest);
   smark("container assembled + hashed");
@@ -1633,8 +1573,7 @@ inline void Engine::saveDocument(std::string& result) {
 // as in SURVEY.md §2 row 12; column expansion and everything downstream run on the device.
 inline void Engine::loadDocument(const u8* buf, size_t len) {
   if (numApplied != 0 || numRows != 0) throw Error(AMG_ERR_INTERNAL, "load needs a fresh backend");
-  HostClock lclk; const bool ltrace = getenv("AMG_PAR_DOC_TRACE") != nullptr;
-  auto lmark = [&](const char* what) { if (ltrace) { sync(ctx); fprintf(stderr, "amgpu load: %-28s %8.2f ms\n", what, lclk.ms()); } };
+  HostClock t0; auto lmark = [&](const char* what) { trace.print("load", what, t0); };
   // columnar.js:688-708 decodeContainerHeader
   if (len < 10 || buf[0] != 0x85 || buf[1] != 0x6f || buf[2] != 0x4a || buf[3] != 0x83) throw Error(AMG_ERR_RANGE, "Data does not begin with magic bytes 85 6f 4a 83");
   ByteReader r(buf, 8, (u32)len); const u32 chunkType = buf[8]; r.pos = 9; const u64 chunkLen = r.uleb();
@@ -1755,7 +1694,7 @@ inline void Engine::loadDocument(const u8* buf, size_t len) {
   if (!counted) {   // short action column: rows by the serial record walk, the succ total still in parallel if there are many rows
     serialMask = 0xffffu;
     foreach(ctx, 1, DocCountRowsKernel{arena.p, dc, flagWord.p, errWord.p});
-    u32 n32 = 0; d2h(ctx, &n32, flagWord.p, 4); sync(ctx); checkErr(actors);
+    u32 n32 = 0; d2h(ctx, &n32, flagWord.p, 4); sync(ctx); checkErr();
     if (n32 >= parDocMinRows && n32 < (1u << 29)) {
       N = n32; ensureRows(); u64 sum = 0;
       if (dc.len[13] == 0) { counted = true; S = 0; }
@@ -1765,7 +1704,7 @@ inline void Engine::loadDocument(const u8* buf, size_t len) {
   if (!counted) {
     serialMask = 0xffffu;
     foreach(ctx, 1, DocCountKernel{arena.p, dc, flagWord.p, errWord.p});
-    u32 cnt[2]; d2h(ctx, cnt, flagWord.p, 8); sync(ctx); checkErr(actors);
+    u32 cnt[2]; d2h(ctx, cnt, flagWord.p, 8); sync(ctx); checkErr();
     N = cnt[0]; S = cnt[1];
   }
   lmark("rows counted");
@@ -1799,19 +1738,19 @@ inline void Engine::loadDocument(const u8* buf, size_t len) {
       DBuf<u32>& recStart = parCols.recOff; DBuf<u32>& recStrOff = parCols.recTok; DBuf<u32>& recStrLen = parCols.recN;
       recStart.ensure(ctx, N + 3); recStrOff.ensure(ctx, N + 3); recStrLen.ensure(ctx, N + 3);
       foreach_warp(ctx, 1, DocKeyStrRecordsKernel{arena.p, dc.off[4], dc.len[4], (u32)N, recStart.p, recStrOff.p, recStrLen.p, flagWord.p, errWord.p});
-      u32 rc[2]; d2h(ctx, rc, flagWord.p, 8); sync(ctx); checkErr(actors);
+      u32 rc[2]; d2h(ctx, rc, flagWord.p, 8); sync(ctx); checkErr();
       foreach(ctx, N, DocKeyStrExpandKernel{recStart.p, recStrOff.p, recStrLen.p, rc[0], raw.keyStrOff, raw.keyStrLen});
       serialMask &= ~(1u << 4);
     }
   }
-  if (getenv("AMG_PAR_DOC_TRACE")) fprintf(stderr, "amgpu load: %zu rows, %zu succ entries, columns left to the serial decoder: mask %04x (counted in parallel: %d)\n", N, S, serialMask & 0xe3ffu, counted ? 1 : 0);
+  if (Trace::enabled()) fprintf(stderr, "amgpu load: %zu rows, %zu succ entries, columns left to the serial decoder: mask %04x (counted in parallel: %d)\n", N, S, serialMask & 0xe3ffu, counted ? 1 : 0);
   if (serialMask & 0xe3ffu) foreach_warp(ctx, 16, DocColumnKernel{arena.p, dc, (u32)N, (u32)S, raw, o_change.p, o_time.p, errWord.p, serialMask});
   lmark("columns decoded");
   doc.ensure(ctx, N + 1); succOff.ensure(ctx, N + 2); succ.ensure(ctx, S + 1);
   DBuf<u64>& maxOpD = pairSucc; maxOpD.ensure(ctx, 1); dev_memset(ctx, maxOpD.p, 0, 8);
   foreach(ctx, N, DocFinalizeKernel{raw, o_change.p, o_time.p, (u32)actors.size(), doc.view(), succOff.p, succ.p, maxOpD.p, errWord.p});
   { const u32 s32 = (u32)S; h2d(ctx, succOff.p + N, &s32, 4); }
-  u64 mx = 0; d2h(ctx, &mx, maxOpD.p, 8); sync(ctx); checkErr(actors);
+  u64 mx = 0; d2h(ctx, &mx, maxOpD.p, 8); sync(ctx); checkErr();
   lmark("rows finalized");
   {   // op columns with unknown ids: their values are kept per op (host; unknowncols.hpp) so that save() writes them again
     bool anyUnknown = false; for (auto& c : opCols) if (!is_known_doc_column(c.id)) anyUnknown = true;
@@ -1826,20 +1765,19 @@ inline void Engine::loadDocument(const u8* buf, size_t len) {
         unknownCols.byOp[ids[i]] = row;
       });
       if (e == KE_UNSUPPORTED_OP) throw Error(AMG_ERR_RANGE, "unexpected VALUE_RAW column");
-      if (e) throwKernelError((u64)e, actors);
+      if (e) throwKernelError((u64)e);
     }
   }
   // ---- change history placeholders: only the head hashes are known (new.js:1727-1739)
   hashes.ensure(ctx, numChanges * 32 + 64); dev_memset(ctx, hashes.p, 0, numChanges * 32 + 64);
   if (!headIdxUnknown) for (size_t i = 0; i < hs.size(); i++) { if (headsIndexes[i] >= numChanges) throw Error(AMG_ERR_RANGE, "head index out of range"); h2d(ctx, hashes.p + (size_t)headsIndexes[i] * 32, hs[i].data(), 32); }
   sync(ctx);
-  numRows = N; numSucc = S; numApplied = numChanges; arenaLen = cur; maxOp = mx; actorIds = actors; actorRep = reps; clock = clk;
-  heads = hs; headIdx = headsIndexes;
-  { std::vector<size_t> o(heads.size()); for (size_t i = 0; i < o.size(); i++) o[i] = i; std::sort(o.begin(), o.end(), [&](size_t a, size_t b) { return hs[a] < hs[b]; });
-    for (size_t i = 0; i < o.size(); i++) { heads[i] = hs[o[i]]; headIdx[i] = headsIndexes[o[i]]; } }
+  numRows = N; numSucc = S; numApplied = numChanges; arenaLen = cur;
+  std::vector<size_t> o(hs.size()); for (size_t i = 0; i < o.size(); i++) o[i] = i; std::sort(o.begin(), o.end(), [&](size_t a, size_t b) { return hs[a] < hs[b]; });
+  st = DocState{actors, reps, clk, mx, {}, {}}; for (size_t i : o) { st.heads.push_back(hs[i]); st.headIdx.push_back(headsIndexes[i]); }
   changes.assign(numChanges, HostChange{0, 0}); haveHashGraph = false; loadedDoc.assign((const char*)buf, len); numLoaded = numChanges; headIndexesUnknown = headIdxUnknown;
   lmark("host state");
-  while (actorCap < 2 * (actorIds.size() + 16)) actorCap *= 2;
+  while (actorCap < 2 * (st.actorIds.size() + 16)) actorCap *= 2;
   actorSlots.ensure(ctx, actorCap); rebuildActorTable();
   if (headIndexesUnknown) computeHashGraph();   // finds the heads' change indexes (and leaves the history rebuilt)
 }

@@ -619,16 +619,16 @@ struct BackendDoc {
   void applyChangesPass(Patches& patches, std::vector<std::shared_ptr<AppliedChange>>& decodedChanges, DocState& ds,
                         std::vector<std::string>& objectIds, bool throwExceptions,
                         std::vector<std::shared_ptr<AppliedChange>>& applied, std::vector<std::shared_ptr<AppliedChange>>& enqueued) {
-    std::set<std::string> headsSet(ds.heads.begin(), ds.heads.end()), changeHashes;
+    std::set<std::string> headsSet(ds.heads.begin(), ds.heads.end()), batchHashes;
     std::map<std::string, int64_t> clk = ds.clock;
     for (auto& chp : decodedChanges) {
       const DecodedChange& change = chp->dc;
-      if (ds.changeIndexByHash->count(change.hash) || changeHashes.count(change.hash)) continue;
+      if (ds.changeIndexByHash->count(change.hash) || batchHashes.count(change.hash)) continue;
       const int64_t expectedSeq = (clk.count(change.actor) ? clk[change.actor] : 0) + 1;
       bool causallyReady = true;
       for (auto& dep : change.deps) {
         auto it = ds.changeIndexByHash->find(dep);
-        if ((it == ds.changeIndexByHash->end() || it->second == -1) && !changeHashes.count(dep)) causallyReady = false;
+        if ((it == ds.changeIndexByHash->end() || it->second == -1) && !batchHashes.count(dep)) causallyReady = false;
       }
       if (!causallyReady) enqueued.push_back(chp);
       else if (change.seq < expectedSeq) {
@@ -637,7 +637,7 @@ struct BackendDoc {
       } else if (change.seq > expectedSeq) {
         throw RangeError("Skipped sequence number " + std::to_string(expectedSeq) + " for actor " + change.actor);
       } else {
-        clk[change.actor] = change.seq; changeHashes.insert(change.hash);
+        clk[change.actor] = change.seq; batchHashes.insert(change.hash);
         for (auto& dep : change.deps) headsSet.erase(dep);
         headsSet.insert(change.hash); applied.push_back(chp);
       }

@@ -14,11 +14,12 @@ for name in sys.argv[1:] or ['C4', 'C2b', 'C2']:
     for it in range(3):
         L.amg_reset(doc.h, C.byref(err))
         pp = C.c_void_p(); t0 = time.perf_counter()
-        if it == 2:
-            os.environ['AMG_DEBUG_LIVE_NOW'] = '1'
+        if it == 2:   # the warm call prints its marks as they happen
+            os.environ['AMG_TRACE'] = '1'
         rc = L.amg_apply_changes_packed(doc.h, t.blob.ctypes.data_as(C.c_void_p), offs.ctypes.data_as(C.c_void_p), C.c_size_t(t.n_changes), 0, 1, C.byref(pp), C.byref(err))
         dt = (time.perf_counter() - t0) * 1e3
         L.amg_patch_free(pp)
     buf = C.create_string_buffer(8192); L.amg_debug_marks(doc.h, buf, 8192)
     print(name, 'rc', rc, 'wall %.2f ms' % dt, 'launches/call', doc.launches() // 3, 'phases', [round(x, 2) for x in doc.timings()[:9]])
     print('  marks:', buf.value.decode())
+    os.environ.pop('AMG_TRACE', None)
