@@ -28,7 +28,7 @@ struct amg_backend {
 
   void ensureGraph() {
     Engine& e = eng;
-    if (!e.haveHashGraph) e.computeHashGraph();   // new.js:1922, 1980, 2000, 2015
+    if (!e.loaded.haveHashGraph) e.computeHashGraph();   // new.js:1922, 1980, 2000, 2015
     if (g.known == e.numApplied) return;
     const size_t from = g.known, to = e.numApplied;
     e.ensureHostMirror();   // the change headers are read from the host copy of the arena (fetched now if the batch came from pinned / device memory)
@@ -52,14 +52,8 @@ struct amg_backend {
   static std::string deflateChange(const std::string& plain) {
     ByteReader r((const u8*)plain.data(), 9, (u32)plain.size()); const u64 bodyLen = r.uleb();
     if (r.err || r.pos + bodyLen != plain.size()) throw amg::Error(AMG_ERR_INTERNAL, "deflateChange: malformed change");
-    z_stream zs; memset(&zs, 0, sizeof(zs));
-    if (deflateInit2(&zs, 6, Z_DEFLATED, -15, 8, Z_DEFAULT_STRATEGY) != Z_OK) throw amg::Error(AMG_ERR_INTERNAL, "deflateInit failed");
-    std::string comp; comp.resize(deflateBound(&zs, (uLong)bodyLen));
-    zs.next_in = (Bytef*)plain.data() + r.pos; zs.avail_in = (uInt)bodyLen; zs.next_out = (Bytef*)comp.data(); zs.avail_out = (uInt)comp.size();
-    const int rc = ::deflate(&zs, Z_FINISH); comp.resize(zs.total_out); deflateEnd(&zs);
-    if (rc != Z_STREAM_END) throw amg::Error(AMG_ERR_INTERNAL, "deflate failed");
-    std::string out(plain, 0, 8); out.push_back(2);
-    { u64 v = comp.size(); do { u8 b = v & 0x7f; v >>= 7; if (v) b |= 0x80; out.push_back((char)b); } while (v); }
+    const std::string comp = amg::deflateRawBytes((const u8*)plain.data() + r.pos, (size_t)bodyLen);
+    std::string out(plain, 0, 8); out.push_back(2); amg::put_uleb(out, comp.size());
     return out + comp;
   }
   std::string changeBytes(u32 idx) {
@@ -67,7 +61,7 @@ struct amg_backend {
     if (const HostChange* o = eng.originalOf(idx)) return std::string((const char*)eng.hostArena.data() + o->off, o->len);
     const HostChange& c = eng.changes[idx];
     std::string plain((const char*)eng.hostArena.data() + c.off, c.len);
-    if (idx < eng.historyRebuilt && plain.size() >= 256) return deflateChange(plain);   // what encodeChange returns for a rebuilt change (columnar.js:738)
+    if (idx < eng.loaded.historyRebuilt && plain.size() >= 256) return deflateChange(plain);   // what encodeChange returns for a rebuilt change (columnar.js:738)
     return plain;
   }
 };
@@ -112,8 +106,8 @@ amg_backend* amg_clone(amg_backend* src, amg_error* err) {
     d.numApplied = s.numApplied; d.hashes.ensure(c, s.numApplied * 32 + 64); d2d(c, d.hashes.p, s.hashes.p, s.numApplied * 32);
     d.numRows = s.numRows; d.doc.copyFrom(c, s.doc, s.numRows);
     d.numSucc = s.numSucc; d.succOff.ensure(c, s.numRows + 2); d2d(c, d.succOff.p, s.succOff.p, (s.numRows + 1) * 4); d.succ.ensure(c, s.numSucc + 1); d2d(c, d.succ.p, s.succ.p, s.numSucc * 8);
-    d.st = s.st; d.changes = s.changes; d.deflatedOriginal = s.deflatedOriginal; d.loadedDoc = s.loadedDoc; d.numLoaded = s.numLoaded; for (int k = 0; k < 9; k++) d.loadedCols[k] = s.loadedCols[k];
-    d.unknownCols = s.unknownCols; d.queue = s.queue; d.queueOriginal = s.queueOriginal; d.haveHashGraph = s.haveHashGraph; d.historyRebuilt = s.historyRebuilt;
+    d.st = s.st; d.changes = s.changes; d.deflatedOriginal = s.deflatedOriginal; d.loaded = s.loaded;
+    d.unknownCols = s.unknownCols; d.queue = s.queue; d.queueOriginal = s.queueOriginal;
     while (d.actorCap < 2 * (d.st.actorIds.size() + 16)) d.actorCap *= 2;
     d.actorSlots.ensure(c, d.actorCap); d.rebuildActorTable();
     sync(c);

@@ -128,6 +128,11 @@ struct PcBoolExpandKernel {   // a reader past the end of the column yields fals
   HD void operator()(size_t i) const { if ((u32)i >= runOff[T]) { out[i] = 0; return; } out[i] = pc_record_of(runOff, T, (u32)i) & 1u; }
 };
 
+// Parallel decoder kinds (ParColumnDecoder::decode). Values go to the row field `u` (NULL32 for null) or, where there is
+// none, to `v` (NULLV for null); PK_LEN / PK_COUNT / PK_EXTRA_LEN also write the running offsets and the total.
+enum ParKind { PK_NONE, PK_UINT, PK_INT, PK_DELTA, PK_BOOL, PK_LEN, PK_COUNT, PK_EXTRA_LEN };
+struct PcOut { u32* u = nullptr; long long* v = nullptr; u32* off = nullptr; u32* len = nullptr; u32 base = 0; u64* sum = nullptr; };
+
 struct ParColumnDecoder {
   Ctx& ctx; ScanTemp& st;
   DBuf<u32> flag, ends, tokPos, nxtA, nxtB, reach, defect, recIdx, recTok, recN, recOff, word; DBuf<u64> tokU, excl; DBuf<long long> tokS, vals;
@@ -257,6 +262,55 @@ struct ParColumnDecoder {
     foreach(ctx, n, PcBoolExpandKernel{recOff.p, T, out});
     return true;
   }
+  // n values of one column through the decoder of its kind (false: take the serial decoder)
+  bool decode(int kind, const u8* bytes, size_t len, size_t n, const PcOut& o) {
+    switch (kind) {
+      case PK_UINT: return o.u ? toU32(bytes, len, n, o.u) : toI64(bytes, len, false, n, o.v);
+      case PK_INT: return toI64(bytes, len, true, n, o.v);
+      case PK_DELTA: return o.u ? deltaToU32(bytes, len, n, o.u) : deltaToI64(bytes, len, n, o.v);
+      case PK_BOOL: return boolean(bytes, len, n, o.u);
+      case PK_LEN: return lenColumn(bytes, len, n, o.u, o.off, o.base, o.sum);
+      case PK_COUNT: return countColumn(bytes, len, n, o.u, o.off, o.sum);
+      case PK_EXTRA_LEN: return extraLenColumn(bytes, len, n, o.v, o.off, o.len, o.base);
+      default: return false;   // utf8 and raw bytes: serial only
+    }
+  }
 };
+
+// The parallel decoder of each change column kind (utf8, raw bytes, child columns: none) and the row fields it fills
+// (rows of one change start at rowBase, its preds at predBase; valBase: arena offset of its valRaw column).
+static const int CX_PAR_KIND[NCOLS] = {PK_UINT, PK_UINT, PK_UINT, PK_DELTA, PK_NONE, PK_BOOL, PK_UINT, PK_LEN, PK_NONE, PK_NONE, PK_NONE, PK_COUNT, PK_UINT, PK_DELTA};
+inline PcOut cx_outputs(const RawRows& r, int cx, u32 rowBase, u32 predBase, u32 valBase, u64* sum) {
+  u32* const field[NCOLS] = {r.objActor, r.objCtr, r.keyActor, r.keyCtr, nullptr, r.insert, r.action, r.valLen, nullptr, nullptr, nullptr, r.predNum, r.predActor, r.predCtr};
+  PcOut o; if (!field[cx]) return o;
+  o.u = field[cx] + (cx == CX_PRED_ACTOR || cx == CX_PRED_CTR ? predBase : rowBase);
+  if (cx == CX_VAL_LEN) { o.off = r.valOff + rowBase; o.base = valBase; o.sum = sum; }
+  if (cx == CX_PRED_NUM) { o.off = r.predOff + rowBase; o.sum = sum; }
+  return o;
+}
+
+// ---------------------------------------------------------------- the document chunk's columns (columnar.js:60-94)
+// Op columns, one value per document row (the succ group: one per succ entry), in directory order.
+enum DocColIx { OC_OBJ_ACTOR, OC_OBJ_CTR, OC_KEY_ACTOR, OC_KEY_CTR, OC_KEY_STR, OC_ID_ACTOR, OC_ID_CTR, OC_INSERT, OC_ACTION, OC_VAL_LEN,
+                OC_VAL_RAW, OC_CHLD_ACTOR, OC_CHLD_CTR, OC_SUCC_NUM, OC_SUCC_ACTOR, OC_SUCC_CTR, NUM_DOC_COLS };
+static const u32 DOC_COL_IDS[NUM_DOC_COLS] = {0x01, 0x02, 0x11, 0x13, 0x15, 0x21, 0x23, 0x34, 0x42, 0x56, 0x57, 0x61, 0x63, 0x80, 0x81, 0x83};
+static const u32 ALL_DOC_COLS = (1u << NUM_DOC_COLS) - 1;
+static const u32 DECODED_DOC_COLS = ALL_DOC_COLS & ~((1u << OC_VAL_RAW) | (1u << OC_CHLD_ACTOR) | (1u << OC_CHLD_CTR));   // valRaw is read through valLen; child columns are always empty
+struct DocCols { u32 off[NUM_DOC_COLS]; u32 len[NUM_DOC_COLS]; };   // arena ranges (len 0: absent)
+// The change column decoder that reads op column k (-1: none). idActor / idCtr have no change column of their own: they
+// are read as objActor (RLE uint) and keyCtr (delta) into the rows doc_col_rows() puts in those fields' place.
+HD int doc_col_decoder(int k) {   // (the succ group has the pred group's layout)
+  const signed char cx[NUM_DOC_COLS] = {CX_OBJ_ACTOR, CX_OBJ_CTR, CX_KEY_ACTOR, CX_KEY_CTR, CX_KEY_STR, CX_OBJ_ACTOR, CX_KEY_CTR, CX_INSERT, CX_ACTION,
+                                        CX_VAL_LEN, -1, -1, -1, CX_PRED_NUM, CX_PRED_ACTOR, CX_PRED_CTR};
+  return cx[k];
+}
+HD RawRows doc_col_rows(int k, RawRows r, u32* idActor, u32* idCtr) { if (k == OC_ID_ACTOR) r.objActor = idActor; if (k == OC_ID_CTR) r.keyCtr = idCtr; return r; }
+
+// Change metadata columns, one value per change (depsIndex: one per dependency). lc: LoadedColKernel's reader, pk: the parallel decoder.
+enum ChangeColIx { CC_ACTOR, CC_SEQ, CC_MAX_OP, CC_TIME, CC_MESSAGE, CC_DEPS_NUM, CC_DEPS_INDEX, CC_EXTRA_LEN, CC_EXTRA_RAW, NUM_CHANGE_COLS };
+struct ChangeColDef { u32 id; int lc, pk; };
+static const ChangeColDef CHANGE_COLS[NUM_CHANGE_COLS] = {
+  {0x01, LC_UINT, PK_UINT}, {0x03, LC_DELTA, PK_DELTA}, {0x13, LC_DELTA, PK_DELTA}, {0x23, LC_DELTA, PK_DELTA}, {0x35, LC_STRING, PK_NONE},
+  {0x40, LC_UINT, PK_UINT}, {0x43, LC_DELTA, PK_DELTA}, {0x56, LC_EXTRA_LEN, PK_EXTRA_LEN}, {0x57, -1, PK_NONE}};
 
 }  // namespace amg

@@ -98,6 +98,16 @@ struct PatchOut {   // flat patch, written straight into the engine's pinned out
 
 struct HostChange { u32 off, len; };   // (arena offset, length) of the inflated change
 
+// What the engine keeps of a document it loaded (Backend.load). loadDocument sets it whole and reset() clears it.
+struct LoadedDoc {
+  std::string bytes;                      // the document as loaded: what save() returns until a change is applied (new.js:2034)
+  size_t numChanges = 0;                  // changes [0, numChanges) came from the document
+  HostChange cols[NUM_CHANGE_COLS] = {};  // arena ranges of its change metadata columns (save() re-encodes them with later changes appended)
+  bool haveHashGraph = true;              // false after a load until computeHashGraph has rebuilt the changes' bytes and hashes (new.js:1887-1912)
+  size_t historyRebuilt = 0;              // changes [0, historyRebuilt) were rebuilt by computeHashGraph (getChanges DEFLATEs the large ones like encodeChange does)
+  bool headIndexesUnknown = false;        // several heads and no head indexes, until computeHashGraph has matched them
+};
+
 // Pinned host mirror of the arena: grows without zero-filling; H2D copies read straight from it.
 struct HostArena {
   HBuf<u8> buf; size_t len = 0;
@@ -121,6 +131,15 @@ inline std::string inflateRawBytes(const u8* p, size_t n) {
     if (zs.avail_out == 0) out.resize(out.size() * 2); else if (zs.avail_in == 0) { inflateEnd(&zs); throw Error(AMG_ERR_RANGE, "unexpected end of deflate data"); }
   }
   inflateEnd(&zs); out.resize(produced); return out;
+}
+inline std::string deflateRawBytes(const u8* p, size_t n) {   // zlib level 6, as pako.deflateRaw
+  z_stream zs; memset(&zs, 0, sizeof(zs));
+  if (deflateInit2(&zs, 6, Z_DEFLATED, -15, 8, Z_DEFAULT_STRATEGY) != Z_OK) throw Error(AMG_ERR_INTERNAL, "deflateInit failed");
+  std::string comp; comp.resize(deflateBound(&zs, (uLong)n));
+  zs.next_in = (Bytef*)p; zs.avail_in = (uInt)n; zs.next_out = (Bytef*)comp.data(); zs.avail_out = (uInt)comp.size();
+  const int rc = ::deflate(&zs, Z_FINISH); comp.resize(zs.total_out); deflateEnd(&zs);
+  if (rc != Z_STREAM_END) throw Error(AMG_ERR_INTERNAL, "deflate failed");
+  return comp;
 }
 inline std::string hex_of(const u8* p, size_t n) { static const char* d = "0123456789abcdef"; std::string s; for (size_t i = 0; i < n; i++) { s.push_back(d[p[i] >> 4]); s.push_back(d[p[i] & 15]); } return s; }
 
@@ -163,7 +182,7 @@ class Engine {
   DBuf<u32> elemPos, keyRankAt, objPos, head, headScan, groupOf, groupRows, groupVisible, groupFirst, groupTouched, groupLinked, objTouchedAt, linkDone, emit, marker, slot;
   DBuf<u32> isObjHead, objIdx, objStart, elemVis, elemVisScan, rowEmit, firstVis, state, nItems, itemBase, qIndex, zero, wzero, zscan, wscan, editObjKey;
   DBuf<DomItem> items, items2; DBuf<PropRec> propOut; DBuf<EditRec> editOut, editOut2; DBuf<u64> editElem, editElem2;
-  std::unique_ptr<ColumnEncoder> encoder; DBuf<long long> saveVals; DBuf<u32> saveStrOff, saveStrLen; std::string loadedDoc; size_t numLoaded = 0; HostChange loadedCols[9] = {}; DBuf<u64> counterTotal; DBuf<int> domW, domW2; DBuf<u32> elemMinT, editRowPos, editRowPos2, editObjKey2, rowClass, firstBare, counterOwner, newSuccTime, counterLast, runHeadFlag, runScan, runStart, elemFollower, domTw, domTw2, oldVisScan, inflLen, inflOff, groupHasChild, gCount, gElem, gT1, gQOrd, gBase, nQ, elemHasRecs, listLinkTime, editElemPos, editElemPos2, editKind, editPred, editDead, editMerge, editMulti, editLive;
+  std::unique_ptr<ColumnEncoder> encoder; DBuf<long long> saveVals; DBuf<u32> saveStrOff, saveStrLen; DBuf<u64> counterTotal; DBuf<int> domW, domW2; DBuf<u32> elemMinT, editRowPos, editRowPos2, editObjKey2, rowClass, firstBare, counterOwner, newSuccTime, counterLast, runHeadFlag, runScan, runStart, elemFollower, domTw, domTw2, oldVisScan, inflLen, inflOff, groupHasChild, gCount, gElem, gT1, gQOrd, gBase, nQ, elemHasRecs, listLinkTime, editElemPos, editElemPos2, editKind, editPred, editDead, editMerge, editMulti, editLive;
   DBuf<u32> seqSlot, actorCnt, actorBaseD, clockD, changeActor, editTime; DBuf<u8> hashTmp; DBuf<u32> headsPack, headsOut;
   DBuf<u32> finalTime, gFailed, memberFinal, opAt, runHead, opGroupHead; DBuf<u64> gBound; DBuf<HostChange> chPairs; DBuf<u32> largeFlag, largeSlot, largeList; size_t lastNumLarge = 0; DBuf<u64> zwScan; DBuf<u32> deflList, patchTriples;
 
@@ -297,8 +316,8 @@ class Engine {
     if (r.err || r.pos + clen > len) throw Error(AMG_ERR_RANGE, "buffer ended with incomplete number");
     const std::string body = inflateRawBytes(buf + r.pos, clen);
     // header: magic + checksum (8 bytes), chunk type 1, LEB128 length, then the inflated body
-    u8 hdr[24]; memcpy(hdr, buf, 8); hdr[8] = 1; size_t hl = 9; u64 v = body.size(); do { u8 b = v & 0x7f; v >>= 7; if (v) b |= 0x80; hdr[hl++] = b; } while (v);
-    return std::string((const char*)hdr, hl) + body;
+    std::string out((const char*)buf, 8); out.push_back(1); put_uleb(out, body.size());
+    return out + body;
   }
 
   // ---------------------------------------------------------------- applyChanges
@@ -331,7 +350,6 @@ class Engine {
   [[noreturn]] void throwActorError(u64 ew, const std::vector<std::string>& actors); [[noreturn]] void throwSequenceError(ApplyCall& a);
   [[noreturn]] void throwOpError(u64 ew, const std::vector<std::string>& actors); [[noreturn]] void throwPatchValueError(u64 ew, size_t numProps);
   void getPatch(PatchOut& out);
-  void saveDocument(std::string& result);
   struct PatchInputs {   // everything buildPatch reads: the rows in document order, their succ CSR and counts; incremental: the batch and the op-set tables
     DocRows d; size_t N; bool wholeDoc; const u32* succOff; const u64* succ; const u32* succCnt; Ord ord;
     const OpRows* ops = nullptr; size_t numOps = 0; const IdTable* idt = nullptr; const u32 *rowOfOp = nullptr, *pos = nullptr;
@@ -341,17 +359,12 @@ class Engine {
   void fillPatchHeader(PatchOut& out);
   void finishPatch(PatchOut& out);
   void reset();
-  void loadDocument(const u8* buf, size_t len);
-  size_t historyRebuilt = 0;   // changes [0, historyRebuilt) were rebuilt by computeHashGraph (getChanges DEFLATEs the large ones like encodeChange does)
   DBuf<u64> excl64, offsDev;
-  bool headIndexesUnknown = false;   // Backend.load of a document with several heads and no head indexes, until computeHashGraph has matched them
-  bool haveHashGraph = true;   // false after Backend.load: change history (hashes, bytes) is not reconstructed (new.js:1887-1912)
   void benchDecode(int iters, float* msSha, float* msParse, float* msDec, u64* algoBytes);
   UnknownStore unknownCols;   // values of columns with ids this version does not know, per op (unknowncols.hpp)
   void collectUnknownColumns(size_t B, std::vector<std::pair<u64, UnknownRow>>& out, std::set<u32>& ids);
   void appendUnknownDocColumns(std::vector<std::pair<u32, std::string>>& cols);   // save(): their document columns
   RawRows rawRows();
-  const HostChange& loadedCol(u32 id) const { static const u32 IDS[9] = {0x01, 0x03, 0x13, 0x23, 0x35, 0x40, 0x43, 0x56, 0x57}; for (int k = 0; k < 9; k++) if (IDS[k] == id) return loadedCols[k]; return loadedCols[0]; }   // a loaded document's change column
   void decodeHugeChanges(const RawRows& raw, size_t numLarge); DBuf<u32> hugeDone;
   void runDecodeTiles(const u8* arenaP, size_t B, size_t batchBytes, const u32* deflListP = nullptr, size_t numDefl = 0, size_t deflStart = 0);
   DecodeTilesArgs decodeArgs(const u8* arenaP, size_t B, size_t batchBytes);
@@ -363,11 +376,51 @@ class Engine {
     d2h(ctx, hostArena.data() + from, arena.p + from, arenaLen - from); sync(ctx);
   }   // sizes the raw row tables and launches the fused decode
   bool decodeOverflowed(const u32 totals[4]);
-  void computeHashGraph();   // change history of a loaded document (history.cuh)
   int debugDecodeColumn(const u8* bytes, size_t len, int kind, size_t n, bool parallel, long long* out);
   void decodeRaw(const u8* blob, const u64* offsets, size_t n, u8* hashesOut, u32* nOpsOut, u32** rowsOut, size_t* totalOps, size_t* totalPreds);
   size_t lastB = 0, lastM = 0, lastP = 0, lastBytes = 0;
   size_t decWantRows = 0, decWantPreds = 0, decRowCap = 0, decPredCap = 0;
+
+  // ---------------------------------------------------------------- load, save, history: what one call's phases hand to each other
+  LoadedDoc loaded;
+  void decodeLoadedCol(int k, size_t count, long long* out, u32* strOff, u32* strLen);   // change metadata column k of the loaded document
+  struct LoadCall {
+    const u8* buf; size_t len; ByteReader r; HostClock t0;
+    struct ColInfo { u32 id; u64 len; std::string data; }; std::vector<ColInfo> changeCols, opCols;
+    std::vector<std::pair<ColInfo*, const u8*>> deflated;   // columns still DEFLATEd, and where their bytes are
+    std::vector<std::string> actors; std::vector<std::array<u8, 32>> heads; std::vector<u32> headIdx;
+    std::vector<std::pair<u32, u32>> reps; DocCols dc{}; size_t arenaLen = 0;   // staged in the arena
+    std::vector<u64> clock; LoadedDoc doc;   // doc: what the engine keeps once the load has succeeded
+    size_t N = 0, S = 0; u32 serialMask = ALL_DOC_COLS; bool counted = false; RawRows raw{}; u64 maxOp = 0;   // rows, succ entries
+    LoadCall(const u8* b, size_t n) : buf(b), len(n), r(b, 8, (u32)n) {}
+  };
+  void loadDocument(const u8* buf, size_t len);   // the phases, in order:
+  void readContainer(LoadCall& l), inflateColumns(LoadCall& l), stageColumns(LoadCall& l), loadClock(LoadCall& l), countRows(LoadCall& l),
+       decodeDocColumns(LoadCall& l), finalizeRows(LoadCall& l), readUnknownOpColumns(LoadCall& l), commitLoad(LoadCall& l);
+  void ensureLoadRows(size_t n);
+  struct SaveCall {
+    size_t C, N, S, L, K;   // changes, rows, succ entries, loaded changes; the K = C - L later ones have their bytes in the arena
+    struct Col { u32 id; size_t off, len; }; std::vector<Col> changeCols, opCols;   // ranges of the encoder's output
+    HostClock t0;
+  };
+  void saveDocument(std::string& result);   // the phases, in order:
+  void saveChangeColumns(SaveCall& s), saveOpColumns(SaveCall& s); void packDocument(SaveCall& s, std::string& result);
+  // computeHashGraph's tables live as long as the call (they go back to the pool when it ends)
+  struct HistoryCall {
+    size_t L, N, S, A; DocRows d; HostClock t0;
+    DBuf<long long> cActor, cSeq, cMaxOp, cTime, cDepsNum, cExtra, depIdxV, scratchV; DBuf<u32> msgOff, msgLen, extraOff, extraLen, tmpOff, tmpLen, depsNum32, depBase, depIdx; size_t D = 0;
+    DBuf<u32> rankD, actorOfRank, repOff, repLen; int ctrBits = 0, idBits = 0;
+    DBuf<u64> idSorted, predKey, succKey, keyA, keyB, groupId, opId; size_t G = 0, numDel = 0, M = 0;
+    DBuf<u32> idRows, pairRow, valA, pairRowSorted, head, groupIdx, groupStart, groupRow, isDel, delSlot, opSrc, opPredStart, opPredNum, opOrder, opChange, predNumSorted, opPredBase;
+    DBuf<u64> opKey, chKey; DBuf<u32> changeOrder, actorStart, chOpStart, chNOps; size_t P = 0;
+    DBuf<u32> slotCnt, slotBase, uniq, uniqSlot, otherStart, slotVal; DBuf<u64> slotKey, other; size_t Q = 0, U = 0;
+    DBuf<u32> objA, keyAi, predA, outLen, outOff, depsAt, bodyAt, chOffD; DBuf<long long> keyDelta, predDelta; u64 T = 0;
+    DBuf<u32> listD; DBuf<u8> newHashes; std::vector<u8> isDep;
+    HistOpView view() { return HistOpView{d, opId.p, opSrc.p, opPredStart.p, opPredNum.p, opOrder.p, pairRowSorted.p, (u32)N}; }
+  };
+  void computeHashGraph();   // change history of a loaded document (history.cuh); the sections, in order:
+  void histChangeColumns(HistoryCall& h), histActorOrder(HistoryCall& h), histPredsAndDeletions(HistoryCall& h), histOpsToChanges(HistoryCall& h),
+       histActorTables(HistoryCall& h), histEncode(HistoryCall& h), histHashes(HistoryCall& h), histCheckHeads(HistoryCall& h), histCommit(HistoryCall& h);
 };
 
 }  // namespace amg

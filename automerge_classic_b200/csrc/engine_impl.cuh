@@ -68,9 +68,9 @@ inline void Engine::finishPatch(PatchOut& out) {
 
 // forgets the document but keeps every allocation (steady-state serving / benchmarking)
 inline void Engine::reset() {
-  sync(ctx); headIndexesUnknown = false; unknownCols.clear();
+  sync(ctx); loaded = LoadedDoc(); unknownCols.clear();
   arenaLen = 0; hostArena.len = 0; numApplied = 0; numRows = 0; numSucc = 0; dev_memset(ctx, succOff.p, 0, 4);
-  st = DocState(); changes.clear(); deflatedOriginal.clear(); loadedDoc.clear(); numLoaded = 0; historyRebuilt = 0; haveHashGraph = true;
+  st = DocState(); changes.clear(); deflatedOriginal.clear();
   queue.clear(); queueOriginal.clear(); rebuildActorTable();
 }
 
@@ -82,7 +82,7 @@ inline void Engine::applyChanges(const u8* const* bufs, const size_t* lens, size
   auto once = [&]() { ApplyCall a{bufs, lens, n, blob, offsets, isLocal, wantPatch}; applyChangesOnce(a, out); };
   try { once(); return; }
   catch (NeedHistory&) {}
-  catch (Error& e) { if (haveHashGraph || e.code != AMG_ERR_RANGE) throw; }
+  catch (Error& e) { if (loaded.haveHashGraph || e.code != AMG_ERR_RANGE) throw; }
   drop_peeks(ctx);
   computeHashGraph();
   out = PatchOut();
@@ -392,7 +392,7 @@ inline void Engine::runGate(ApplyCall& a) {
     a.appliedH.resize(B); a.primaryH.resize(B); a.appRankH.resize(B);
     d2h(ctx, a.appliedH.data(), applied.p, B); d2h(ctx, a.primaryH.data(), primary.p, B * 4); d2h(ctx, a.appRankH.data(), appRank.p, B * 4); sync(ctx);
   }
-  if (!haveHashGraph && a.numNew < B) throw NeedHistory{};   // a change waits for (or repeats) something older than the loaded heads
+  if (!loaded.haveHashGraph && a.numNew < B) throw NeedHistory{};   // a change waits for (or repeats) something older than the loaded heads
   // the queue after this call: every batch entry whose hash is still not applied (new.js:1569-1570, 1832)
   if (a.numNew < B) {
     a.needBatch(); a.finishInflate(*this);
@@ -738,7 +738,7 @@ inline void Engine::commit(ApplyCall& a) {
     fill32(doc.time.p, 0, a.N);
     for (auto& kv : a.unknownRows) unknownCols.byOp[kv.first] = std::move(kv.second);
     unknownCols.colIds.insert(a.unknownIds.begin(), a.unknownIds.end());
-    loadedDoc.clear(); numApplied += numNew; st = std::move(a.now);
+    loaded.bytes.clear(); numApplied += numNew; st = std::move(a.now);
     trace.mark("commit:state-swapped");
     rebuildActorTable();   // slots of actors registered in this call become permanent (first = 0)
     trace.mark("commit:actors-rebuilt");
@@ -1089,23 +1089,14 @@ inline void Engine::decodeHugeChanges(const RawRows& raw, size_t numLarge) {
     { ByteReader d(dir.data(), 0, (u32)dir.size()); u32 pos = h.dataOff;
       while (!d.done() && !d.err) { const u32 id = (u32)d.uleb(), l = (u32)d.uleb(); const int ix = col_index_of(id); if (ix >= 0) { cOff[ix] = pos; cLen[ix] = l; have[ix] = true; } pos += l; } }
     std::vector<u32> done(NCOLS, 0);
-    auto bytesOf = [&](int ix) { return arena.p + cOff[ix]; };
-    struct Plan { int col; u32* out; size_t cnt; };
-    const Plan plan[] = {{CX_OBJ_ACTOR, raw.objActor + rb, n}, {CX_OBJ_CTR, raw.objCtr + rb, n}, {CX_KEY_ACTOR, raw.keyActor + rb, n}, {CX_KEY_CTR, raw.keyCtr + rb, n},
-                         {CX_INSERT, raw.insert + rb, n}, {CX_ACTION, raw.action + rb, n}, {CX_VAL_LEN, raw.valLen + rb, n}, {CX_PRED_NUM, raw.predNum + rb, n},
-                         {CX_PRED_ACTOR, raw.predActor + rpb, np}, {CX_PRED_CTR, raw.predCtr + rpb, np}};
-    for (const Plan& pl : plan) {
-      if (!have[pl.col] || cLen[pl.col] == 0 || pl.cnt == 0) continue;   // absent / empty: the serial path fills the defaults
-      const u8* bytes = bytesOf(pl.col); const u32 len = cLen[pl.col]; bool ok = false;
-      switch (pl.col) {
-        case CX_OBJ_ACTOR: case CX_OBJ_CTR: case CX_KEY_ACTOR: case CX_ACTION: case CX_PRED_ACTOR: ok = parCols.toU32(bytes, len, pl.cnt, pl.out); break;
-        case CX_KEY_CTR: case CX_PRED_CTR: ok = parCols.deltaToU32(bytes, len, pl.cnt, pl.out); break;
-        case CX_INSERT: ok = parCols.boolean(bytes, len, pl.cnt, pl.out); break;
-        case CX_VAL_LEN: { u64 sum = 0; ok = parCols.lenColumn(bytes, len, pl.cnt, raw.valLen + rb, raw.valOff + rb, have[CX_VAL_RAW] ? cOff[CX_VAL_RAW] : 0, &sum) && sum <= (have[CX_VAL_RAW] ? cLen[CX_VAL_RAW] : 0); } break;
-        case CX_PRED_NUM: { u64 sum = 0; ok = parCols.countColumn(bytes, len, pl.cnt, raw.predNum + rb, raw.predOff + rb, &sum) && sum == np; if (ok && rpb) foreach(ctx, pl.cnt, PcAddBaseKernel{raw.predOff + rb, rpb}); } break;
-        default: break;
-      }
-      if (ok) { done[pl.col] = 1; any |= 1u << pl.col; }
+    for (int col = 0; col < NCOLS; col++) {
+      const size_t cnt = (col == CX_PRED_ACTOR || col == CX_PRED_CTR) ? np : n;
+      if (CX_PAR_KIND[col] == PK_NONE || !have[col] || cLen[col] == 0 || cnt == 0) continue;   // absent / empty: the serial path fills the defaults
+      u64 sum = 0;
+      bool ok = parCols.decode(CX_PAR_KIND[col], arena.p + cOff[col], cLen[col], cnt, cx_outputs(raw, col, rb, rpb, have[CX_VAL_RAW] ? cOff[CX_VAL_RAW] : 0, &sum));
+      if (ok && col == CX_VAL_LEN) ok = sum <= (have[CX_VAL_RAW] ? cLen[CX_VAL_RAW] : 0);
+      if (ok && col == CX_PRED_NUM) { ok = sum == np; if (ok && rpb) foreach(ctx, cnt, PcAddBaseKernel{raw.predOff + rb, rpb}); }
+      if (ok) { done[col] = 1; any |= 1u << col; }
     }
     h2d(ctx, hugeDone.p + k * NCOLS, done.data(), NCOLS * 4); sync(ctx);
     if (trace.live) fprintf(stderr, "amgpu decode: bulk change %u (%u ops, %u preds): columns expanded in parallel: mask %04x\n", c, n, np, any);
@@ -1146,166 +1137,184 @@ inline void Engine::benchDecode(int iters, float* msSha, float* msParse, float* 
 // loaded change - ops from the document rows and the deletions implied by their succ lists, preds, actor tables, canonical
 // column bytes - and its hash. Kernels: history.cuh. Nothing persistent is touched until the heads check has passed.
 inline void Engine::computeHashGraph() {
-  if (haveHashGraph) return;
+  if (loaded.haveHashGraph) return;
   if (!unknownCols.empty()) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: the change history of a loaded document that holds columns with unknown ids cannot be reconstructed");
-  const size_t L = numLoaded, N = numRows, S = numSucc, A = st.actorIds.size();
-  if (L == 0) { haveHashGraph = true; return; }
-  if (L >= (1u << 29) || N + S >= (1u << 30)) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: document too large for history reconstruction");
-  DocRows d = doc.view();
-  HostClock t0; auto hmark = [&](const char* what) { trace.print("history", what, t0); };
+  const size_t L = loaded.numChanges;
+  if (L == 0) { loaded.haveHashGraph = true; return; }
+  if (L >= (1u << 29) || numRows + numSucc >= (1u << 30)) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: document too large for history reconstruction");
+  HistoryCall h{L, numRows, numSucc, st.actorIds.size(), doc.view()};
   dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
-  // ---- 1. change metadata columns (the same decoders as save() after load())
-  DBuf<long long> cActor, cSeq, cMaxOp, cTime, cDepsNum, cExtra, depIdxV, scratchV; DBuf<u32> msgOff, msgLen, extraOff, extraLen, tmpOff, tmpLen, depsNum32, depBase, depIdx;
-  for (DBuf<long long>* b : {&cActor, &cSeq, &cMaxOp, &cTime, &cDepsNum, &cExtra, &scratchV}) b->ensure(ctx, L + 1);
-  for (DBuf<u32>* b : {&msgOff, &msgLen, &extraOff, &extraLen, &tmpOff, &tmpLen, &depsNum32}) b->ensure(ctx, L + 2);
-  depBase.ensure(ctx, L + 2);
-  auto decodeCol = [&](int kind, u32 id, size_t count, long long* out, u32* so, u32* sl) {
-    const HostChange& c = loadedCol(id);
-    if (count >= parDocMinRows && c.len > 0) {
-      const u8* bytes = arena.p + c.off; bool ok = false;
-      if (kind == LC_UINT) ok = parCols.toI64(bytes, c.len, false, count, out);
-      else if (kind == LC_DELTA) ok = parCols.deltaToI64(bytes, c.len, count, out);
-      else if (kind == LC_EXTRA_LEN) ok = parCols.extraLenColumn(bytes, c.len, count, out, so, sl, loadedCol(0x57).off);
-      if (ok) return;
-    }
-    if (count) foreach_warp(ctx, 1, LoadedColKernel{kind, arena.p, c.off, c.len, loadedCol(0x57).off, (u32)count, out, so, sl, nullptr});
-  };
-  decodeCol(LC_UINT, 0x01, L, cActor.p, tmpOff.p, tmpLen.p);
-  decodeCol(LC_DELTA, 0x03, L, cSeq.p, tmpOff.p, tmpLen.p);
-  decodeCol(LC_DELTA, 0x13, L, cMaxOp.p, tmpOff.p, tmpLen.p);
-  decodeCol(LC_DELTA, 0x23, L, cTime.p, tmpOff.p, tmpLen.p);
-  decodeCol(LC_STRING, 0x35, L, scratchV.p, msgOff.p, msgLen.p);
-  decodeCol(LC_UINT, 0x40, L, cDepsNum.p, tmpOff.p, tmpLen.p);
-  decodeCol(LC_EXTRA_LEN, 0x56, L, cExtra.p, extraOff.p, extraLen.p);
-  foreach(ctx, L, HistI64ToU32Kernel{cDepsNum.p, depsNum32.p});
-  scan_exclusive(ctx, scanTmp, depsNum32.p, depBase.p, L);
-  const size_t D = readU32(depBase.p + L);
-  depIdxV.ensure(ctx, D + 1); depIdx.ensure(ctx, D + 2);
-  decodeCol(LC_DELTA, 0x43, D, depIdxV.p, tmpOff.p, tmpLen.p);
-  if (D) foreach(ctx, D, HistI64ToU32Kernel{depIdxV.p, depIdx.p});
-  // ---- 2. actor order (hex string order = byte order), representatives
+  histChangeColumns(h); histActorOrder(h); histPredsAndDeletions(h); histOpsToChanges(h); histActorTables(h);
+  histEncode(h); histHashes(h); histCheckHeads(h); histCommit(h);
+}
+
+// Change metadata column k of the loaded document, `count` values: the parallel decoder when the history is long (it
+// declines what is not canonical), else LoadedColKernel.
+inline void Engine::decodeLoadedCol(int k, size_t count, long long* out, u32* strOff, u32* strLen) {
+  const HostChange& c = loaded.cols[k]; const u32 rawOff = loaded.cols[CC_EXTRA_RAW].off;
+  if (count >= parDocMinRows && c.len > 0 && parCols.decode(CHANGE_COLS[k].pk, arena.p + c.off, c.len, count, PcOut{nullptr, out, strOff, strLen, rawOff})) return;
+  foreach_warp(ctx, 1, LoadedColKernel{CHANGE_COLS[k].lc, arena.p, c.off, c.len, rawOff, (u32)count, out, strOff, strLen, nullptr});
+}
+
+// 1. change metadata columns (the same decoders as save() after load())
+inline void Engine::histChangeColumns(HistoryCall& h) {
+  const size_t L = h.L;
+  for (DBuf<long long>* b : {&h.cActor, &h.cSeq, &h.cMaxOp, &h.cTime, &h.cDepsNum, &h.cExtra, &h.scratchV}) b->ensure(ctx, L + 1);
+  for (DBuf<u32>* b : {&h.msgOff, &h.msgLen, &h.extraOff, &h.extraLen, &h.tmpOff, &h.tmpLen, &h.depsNum32}) b->ensure(ctx, L + 2);
+  h.depBase.ensure(ctx, L + 2);
+  decodeLoadedCol(CC_ACTOR, L, h.cActor.p, h.tmpOff.p, h.tmpLen.p);
+  decodeLoadedCol(CC_SEQ, L, h.cSeq.p, h.tmpOff.p, h.tmpLen.p);
+  decodeLoadedCol(CC_MAX_OP, L, h.cMaxOp.p, h.tmpOff.p, h.tmpLen.p);
+  decodeLoadedCol(CC_TIME, L, h.cTime.p, h.tmpOff.p, h.tmpLen.p);
+  decodeLoadedCol(CC_MESSAGE, L, h.scratchV.p, h.msgOff.p, h.msgLen.p);
+  decodeLoadedCol(CC_DEPS_NUM, L, h.cDepsNum.p, h.tmpOff.p, h.tmpLen.p);
+  decodeLoadedCol(CC_EXTRA_LEN, L, h.cExtra.p, h.extraOff.p, h.extraLen.p);
+  foreach(ctx, L, HistI64ToU32Kernel{h.cDepsNum.p, h.depsNum32.p});
+  scan_exclusive(ctx, scanTmp, h.depsNum32.p, h.depBase.p, L);
+  const size_t D = h.D = readU32(h.depBase.p + L);
+  h.depIdxV.ensure(ctx, D + 1); h.depIdx.ensure(ctx, D + 2);
+  if (D) { decodeLoadedCol(CC_DEPS_INDEX, D, h.depIdxV.p, h.tmpOff.p, h.tmpLen.p); foreach(ctx, D, HistI64ToU32Kernel{h.depIdxV.p, h.depIdx.p}); }
+}
+
+// 2. actor order (hex string order = byte order), representatives
+inline void Engine::histActorOrder(HistoryCall& h) {
+  const size_t A = h.A;
   std::vector<u32> order(A), rankH(A), repOffH(A), repLenH(A);
   for (size_t a = 0; a < A; a++) { order[a] = (u32)a; repOffH[a] = st.actorRep[a].first; repLenH[a] = st.actorRep[a].second; }
   std::sort(order.begin(), order.end(), [&](u32 x, u32 y) { return st.actorIds[x] < st.actorIds[y]; });
   for (size_t i = 0; i < A; i++) rankH[order[i]] = (u32)i;
-  DBuf<u32> rankD, actorOfRank, repOff, repLen;
-  for (DBuf<u32>* b : {&rankD, &actorOfRank, &repOff, &repLen}) b->ensure(ctx, A + 1);
-  h2d(ctx, rankD.p, rankH.data(), A * 4); h2d(ctx, actorOfRank.p, order.data(), A * 4); h2d(ctx, repOff.p, repOffH.data(), A * 4); h2d(ctx, repLen.p, repLenH.data(), A * 4);
-  const int ctrBits = bits_for(st.maxOp + 1), idBits = std::min(64, ctrBits + 16);
-  hmark("change columns decoded");
-  // ---- 3. (successor, predecessor) pairs -> pred lists and deletions
-  DBuf<u64> predKey, succKey, keyA, keyB, groupId, opId; DBuf<u32> pairRow, valA, pairRowSorted, head, groupIdx, groupStart, groupRow, isDel, delSlot, idRows;
-  DBuf<u64> idSorted; idSorted.ensure(ctx, N + 1); idRows.ensure(ctx, N + 1);
-  if (N) { foreach(ctx, N, HistIdKeyKernel{d, idSorted.p, idRows.p}); radix_sort_pairs(ctx, sortTmp, idSorted, idRows, N, 0, idBits); }
-  size_t G = 0, numDel = 0;
-  for (DBuf<u64>* b : {&predKey, &succKey, &keyA, &keyB}) b->ensure(ctx, S + 1);
-  for (DBuf<u32>* b : {&pairRow, &valA, &pairRowSorted, &head, &groupIdx}) b->ensure(ctx, S + 2);
+  for (DBuf<u32>* b : {&h.rankD, &h.actorOfRank, &h.repOff, &h.repLen}) b->ensure(ctx, A + 1);
+  h2d(ctx, h.rankD.p, rankH.data(), A * 4); h2d(ctx, h.actorOfRank.p, order.data(), A * 4); h2d(ctx, h.repOff.p, repOffH.data(), A * 4); h2d(ctx, h.repLen.p, repLenH.data(), A * 4);
+  h.ctrBits = bits_for(st.maxOp + 1); h.idBits = std::min(64, h.ctrBits + 16);
+  trace.print("history", "change columns decoded", h.t0);
+}
+
+// 3. (successor, predecessor) pairs -> pred lists and deletions
+inline void Engine::histPredsAndDeletions(HistoryCall& h) {
+  const size_t N = h.N, S = h.S;
+  h.idSorted.ensure(ctx, N + 1); h.idRows.ensure(ctx, N + 1);
+  if (N) { foreach(ctx, N, HistIdKeyKernel{h.d, h.idSorted.p, h.idRows.p}); radix_sort_pairs(ctx, sortTmp, h.idSorted, h.idRows, N, 0, h.idBits); }
+  for (DBuf<u64>* b : {&h.predKey, &h.succKey, &h.keyA, &h.keyB}) b->ensure(ctx, S + 1);
+  for (DBuf<u32>* b : {&h.pairRow, &h.valA, &h.pairRowSorted, &h.head, &h.groupIdx}) b->ensure(ctx, S + 2);
   if (S) {
-    foreach(ctx, N, HistPairKernel{d, succOff.p, succ.p, rankD.p, predKey.p, succKey.p, pairRow.p});
-    foreach(ctx, S, HistIotaKernel{valA.p});
-    d2d(ctx, keyA.p, predKey.p, S * 8);
-    radix_sort_pairs(ctx, sortTmp, keyA, valA, S, 0, idBits);                 // by predecessor (counter, actor order) ...
-    foreach(ctx, S, HistGatherKeyKernel{succKey.p, valA.p, keyB.p});
-    radix_sort_pairs(ctx, sortTmp, keyB, valA, S, 0, idBits);                 // ... then, stably, by successor id
-    foreach(ctx, S, HistGatherU32Kernel{pairRow.p, valA.p, pairRowSorted.p});
-    foreach(ctx, S, HistGroupHeadKernel{keyB.p, head.p});
-    scan_exclusive(ctx, scanTmp, head.p, groupIdx.p, S);
-    G = readU32(groupIdx.p + S);
+    foreach(ctx, N, HistPairKernel{h.d, succOff.p, succ.p, h.rankD.p, h.predKey.p, h.succKey.p, h.pairRow.p});
+    foreach(ctx, S, HistIotaKernel{h.valA.p});
+    d2d(ctx, h.keyA.p, h.predKey.p, S * 8);
+    radix_sort_pairs(ctx, sortTmp, h.keyA, h.valA, S, 0, h.idBits);                 // by predecessor (counter, actor order) ...
+    foreach(ctx, S, HistGatherKeyKernel{h.succKey.p, h.valA.p, h.keyB.p});
+    radix_sort_pairs(ctx, sortTmp, h.keyB, h.valA, S, 0, h.idBits);                 // ... then, stably, by successor id
+    foreach(ctx, S, HistGatherU32Kernel{h.pairRow.p, h.valA.p, h.pairRowSorted.p});
+    foreach(ctx, S, HistGroupHeadKernel{h.keyB.p, h.head.p});
+    scan_exclusive(ctx, scanTmp, h.head.p, h.groupIdx.p, S);
+    h.G = readU32(h.groupIdx.p + S);
   }
-  for (DBuf<u32>* b : {&groupStart, &groupRow, &isDel, &delSlot}) b->ensure(ctx, G + 2);
-  groupId.ensure(ctx, G + 1);
+  const size_t G = h.G;
+  for (DBuf<u32>* b : {&h.groupStart, &h.groupRow, &h.isDel, &h.delSlot}) b->ensure(ctx, G + 2);
+  h.groupId.ensure(ctx, G + 1);
   if (G) {
-    foreach(ctx, S, HistGroupKernel{head.p, groupIdx.p, keyB.p, (u32)S, idSorted.p, idRows.p, (u32)N, groupStart.p, groupId.p, groupRow.p, isDel.p});
-    scan_exclusive(ctx, scanTmp, isDel.p, delSlot.p, G);
-    numDel = readU32(delSlot.p + G);
+    foreach(ctx, S, HistGroupKernel{h.head.p, h.groupIdx.p, h.keyB.p, (u32)S, h.idSorted.p, h.idRows.p, (u32)N, h.groupStart.p, h.groupId.p, h.groupRow.p, h.isDel.p});
+    scan_exclusive(ctx, scanTmp, h.isDel.p, h.delSlot.p, G);
+    h.numDel = readU32(h.delSlot.p + G);
   }
-  const size_t M = N + numDel;
-  DBuf<u32> opSrc, opPredStart, opPredNum, opOrder, opChange, predNumSorted, opPredBase;
-  opId.ensure(ctx, M + 1); for (DBuf<u32>* b : {&opSrc, &opPredStart, &opPredNum, &opOrder, &opChange, &predNumSorted}) b->ensure(ctx, M + 2);
-  opPredBase.ensure(ctx, M + 3);
-  if (N) foreach(ctx, N, HistRowOpKernel{d, opId.p, opSrc.p, opPredStart.p, opPredNum.p});
-  if (G) foreach(ctx, G, HistGroupOpKernel{groupStart.p, groupId.p, groupRow.p, isDel.p, delSlot.p, pairRowSorted.p, (u32)G, (u32)S, (u32)N, opId.p, opSrc.p, opPredStart.p, opPredNum.p});
-  hmark("preds and deletions");
-  // ---- 4. ops by (actor, counter); changes by (actor, seq); every op finds its change
-  DBuf<u64> opKey, chKey; opKey.ensure(ctx, M + 1); chKey.ensure(ctx, L + 1);
-  DBuf<u32> changeOrder, actorStart, chOpStart, chNOps; changeOrder.ensure(ctx, L + 1); actorStart.ensure(ctx, A + 2); chOpStart.ensure(ctx, L + 2); chNOps.ensure(ctx, L + 2);
-  if (M) { foreach(ctx, M, HistOpKeyKernel{opId.p, opKey.p, opOrder.p}); radix_sort_pairs(ctx, sortTmp, opKey, opOrder, M, 0, ctrBits); radix_sort_pairs(ctx, sortTmp, opKey, opOrder, M, 48, 64); }
-  foreach(ctx, L, HistChangeKeyKernel{cActor.p, cSeq.p, chKey.p, changeOrder.p});
-  radix_sort_pairs(ctx, sortTmp, chKey, changeOrder, L, 0, 40); radix_sort_pairs(ctx, sortTmp, chKey, changeOrder, L, 40, 57);
-  foreach(ctx, A + 1, HistLowerBoundKernel{chKey.p, (u32)L, 40, actorStart.p});
-  dev_memset(ctx, chOpStart.p, 0, (L + 1) * 4); dev_memset(ctx, chNOps.p, 0, (L + 1) * 4);
+  const size_t M = h.M = N + h.numDel;
+  h.opId.ensure(ctx, M + 1); for (DBuf<u32>* b : {&h.opSrc, &h.opPredStart, &h.opPredNum, &h.opOrder, &h.opChange, &h.predNumSorted}) b->ensure(ctx, M + 2);
+  h.opPredBase.ensure(ctx, M + 3);
+  if (N) foreach(ctx, N, HistRowOpKernel{h.d, h.opId.p, h.opSrc.p, h.opPredStart.p, h.opPredNum.p});
+  if (G) foreach(ctx, G, HistGroupOpKernel{h.groupStart.p, h.groupId.p, h.groupRow.p, h.isDel.p, h.delSlot.p, h.pairRowSorted.p, (u32)G, (u32)S, (u32)N, h.opId.p, h.opSrc.p, h.opPredStart.p, h.opPredNum.p});
+  trace.print("history", "preds and deletions", h.t0);
+}
+
+// 4. ops by (actor, counter); changes by (actor, seq); every op finds its change
+inline void Engine::histOpsToChanges(HistoryCall& h) {
+  const size_t L = h.L, A = h.A, M = h.M;
+  h.opKey.ensure(ctx, M + 1); h.chKey.ensure(ctx, L + 1);
+  h.changeOrder.ensure(ctx, L + 1); h.actorStart.ensure(ctx, A + 2); h.chOpStart.ensure(ctx, L + 2); h.chNOps.ensure(ctx, L + 2);
+  if (M) { foreach(ctx, M, HistOpKeyKernel{h.opId.p, h.opKey.p, h.opOrder.p}); radix_sort_pairs(ctx, sortTmp, h.opKey, h.opOrder, M, 0, h.ctrBits); radix_sort_pairs(ctx, sortTmp, h.opKey, h.opOrder, M, 48, 64); }
+  foreach(ctx, L, HistChangeKeyKernel{h.cActor.p, h.cSeq.p, h.chKey.p, h.changeOrder.p});
+  radix_sort_pairs(ctx, sortTmp, h.chKey, h.changeOrder, L, 0, 40); radix_sort_pairs(ctx, sortTmp, h.chKey, h.changeOrder, L, 40, 57);
+  foreach(ctx, A + 1, HistLowerBoundKernel{h.chKey.p, (u32)L, 40, h.actorStart.p});
+  dev_memset(ctx, h.chOpStart.p, 0, (L + 1) * 4); dev_memset(ctx, h.chNOps.p, 0, (L + 1) * 4);
   if (M) {
-    foreach(ctx, M, HistAssignKernel{opKey.p, actorStart.p, changeOrder.p, cMaxOp.p, (u32)A, numApplied == L ? 1 : 0, opChange.p, errWord.p});
-    foreach(ctx, M, HistChangeStartKernel{opChange.p, chOpStart.p});
-    foreach(ctx, M, HistChangeCountKernel{opChange.p, chNOps.p});
-    foreach(ctx, M, HistCheckIdsKernel{opKey.p, opChange.p, chOpStart.p, chNOps.p, cMaxOp.p, errWord.p});
-    foreach(ctx, M, HistPredNumSortedKernel{opPredNum.p, opOrder.p, predNumSorted.p});
-    scan_exclusive(ctx, scanTmp, predNumSorted.p, opPredBase.p, M);
-  } else dev_memset(ctx, opPredBase.p, 0, 8);
-  const size_t P = M ? readU32(opPredBase.p + M) : 0;
+    foreach(ctx, M, HistAssignKernel{h.opKey.p, h.actorStart.p, h.changeOrder.p, h.cMaxOp.p, (u32)A, numApplied == L ? 1 : 0, h.opChange.p, errWord.p});
+    foreach(ctx, M, HistChangeStartKernel{h.opChange.p, h.chOpStart.p});
+    foreach(ctx, M, HistChangeCountKernel{h.opChange.p, h.chNOps.p});
+    foreach(ctx, M, HistCheckIdsKernel{h.opKey.p, h.opChange.p, h.chOpStart.p, h.chNOps.p, h.cMaxOp.p, errWord.p});
+    foreach(ctx, M, HistPredNumSortedKernel{h.opPredNum.p, h.opOrder.p, h.predNumSorted.p});
+    scan_exclusive(ctx, scanTmp, h.predNumSorted.p, h.opPredBase.p, M);
+  } else dev_memset(ctx, h.opPredBase.p, 0, 8);
+  h.P = M ? readU32(h.opPredBase.p + M) : 0;
   checkErr();
-  hmark("ops assigned to changes");
-  // ---- 5. the other actors of every change
-  HistOpView view{d, opId.p, opSrc.p, opPredStart.p, opPredNum.p, opOrder.p, pairRowSorted.p, (u32)N};
-  DBuf<u32> slotCnt, slotBase, uniq, uniqSlot, otherStart; DBuf<u64> slotKey, other; DBuf<u32> slotVal;
-  slotCnt.ensure(ctx, M + 2); slotBase.ensure(ctx, M + 3); otherStart.ensure(ctx, L + 3);
-  size_t Q = 0, U = 0;
-  if (M) { foreach(ctx, M, HistActorSlotCountKernel{view, slotCnt.p}); scan_exclusive(ctx, scanTmp, slotCnt.p, slotBase.p, M); Q = readU32(slotBase.p + M); }
-  slotKey.ensure(ctx, Q + 1); slotVal.ensure(ctx, Q + 1); uniq.ensure(ctx, Q + 2); uniqSlot.ensure(ctx, Q + 3);
+  trace.print("history", "ops assigned to changes", h.t0);
+}
+
+// 5. the other actors of every change
+inline void Engine::histActorTables(HistoryCall& h) {
+  const size_t L = h.L, M = h.M; const HistOpView view = h.view();
+  h.slotCnt.ensure(ctx, M + 2); h.slotBase.ensure(ctx, M + 3); h.otherStart.ensure(ctx, L + 3);
+  if (M) { foreach(ctx, M, HistActorSlotCountKernel{view, h.slotCnt.p}); scan_exclusive(ctx, scanTmp, h.slotCnt.p, h.slotBase.p, M); h.Q = readU32(h.slotBase.p + M); }
+  const size_t Q = h.Q;
+  h.slotKey.ensure(ctx, Q + 1); h.slotVal.ensure(ctx, Q + 1); h.uniq.ensure(ctx, Q + 2); h.uniqSlot.ensure(ctx, Q + 3);
   if (Q) {
-    foreach(ctx, M, HistActorPairKernel{view, slotBase.p, opChange.p, cActor.p, rankD.p, slotKey.p});
-    foreach(ctx, Q, HistIotaKernel{slotVal.p});
-    radix_sort_pairs(ctx, sortTmp, slotKey, slotVal, Q, 0, 64);
-    foreach(ctx, Q, HistUniqueKernel{slotKey.p, uniq.p});
-    scan_exclusive(ctx, scanTmp, uniq.p, uniqSlot.p, Q);
-    U = readU32(uniqSlot.p + Q);
+    foreach(ctx, M, HistActorPairKernel{view, h.slotBase.p, h.opChange.p, h.cActor.p, h.rankD.p, h.slotKey.p});
+    foreach(ctx, Q, HistIotaKernel{h.slotVal.p});
+    radix_sort_pairs(ctx, sortTmp, h.slotKey, h.slotVal, Q, 0, 64);
+    foreach(ctx, Q, HistUniqueKernel{h.slotKey.p, h.uniq.p});
+    scan_exclusive(ctx, scanTmp, h.uniq.p, h.uniqSlot.p, Q);
+    h.U = readU32(h.uniqSlot.p + Q);
   }
-  other.ensure(ctx, U + 1);
-  if (U) foreach(ctx, Q, HistOtherFillKernel{slotKey.p, uniq.p, uniqSlot.p, other.p});
-  foreach(ctx, L + 1, HistLowerBoundKernel{other.p, (u32)U, 16, otherStart.p});
-  hmark("actor tables");
-  // ---- 6. local actor indexes and delta values, then the bytes (two passes)
-  DBuf<u32> objA, keyAi, predA, outLen, outOff, depsAt, bodyAt, chOffD; DBuf<long long> keyDelta, predDelta;
-  objA.ensure(ctx, M + 1); keyAi.ensure(ctx, M + 1); keyDelta.ensure(ctx, M + 1); predA.ensure(ctx, P + 1); predDelta.ensure(ctx, P + 1);
-  for (DBuf<u32>* b : {&outLen, &depsAt, &bodyAt, &chOffD}) b->ensure(ctx, L + 2);
-  outOff.ensure(ctx, L + 3);
-  HistChanges hc{cActor.p, cSeq.p, cMaxOp.p, cTime.p, msgOff.p, msgLen.p, cDepsNum.p, extraOff.p, extraLen.p};
-  foreach(ctx, L, HistPrepKernel{view, hc, chOpStart.p, chNOps.p, opPredBase.p, other.p, otherStart.p, rankD.p, objA.p, keyAi.p, keyDelta.p, predA.p, predDelta.p});
-  HistEncodeKernel enc{0, view, hc, arena.p, chOpStart.p, chNOps.p, opPredBase.p, (u32)M, (u32)P, other.p, otherStart.p, repOff.p, repLen.p, actorOfRank.p,
-                       objA.p, keyAi.p, keyDelta.p, predA.p, predDelta.p, outLen.p, outOff.p, nullptr, 0, depsAt.p, bodyAt.p};
+  h.other.ensure(ctx, h.U + 1);
+  if (h.U) foreach(ctx, Q, HistOtherFillKernel{h.slotKey.p, h.uniq.p, h.uniqSlot.p, h.other.p});
+  foreach(ctx, L + 1, HistLowerBoundKernel{h.other.p, (u32)h.U, 16, h.otherStart.p});
+  trace.print("history", "actor tables", h.t0);
+}
+
+// 6. local actor indexes and delta values, then the bytes (two passes)
+inline void Engine::histEncode(HistoryCall& h) {
+  const size_t L = h.L, M = h.M, P = h.P; const HistOpView view = h.view();
+  h.objA.ensure(ctx, M + 1); h.keyAi.ensure(ctx, M + 1); h.keyDelta.ensure(ctx, M + 1); h.predA.ensure(ctx, P + 1); h.predDelta.ensure(ctx, P + 1);
+  for (DBuf<u32>* b : {&h.outLen, &h.depsAt, &h.bodyAt, &h.chOffD}) b->ensure(ctx, L + 2);
+  h.outOff.ensure(ctx, L + 3);
+  HistChanges hc{h.cActor.p, h.cSeq.p, h.cMaxOp.p, h.cTime.p, h.msgOff.p, h.msgLen.p, h.cDepsNum.p, h.extraOff.p, h.extraLen.p};
+  foreach(ctx, L, HistPrepKernel{view, hc, h.chOpStart.p, h.chNOps.p, h.opPredBase.p, h.other.p, h.otherStart.p, h.rankD.p, h.objA.p, h.keyAi.p, h.keyDelta.p, h.predA.p, h.predDelta.p});
+  HistEncodeKernel enc{0, view, hc, arena.p, h.chOpStart.p, h.chNOps.p, h.opPredBase.p, (u32)M, (u32)P, h.other.p, h.otherStart.p, h.repOff.p, h.repLen.p, h.actorOfRank.p,
+                       h.objA.p, h.keyAi.p, h.keyDelta.p, h.predA.p, h.predDelta.p, h.outLen.p, h.outOff.p, nullptr, 0, h.depsAt.p, h.bodyAt.p};
   foreach(ctx, L, enc);
-  scan_exclusive(ctx, scanTmp, outLen.p, outOff.p, L);
-  excl64.ensure(ctx, L + 2); scan_exclusive64(ctx, scanTmp, ParColumnDecoder::PcDeltaInputU32{outLen.p}, excl64.p, L);
-  u64 tot64 = 0; u32 lastLen = 0; d2h(ctx, &tot64, excl64.p + L - 1, 8); d2h(ctx, &lastLen, outLen.p + L - 1, 4); sync(ctx);
-  const u64 T = tot64 + lastLen;
+  scan_exclusive(ctx, scanTmp, h.outLen.p, h.outOff.p, L);
+  excl64.ensure(ctx, L + 2); scan_exclusive64(ctx, scanTmp, ParColumnDecoder::PcDeltaInputU32{h.outLen.p}, excl64.p, L);
+  u64 tot64 = 0; u32 lastLen = 0; d2h(ctx, &tot64, excl64.p + L - 1, 8); d2h(ctx, &lastLen, h.outLen.p + L - 1, 4); sync(ctx);
+  const u64 T = h.T = tot64 + lastLen;
   if ((u64)arenaLen + T + 64 >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: change arena limited to 4 GiB per document");
   arena.ensure(ctx, arenaLen + T + 64, arenaLen);
   enc.pass = 1; enc.arena = arena.p; enc.outArena = arena.p; enc.outBase = (u32)arenaLen;
   foreach(ctx, L, enc);
-  foreach(ctx, L, HistChOffKernel{outOff.p, (u32)arenaLen, chOffD.p});
+  foreach(ctx, L, HistChOffKernel{h.outOff.p, (u32)arenaLen, h.chOffD.p});
   checkErr();
-  hmark("changes encoded");
-  // ---- 7. dependency levels (host: one pass over the dependency indexes), hashes level by level
+  trace.print("history", "changes encoded", h.t0);
+}
+
+// 7. dependency levels (host: one pass over the dependency indexes), hashes level by level
+inline void Engine::histHashes(HistoryCall& h) {
+  const size_t L = h.L, D = h.D;
   std::vector<u32> depsNumH(L), depBaseH(L + 1), depIdxH(D), level(L), list(L);
-  d2h(ctx, depsNumH.data(), depsNum32.p, L * 4); d2h(ctx, depBaseH.data(), depBase.p, (L + 1) * 4); if (D) d2h(ctx, depIdxH.data(), depIdx.p, D * 4); sync(ctx);
-  u32 maxLevel = 0; std::vector<u8> isDep(L, 0);
+  d2h(ctx, depsNumH.data(), h.depsNum32.p, L * 4); d2h(ctx, depBaseH.data(), h.depBase.p, (L + 1) * 4); if (D) d2h(ctx, depIdxH.data(), h.depIdx.p, D * 4); sync(ctx);
+  u32 maxLevel = 0; h.isDep.assign(L, 0);
   for (size_t k = 0; k < L; k++) {
     u32 lv = 0;
-    for (u32 i = 0; i < depsNumH[k]; i++) { const u32 di = depIdxH[depBaseH[k] + i]; if (di >= k) throw Error(AMG_ERR_RANGE, "No hash for index " + std::to_string(di) + " while processing index " + std::to_string(k)); lv = std::max(lv, level[di] + 1); isDep[di] = 1; }
+    for (u32 i = 0; i < depsNumH[k]; i++) { const u32 di = depIdxH[depBaseH[k] + i]; if (di >= k) throw Error(AMG_ERR_RANGE, "No hash for index " + std::to_string(di) + " while processing index " + std::to_string(k)); lv = std::max(lv, level[di] + 1); h.isDep[di] = 1; }
     level[k] = lv; maxLevel = std::max(maxLevel, lv);
   }
   std::vector<u32> levelStart(maxLevel + 2, 0);
   for (size_t k = 0; k < L; k++) levelStart[level[k] + 1]++;
   for (u32 l = 0; l <= maxLevel; l++) levelStart[l + 1] += levelStart[l];
   { std::vector<u32> at(levelStart.begin(), levelStart.end() - 1); for (size_t k = 0; k < L; k++) list[at[level[k]]++] = (u32)k; }
-  DBuf<u32> listD; listD.ensure(ctx, L + 1); h2d(ctx, listD.p, list.data(), L * 4);
-  DBuf<u8> newHashes; newHashes.ensure(ctx, L * 32 + 64); d2d(ctx, newHashes.p, hashes.p, L * 32);   // scratch copy: committed only after the heads check
-  {
-    const HistHashKernel hk{listD.p, arena.p, chOffD.p, outLen.p, depsAt.p, bodyAt.p, cDepsNum.p, depBase.p, depIdx.p, (u32)L, newHashes.p, errWord.p};
-    auto wide = [&](u32 l) { HistHashKernel k = hk; k.list = listD.p + levelStart[l]; const size_t cnt = levelStart[l + 1] - levelStart[l]; if (cnt) foreach(ctx, cnt, k); };
+  h.listD.ensure(ctx, L + 1); h2d(ctx, h.listD.p, list.data(), L * 4);
+  h.newHashes.ensure(ctx, L * 32 + 64); d2d(ctx, h.newHashes.p, hashes.p, L * 32);   // scratch copy: committed only after the heads check
+  const HistHashKernel hk{h.listD.p, arena.p, h.chOffD.p, h.outLen.p, h.depsAt.p, h.bodyAt.p, h.cDepsNum.p, h.depBase.p, h.depIdx.p, (u32)L, h.newHashes.p, errWord.p};
+  auto wide = [&](u32 l) { HistHashKernel k = hk; k.list = h.listD.p + levelStart[l]; const size_t cnt = levelStart[l + 1] - levelStart[l]; if (cnt) foreach(ctx, cnt, k); };
 #ifdef AMG_EMU
-    for (u32 l = 0; l <= maxLevel; l++) wide(l);
+  for (u32 l = 0; l <= maxLevel; l++) wide(l);
 #else
+  {
     DBuf<u32> levelStartD; levelStartD.ensure(ctx, levelStart.size() + 1); h2d(ctx, levelStartD.p, levelStart.data(), levelStart.size() * 4);
     const u32 kNarrow = 1024;   // levels up to this many changes are walked by one CTA (k_hist_hash_chain); wider ones get their own launch
     for (u32 l = 0; l <= maxLevel;) {
@@ -1316,44 +1325,50 @@ inline void Engine::computeHashGraph() {
       l = r;
     }
     sync(ctx);   // levelStartD is a local
+  }
 #endif
-  }
   checkErr();
-  hmark("hashes (all levels)");
-  // ---- 8. heads: the changes nobody depends on must be exactly the document's heads (columnar.js:968-980)
-  {
-    size_t nHeads = 0; for (size_t k = 0; k < L; k++) if (!isDep[k]) nHeads++;
-    bool ok = numApplied != L || nHeads == st.heads.size();   // (changes applied after the load have moved the heads)
-    std::vector<std::array<u8, 32>> got(st.heads.size());
-    if (headIndexesUnknown) {   // loaded without head indexes: the heads are the changes nobody depends on, matched by hash
-      if (numApplied != L) throw Error(AMG_ERR_INTERNAL, "amgpu: head indexes must be resolved right after the load");
-      std::vector<u32> cand; for (size_t k = 0; k < L; k++) if (!isDep[k]) cand.push_back((u32)k);
-      ok = cand.size() == st.heads.size();
-      std::vector<std::array<u8, 32>> ch(cand.size());
-      if (ok) { for (size_t i = 0; i < cand.size(); i++) d2h(ctx, ch[i].data(), newHashes.p + (size_t)cand[i] * 32, 32); sync(ctx); }
-      for (size_t i = 0; i < st.heads.size() && ok; i++) {
-        size_t j = 0; while (j < cand.size() && ch[j] != st.heads[i]) j++;
-        if (j == cand.size()) ok = false; else st.headIdx[i] = cand[j];
-      }
-      if (ok) headIndexesUnknown = false;
-    } else if (numApplied == L) {
-      for (size_t i = 0; i < st.heads.size(); i++) d2h(ctx, got[i].data(), newHashes.p + (size_t)st.headIdx[i] * 32, 32);
-      sync(ctx);
-      for (size_t i = 0; i < st.heads.size() && ok; i++) if (isDep[st.headIdx[i]] || got[i] != st.heads[i]) ok = false;
+  trace.print("history", "hashes (all levels)", h.t0);
+}
+
+// 8. heads: the changes nobody depends on must be exactly the document's heads (columnar.js:968-980)
+inline void Engine::histCheckHeads(HistoryCall& h) {
+  const size_t L = h.L;
+  size_t nHeads = 0; for (size_t k = 0; k < L; k++) if (!h.isDep[k]) nHeads++;
+  bool ok = numApplied != L || nHeads == st.heads.size();   // (changes applied after the load have moved the heads)
+  std::vector<std::array<u8, 32>> got(st.heads.size());
+  if (loaded.headIndexesUnknown) {   // loaded without head indexes: the heads are the changes nobody depends on, matched by hash
+    if (numApplied != L) throw Error(AMG_ERR_INTERNAL, "amgpu: head indexes must be resolved right after the load");
+    std::vector<u32> cand; for (size_t k = 0; k < L; k++) if (!h.isDep[k]) cand.push_back((u32)k);
+    ok = cand.size() == st.heads.size();
+    std::vector<std::array<u8, 32>> ch(cand.size());
+    if (ok) { for (size_t i = 0; i < cand.size(); i++) d2h(ctx, ch[i].data(), h.newHashes.p + (size_t)cand[i] * 32, 32); sync(ctx); }
+    for (size_t i = 0; i < st.heads.size() && ok; i++) {
+      size_t j = 0; while (j < cand.size() && ch[j] != st.heads[i]) j++;
+      if (j == cand.size()) ok = false; else st.headIdx[i] = cand[j];
     }
-    if (!ok) throw Error(AMG_ERR_RANGE, "Mismatched heads hashes: the document's heads are not the hashes of its reconstructed changes");
+    if (ok) loaded.headIndexesUnknown = false;
+  } else if (numApplied == L) {
+    for (size_t i = 0; i < st.heads.size(); i++) d2h(ctx, got[i].data(), h.newHashes.p + (size_t)st.headIdx[i] * 32, 32);
+    sync(ctx);
+    for (size_t i = 0; i < st.heads.size() && ok; i++) if (h.isDep[st.headIdx[i]] || got[i] != st.heads[i]) ok = false;
   }
-  hmark("heads checked");
-  // ---- 9. commit: bytes into the arena and its host mirror, hashes, change table
+  if (!ok) throw Error(AMG_ERR_RANGE, "Mismatched heads hashes: the document's heads are not the hashes of its reconstructed changes");
+  trace.print("history", "heads checked", h.t0);
+}
+
+// 9. commit: bytes into the arena and its host mirror, hashes, change table
+inline void Engine::histCommit(HistoryCall& h) {
+  const size_t L = h.L; const u64 T = h.T;
   if (hostArena.size() == arenaLen) {   // the mirror is complete: keep it complete (otherwise it is fetched when asked for)
     hostArena.resize(arenaLen + T);
     if (T) d2h(ctx, hostArena.data() + arenaLen, arena.p + arenaLen, T);
   }
-  d2d(ctx, hashes.p, newHashes.p, L * 32);
-  std::vector<u32> offH(L), lenH(L); d2h(ctx, offH.data(), chOffD.p, L * 4); d2h(ctx, lenH.data(), outLen.p, L * 4); sync(ctx);
+  d2d(ctx, hashes.p, h.newHashes.p, L * 32);
+  std::vector<u32> offH(L), lenH(L); d2h(ctx, offH.data(), h.chOffD.p, L * 4); d2h(ctx, lenH.data(), h.outLen.p, L * 4); sync(ctx);
   for (size_t k = 0; k < L; k++) changes[k] = HostChange{offH[k], lenH[k]};
-  arenaLen += T; haveHashGraph = true; historyRebuilt = L;
-  hmark("committed");
+  arenaLen += T; loaded.haveHashGraph = true; loaded.historyRebuilt = L;
+  trace.print("history", "committed", h.t0);
 }
 
 // Parity hook: one document column through the parallel or the serial decoder (include/amgpu.h)
@@ -1363,12 +1378,10 @@ inline int Engine::debugDecodeColumn(const u8* bytes, size_t len, int kind, size
   colBytes.ensure(ctx, len + 64); dev_memset(ctx, colBytes.p, 0, len + 64); if (len) h2d(ctx, colBytes.p, bytes, len);
   outD.ensure(ctx, n + 1); tmp.ensure(ctx, n + 1);
   if (parallel) {
-    bool ok = false;
-    if (kind == 0) ok = parCols.toI64(colBytes.p, len, false, n, outD.p);
-    else if (kind == 1) ok = parCols.toI64(colBytes.p, len, true, n, outD.p);
-    else if (kind == 2) ok = parCols.deltaToI64(colBytes.p, len, n, outD.p);
-    else { ok = parCols.boolean(colBytes.p, len, n, tmp.p); if (ok && n) foreach(ctx, n, U32ToI64Kernel{tmp.p, outD.p}); }
+    static const int PK[4] = {PK_UINT, PK_INT, PK_DELTA, PK_BOOL};   // kind 3 (boolean) decodes into u32 rows, widened below
+    const bool ok = parCols.decode(PK[kind], colBytes.p, len, n, kind == 3 ? PcOut{tmp.p} : PcOut{nullptr, outD.p});
     if (!ok) { sync(ctx); return 1; }
+    if (kind == 3 && n) foreach(ctx, n, U32ToI64Kernel{tmp.p, outD.p});
   } else {
     dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
     foreach_warp(ctx, 1, DebugColumnKernel{kind, colBytes.p, (u32)len, (u32)n, outD.p, tmp.p, errWord.p});
@@ -1399,7 +1412,6 @@ inline void Engine::decodeRaw(const u8* blob, const u64* offsets, size_t n, u8* 
   if (decodeOverflowed(tot)) { runDecodeTiles(ar.p, n, staged.size()); readWords({{decTotalsPtr(), 4}, {decTotalsPtr() + 1, 4}, {decTotalsPtr() + 2, 4}, {decTotalsPtr() + 3, 4}}, dst); }
   checkErr();
   const size_t M = tot[0];
-  DBuf<u32>* cols[12] = {&r_objActor, &r_objCtr, &r_keyActor, &r_keyCtr, &r_keyStrOff, &r_keyStrLen, &r_insert, &r_action, &r_valLen, &r_valOff, &r_predNum, &r_predOff};
   RawRows raw = rawRows();
   if (tot[3] & 1u) {
     largeFlag.ensure(ctx, n + 1); largeSlot.ensure(ctx, n + 2); largeList.ensure(ctx, n + 1);
@@ -1434,105 +1446,106 @@ inline void host_sha256(const u8* data, size_t len, u8 out[32]) { amg_host_sha25
 // on the device (encode.cuh); the container (column directory, DEFLATE of columns >= 256 bytes, checksum) is assembled
 // on the host, as the reference does.
 inline void Engine::saveDocument(std::string& result) {
-  if (!loadedDoc.empty()) { result = loadedDoc; return; }   // unchanged since Backend.load (new.js:2034)
+  if (!loaded.bytes.empty()) { result = loaded.bytes; return; }   // unchanged since Backend.load (new.js:2034)
   if (!encoder) encoder.reset(new ColumnEncoder(ctx, scanTmp));
-  ColumnEncoder& enc = *encoder; enc.outLen = 0;
-  HostClock t0; auto smark = [&](const char* what) { trace.print("save", what, t0); };
-  struct Col { u32 id; size_t off, len; };
-  std::vector<Col> changeCols, opCols;
-  auto add = [&](std::vector<Col>& cols, u32 id, size_t len) { cols.push_back({id, enc.outLen - len, len}); };
-  const size_t C = numApplied, N = numRows, S = numSucc, L = numLoaded, K = C - L;   // K changes have their bytes in the arena
+  encoder->outLen = 0;
+  SaveCall s{numApplied, numRows, numSucc, loaded.numChanges, numApplied - loaded.numChanges};
   dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
-  saveVals.ensure(ctx, std::max(std::max(C, N), S) + 2);
-  // ---- change metadata (new.js:1680-1692 appendChange); the first L rows come from the loaded document's own columns
-  if (C > 0) {
-    u32 totalDeps = 0, loadedDeps = 0;
-    if (K > 0) {
-      chPairs.ensure(ctx, K); chOff.ensure(ctx, K); chLen.ensure(ctx, K);
-      h2d(ctx, chPairs.p, changes.data() + L, K * sizeof(HostChange));
-      foreach(ctx, K, SplitPairsKernel{chPairs.p, chOff.p, chLen.p});
-      meta.ensure(ctx, K); colOff.ensure(ctx, (size_t)NCOLS * K); colLen.ensure(ctx, (size_t)NCOLS * K);
-      nOps.ensure(ctx, K + 1); nPreds.ensure(ctx, K + 1); nDeps.ensure(ctx, K + 1); nActors.ensure(ctx, K + 1);
-      foreach(ctx, K, ParseKernel{arena.p, chOff.p, chLen.p, K, meta.p, colOff.p, colLen.p, nOps.p, nPreds.p, nDeps.p, nActors.p, errWord.p, flagWord.p + 8});
-      depBase.ensure(ctx, K + 1); scan_exclusive(ctx, scanTmp, nDeps.p, depBase.p, K);
-      totalDeps = readU32(depBase.p + K);
-      depIdx.ensure(ctx, totalDeps + 1); primary.ensure(ctx, K);
-      const size_t tcap = pow2_at_least(2 * C + 2);
-      hashTable.ensure(ctx, tcap); dev_memset(ctx, hashTable.p, 0xff, tcap * 4);
-      foreach(ctx, C, HashInsertKernel{hashes.p, hashTable.p, (u64)tcap - 1});
-      foreach(ctx, K, ResolveDepsKernelT<ChangeMeta>{arena.p, hashes.p, hashTable.p, (u64)tcap - 1, meta.p, nDeps.p, L, depBase.p, depIdx.p, primary.p});
-    }
-    if (L > 0) {   // number of dependency indexes the loaded changes carry
-      DBuf<u64>& sumD = pairSucc; sumD.ensure(ctx, 1);
-      const HostChange& dn = loadedCol(0x40);
-      u64 sum = 0;
-      if (!(L >= parDocMinRows && dn.len > 0 && parCols.sumColumn(arena.p + dn.off, dn.len, L, &sum))) {
-        foreach_warp(ctx, 1, LoadedColKernel{LC_SUM, arena.p, dn.off, dn.len, 0, 0, nullptr, nullptr, nullptr, sumD.p});
-        d2h(ctx, &sum, sumD.p, 8); sync(ctx);
-      }
-      loadedDeps = (u32)sum;
-    }
-    saveVals.ensure(ctx, std::max<size_t>(std::max(std::max(C, N), S), (size_t)loadedDeps + totalDeps) + 2);
-    saveStrOff.ensure(ctx, std::max(C, N) + 1); saveStrLen.ensure(ctx, std::max(C, N) + 1);
-    auto loadedVal = [&](int kind, u32 id, u32 count) {
-      if (L == 0) return; const HostChange& c = loadedCol(id);
-      if (count >= parDocMinRows && c.len > 0) {   // long history: the parallel column decoders (doccols.cuh); they decline what is not canonical
-        const u8* bytes = arena.p + c.off; bool ok = false;
-        if (kind == LC_UINT) ok = parCols.toI64(bytes, c.len, false, count, saveVals.p);
-        else if (kind == LC_DELTA) ok = parCols.deltaToI64(bytes, c.len, count, saveVals.p);
-        else if (kind == LC_EXTRA_LEN) ok = parCols.extraLenColumn(bytes, c.len, count, saveVals.p, saveStrOff.p, saveStrLen.p, loadedCol(0x57).off);
-        if (ok) return;
-      }
-      foreach_warp(ctx, 1, LoadedColKernel{kind, arena.p, c.off, c.len, loadedCol(0x57).off, count, saveVals.p, saveStrOff.p, saveStrLen.p, nullptr});
-    };
-    auto changeVal = [&](int which) { if (K == 0) return; foreach(ctx, K, SaveChangeValKernel{which, arena.p, meta.p, actorSlots.p, (u64)actorCap - 1, saveVals.p + L, saveStrOff.p + L, saveStrLen.p + L, errWord.p}); };
-    loadedVal(LC_UINT, 0x01, (u32)L);  changeVal(SM_ACTOR);     add(changeCols, 0x01, enc.rleNum(saveVals.p, C, false));
-    loadedVal(LC_DELTA, 0x03, (u32)L); changeVal(SM_SEQ);       add(changeCols, 0x03, enc.deltaNum(saveVals.p, C));
-    loadedVal(LC_DELTA, 0x13, (u32)L); changeVal(SM_MAX_OP);    add(changeCols, 0x13, enc.deltaNum(saveVals.p, C));
-    loadedVal(LC_DELTA, 0x23, (u32)L); changeVal(SM_TIME);      add(changeCols, 0x23, enc.deltaNum(saveVals.p, C));
-    loadedVal(LC_STRING, 0x35, (u32)L); if (K > 0) foreach(ctx, K, SaveMessageKernel{meta.p, saveStrOff.p + L, saveStrLen.p + L});
-                                       add(changeCols, 0x35, enc.rle(StrCol{arena.p, saveStrOff.p, saveStrLen.p}, C));
-    loadedVal(LC_UINT, 0x40, (u32)L);  changeVal(SM_DEPS_NUM);  add(changeCols, 0x40, enc.rleNum(saveVals.p, C, false));
-    loadedVal(LC_DELTA, 0x43, loadedDeps); if (totalDeps > 0) foreach(ctx, totalDeps, SaveDepIndexKernel{depIdx.p, saveVals.p + loadedDeps});
-                                       add(changeCols, 0x43, enc.deltaNum(saveVals.p, (size_t)loadedDeps + totalDeps));
-    loadedVal(LC_EXTRA_LEN, 0x56, (u32)L); changeVal(SM_EXTRA_LEN); add(changeCols, 0x56, enc.rleNum(saveVals.p, C, false));
-                                       add(changeCols, 0x57, enc.raw(arena.p, saveStrOff.p, saveStrLen.p, C));
-    checkErr();
+  saveVals.ensure(ctx, std::max(std::max(s.C, s.N), s.S) + 2);
+  saveChangeColumns(s); saveOpColumns(s); packDocument(s, result);
+}
+
+// change metadata (new.js:1680-1692 appendChange); the first L rows come from the loaded document's own columns
+inline void Engine::saveChangeColumns(SaveCall& s) {
+  const size_t C = s.C, N = s.N, L = s.L, K = s.K;
+  if (C == 0) return;
+  ColumnEncoder& enc = *encoder;
+  u32 totalDeps = 0, loadedDeps = 0;
+  if (K > 0) {
+    chPairs.ensure(ctx, K); chOff.ensure(ctx, K); chLen.ensure(ctx, K);
+    h2d(ctx, chPairs.p, changes.data() + L, K * sizeof(HostChange));
+    foreach(ctx, K, SplitPairsKernel{chPairs.p, chOff.p, chLen.p});
+    meta.ensure(ctx, K); colOff.ensure(ctx, (size_t)NCOLS * K); colLen.ensure(ctx, (size_t)NCOLS * K);
+    nOps.ensure(ctx, K + 1); nPreds.ensure(ctx, K + 1); nDeps.ensure(ctx, K + 1); nActors.ensure(ctx, K + 1);
+    foreach(ctx, K, ParseKernel{arena.p, chOff.p, chLen.p, K, meta.p, colOff.p, colLen.p, nOps.p, nPreds.p, nDeps.p, nActors.p, errWord.p, flagWord.p + 8});
+    depBase.ensure(ctx, K + 1); scan_exclusive(ctx, scanTmp, nDeps.p, depBase.p, K);
+    totalDeps = readU32(depBase.p + K);
+    depIdx.ensure(ctx, totalDeps + 1); primary.ensure(ctx, K);
+    const size_t tcap = pow2_at_least(2 * C + 2);
+    hashTable.ensure(ctx, tcap); dev_memset(ctx, hashTable.p, 0xff, tcap * 4);
+    foreach(ctx, C, HashInsertKernel{hashes.p, hashTable.p, (u64)tcap - 1});
+    foreach(ctx, K, ResolveDepsKernelT<ChangeMeta>{arena.p, hashes.p, hashTable.p, (u64)tcap - 1, meta.p, nDeps.p, L, depBase.p, depIdx.p, primary.p});
   }
-  // ---- document ops (columnar.js:60-82)
+  if (L > 0) {   // number of dependency indexes the loaded changes carry
+    DBuf<u64>& sumD = pairSucc; sumD.ensure(ctx, 1);
+    const HostChange& dn = loaded.cols[CC_DEPS_NUM];
+    u64 sum = 0;
+    if (!(L >= parDocMinRows && dn.len > 0 && parCols.sumColumn(arena.p + dn.off, dn.len, L, &sum))) {
+      foreach_warp(ctx, 1, LoadedColKernel{LC_SUM, arena.p, dn.off, dn.len, 0, 0, nullptr, nullptr, nullptr, sumD.p});
+      d2h(ctx, &sum, sumD.p, 8); sync(ctx);
+    }
+    loadedDeps = (u32)sum;
+  }
+  saveVals.ensure(ctx, std::max<size_t>(std::max(std::max(C, N), s.S), (size_t)loadedDeps + totalDeps) + 2);
+  saveStrOff.ensure(ctx, std::max(C, N) + 1); saveStrLen.ensure(ctx, std::max(C, N) + 1);
+  auto loadedVal = [&](int k, size_t count) { if (L > 0) decodeLoadedCol(k, count, saveVals.p, saveStrOff.p, saveStrLen.p); };
+  auto changeVal = [&](int which) { if (K > 0) foreach(ctx, K, SaveChangeValKernel{which, arena.p, meta.p, actorSlots.p, (u64)actorCap - 1, saveVals.p + L, saveStrOff.p + L, saveStrLen.p + L, errWord.p}); };
+  auto add = [&](int k, size_t len) { s.changeCols.push_back({CHANGE_COLS[k].id, enc.outLen - len, len}); };
+  loadedVal(CC_ACTOR, L);     changeVal(SM_ACTOR);     add(CC_ACTOR, enc.rleNum(saveVals.p, C, false));
+  loadedVal(CC_SEQ, L);       changeVal(SM_SEQ);       add(CC_SEQ, enc.deltaNum(saveVals.p, C));
+  loadedVal(CC_MAX_OP, L);    changeVal(SM_MAX_OP);    add(CC_MAX_OP, enc.deltaNum(saveVals.p, C));
+  loadedVal(CC_TIME, L);      changeVal(SM_TIME);      add(CC_TIME, enc.deltaNum(saveVals.p, C));
+  loadedVal(CC_MESSAGE, L);   if (K > 0) foreach(ctx, K, SaveMessageKernel{meta.p, saveStrOff.p + L, saveStrLen.p + L});
+                              add(CC_MESSAGE, enc.rle(StrCol{arena.p, saveStrOff.p, saveStrLen.p}, C));
+  loadedVal(CC_DEPS_NUM, L);  changeVal(SM_DEPS_NUM);  add(CC_DEPS_NUM, enc.rleNum(saveVals.p, C, false));
+  loadedVal(CC_DEPS_INDEX, loadedDeps); if (totalDeps > 0) foreach(ctx, totalDeps, SaveDepIndexKernel{depIdx.p, saveVals.p + loadedDeps});
+                              add(CC_DEPS_INDEX, enc.deltaNum(saveVals.p, (size_t)loadedDeps + totalDeps));
+  loadedVal(CC_EXTRA_LEN, L); changeVal(SM_EXTRA_LEN); add(CC_EXTRA_LEN, enc.rleNum(saveVals.p, C, false));
+                              add(CC_EXTRA_RAW, enc.raw(arena.p, saveStrOff.p, saveStrLen.p, C));
+  checkErr();
+}
+
+// document ops (columnar.js:60-82); chldActor / chldCtr are always null in this format version: empty
+inline void Engine::saveOpColumns(SaveCall& s) {
+  const size_t N = s.N, S = s.S;
+  ColumnEncoder& enc = *encoder;
+  auto add = [&](int k, size_t len) { s.opCols.push_back({DOC_COL_IDS[k], enc.outLen - len, len}); };
   if (N > 0) {
     DocRows d = doc.view();
     saveStrOff.ensure(ctx, N + 1); saveStrLen.ensure(ctx, N + 1);
     auto opVal = [&](int which) { foreach(ctx, N, SaveOpValKernel{which, d, succOff.p, saveVals.p}); };
-    opVal(SC_OBJ_ACTOR); add(opCols, 0x01, enc.rleNum(saveVals.p, N, false));
-    opVal(SC_OBJ_CTR);   add(opCols, 0x02, enc.rleNum(saveVals.p, N, false));
-    opVal(SC_KEY_ACTOR); add(opCols, 0x11, enc.rleNum(saveVals.p, N, false));
-    opVal(SC_KEY_CTR);   add(opCols, 0x13, enc.deltaNum(saveVals.p, N));
-                         add(opCols, 0x15, enc.rle(StrCol{arena.p, d.keyStrOff, d.keyStrLen}, N));
-    opVal(SC_ID_ACTOR);  add(opCols, 0x21, enc.rleNum(saveVals.p, N, false));
-    opVal(SC_ID_CTR);    add(opCols, 0x23, enc.deltaNum(saveVals.p, N));
+    opVal(SC_OBJ_ACTOR); add(OC_OBJ_ACTOR, enc.rleNum(saveVals.p, N, false));
+    opVal(SC_OBJ_CTR);   add(OC_OBJ_CTR, enc.rleNum(saveVals.p, N, false));
+    opVal(SC_KEY_ACTOR); add(OC_KEY_ACTOR, enc.rleNum(saveVals.p, N, false));
+    opVal(SC_KEY_CTR);   add(OC_KEY_CTR, enc.deltaNum(saveVals.p, N));
+                         add(OC_KEY_STR, enc.rle(StrCol{arena.p, d.keyStrOff, d.keyStrLen}, N));
+    opVal(SC_ID_ACTOR);  add(OC_ID_ACTOR, enc.rleNum(saveVals.p, N, false));
+    opVal(SC_ID_CTR);    add(OC_ID_CTR, enc.deltaNum(saveVals.p, N));
     foreach(ctx, N, SaveInsertKernel{d, saveStrLen.p});
-                         add(opCols, 0x34, enc.boolean(saveStrLen.p, N));
-    opVal(SC_ACTION);    add(opCols, 0x42, enc.rleNum(saveVals.p, N, false));
-    opVal(SC_VAL_LEN);   add(opCols, 0x56, enc.rleNum(saveVals.p, N, false));
+                         add(OC_INSERT, enc.boolean(saveStrLen.p, N));
+    opVal(SC_ACTION);    add(OC_ACTION, enc.rleNum(saveVals.p, N, false));
+    opVal(SC_VAL_LEN);   add(OC_VAL_LEN, enc.rleNum(saveVals.p, N, false));
     foreach(ctx, N, SaveValBytesKernel{d, saveStrLen.p});
-                         add(opCols, 0x57, enc.raw(arena.p, d.valOff, saveStrLen.p, N));
-    // chldActor 0x61 / chldCtr 0x63: always null in this format version -> empty
-    opVal(SC_SUCC_NUM);  add(opCols, 0x80, enc.rleNum(saveVals.p, N, false));
+                         add(OC_VAL_RAW, enc.raw(arena.p, d.valOff, saveStrLen.p, N));
+    opVal(SC_SUCC_NUM);  add(OC_SUCC_NUM, enc.rleNum(saveVals.p, N, false));
     if (S > 0) {
-      foreach(ctx, S, SaveSuccValKernel{0, succ.p, saveVals.p}); add(opCols, 0x81, enc.rleNum(saveVals.p, S, false));
-      foreach(ctx, S, SaveSuccValKernel{1, succ.p, saveVals.p}); add(opCols, 0x83, enc.deltaNum(saveVals.p, S));
+      foreach(ctx, S, SaveSuccValKernel{0, succ.p, saveVals.p}); add(OC_SUCC_ACTOR, enc.rleNum(saveVals.p, S, false));
+      foreach(ctx, S, SaveSuccValKernel{1, succ.p, saveVals.p}); add(OC_SUCC_CTR, enc.deltaNum(saveVals.p, S));
     }
   }
-  smark("columns encoded (device)");
+  trace.print("save", "columns encoded (device)", s.t0);
+}
+
+// host: DEFLATE of large columns (columnar.js:1052-1057), directory, container (columnar.js:659-686)
+inline void Engine::packDocument(SaveCall& s, std::string& result) {
+  const ColumnEncoder& enc = *encoder;
   std::vector<u8> raw(enc.outLen);
   if (enc.outLen) { d2h(ctx, raw.data(), enc.out.p, enc.outLen); sync(ctx); }
-  // ---- host: DEFLATE of large columns (columnar.js:1052-1057), directory, container (columnar.js:659-686)
   struct Packed { u32 id; std::string data; };
-  std::vector<Packed> packed; std::vector<size_t> firstOp;
-  auto pack = [&](const std::vector<Col>& cols) { for (auto& c : cols) if (c.len > 0) packed.push_back({c.id, std::string((const char*)raw.data() + c.off, c.len)}); };
-  pack(changeCols); const size_t numChangeCols = packed.size(); pack(opCols);
-  if (!unknownCols.empty() && N > 0) {   // columns with ids this version does not know: host-encoded from the values kept per op (unknowncols.hpp)
+  std::vector<Packed> packed;
+  auto pack = [&](const std::vector<SaveCall::Col>& cols) { for (auto& c : cols) if (c.len > 0) packed.push_back({c.id, std::string((const char*)raw.data() + c.off, c.len)}); };
+  pack(s.changeCols); const size_t numChangeCols = packed.size(); pack(s.opCols);
+  if (!unknownCols.empty() && s.N > 0) {   // columns with ids this version does not know: host-encoded from the values kept per op (unknowncols.hpp)
     std::vector<std::pair<u32, std::string>> extra; appendUnknownDocColumns(extra);
     for (auto& e : extra) if (!e.second.empty()) packed.push_back({e.first, e.second});
     std::stable_sort(packed.begin() + numChangeCols, packed.end(), [](const Packed& a, const Packed& b) { return (a.id & ~8u) < (b.id & ~8u); });
@@ -1540,29 +1553,22 @@ inline void Engine::saveDocument(std::string& result) {
   {
     std::vector<std::thread> ts; std::vector<std::string> errs(packed.size());
     for (size_t k = 0; k < packed.size(); k++) if (packed[k].data.size() >= 256) ts.emplace_back([&, k] {
-      z_stream zs; memset(&zs, 0, sizeof(zs));
-      if (deflateInit2(&zs, 6, Z_DEFLATED, -15, 8, Z_DEFAULT_STRATEGY) != Z_OK) { errs[k] = "deflateInit failed"; return; }
-      std::string comp; comp.resize(deflateBound(&zs, (uLong)packed[k].data.size()));
-      zs.next_in = (Bytef*)packed[k].data.data(); zs.avail_in = (uInt)packed[k].data.size(); zs.next_out = (Bytef*)comp.data(); zs.avail_out = (uInt)comp.size();
-      const int rc = ::deflate(&zs, Z_FINISH); comp.resize(zs.total_out); deflateEnd(&zs);
-      if (rc != Z_STREAM_END) { errs[k] = "deflate failed"; return; }
-      packed[k].data.swap(comp); packed[k].id |= 8;
+      try { packed[k].data = deflateRawBytes((const u8*)packed[k].data.data(), packed[k].data.size()); packed[k].id |= 8; } catch (Error& e) { errs[k] = e.what(); }
     });
     for (auto& t : ts) t.join();
-    for (auto& e : errs) if (!e.empty()) throw Error(AMG_ERR_INTERNAL, e);
+    for (auto& e : errs) if (!e.empty()) throw Error(AMG_ERR_INTERNAL, e);   // the first in column order
   }
-  smark("columns deflated (host)");
+  trace.print("save", "columns deflated (host)", s.t0);
   std::string body;
-  auto uleb = [&](u64 v) { do { u8 b = v & 0x7f; v >>= 7; if (v) b |= 0x80; body.push_back((char)b); } while (v); };
-  uleb(st.actorIds.size()); for (auto& a : st.actorIds) { uleb(a.size()); body += a; }
-  uleb(st.heads.size()); for (auto& h : st.heads) body.append((const char*)h.data(), 32);
-  uleb(numChangeCols); for (size_t k = 0; k < numChangeCols; k++) { uleb(packed[k].id); uleb(packed[k].data.size()); }
-  uleb(packed.size() - numChangeCols); for (size_t k = numChangeCols; k < packed.size(); k++) { uleb(packed[k].id); uleb(packed[k].data.size()); }
+  put_uleb(body, st.actorIds.size()); for (auto& a : st.actorIds) { put_uleb(body, a.size()); body += a; }
+  put_uleb(body, st.heads.size()); for (auto& h : st.heads) body.append((const char*)h.data(), 32);
+  put_uleb(body, numChangeCols); for (size_t k = 0; k < numChangeCols; k++) { put_uleb(body, packed[k].id); put_uleb(body, packed[k].data.size()); }
+  put_uleb(body, packed.size() - numChangeCols); for (size_t k = numChangeCols; k < packed.size(); k++) { put_uleb(body, packed[k].id); put_uleb(body, packed[k].data.size()); }
   for (auto& p : packed) body += p.data;
-  for (u32 i : st.headIdx) uleb(i);
-  std::string head; head.push_back(0); { u64 v = body.size(); do { u8 b = v & 0x7f; v >>= 7; if (v) b |= 0x80; head.push_back((char)b); } while (v); }
-  std::string hashed = head + body; u8 digest[32]; host_sha256((const u8*)hashed.data(), hashed.size(), digest);
-  smark("container assembled + hashed");
+  for (u32 i : st.headIdx) put_uleb(body, i);
+  std::string hashed(1, '\0'); put_uleb(hashed, body.size()); hashed += body;
+  u8 digest[32]; host_sha256((const u8*)hashed.data(), hashed.size(), digest);
+  trace.print("save", "container assembled + hashed", s.t0);
   static const u8 magic[4] = {0x85, 0x6f, 0x4a, 0x83};
   result.assign((const char*)magic, 4); result.append((const char*)digest, 4); result += hashed;
 }
@@ -1573,213 +1579,223 @@ inline void Engine::saveDocument(std::string& result) {
 // as in SURVEY.md §2 row 12; column expansion and everything downstream run on the device.
 inline void Engine::loadDocument(const u8* buf, size_t len) {
   if (numApplied != 0 || numRows != 0) throw Error(AMG_ERR_INTERNAL, "load needs a fresh backend");
-  HostClock t0; auto lmark = [&](const char* what) { trace.print("load", what, t0); };
-  // columnar.js:688-708 decodeContainerHeader
+  LoadCall l(buf, len);
+  readContainer(l); inflateColumns(l); stageColumns(l); loadClock(l); countRows(l); decodeDocColumns(l); finalizeRows(l);
+  readUnknownOpColumns(l); commitLoad(l);
+  if (loaded.headIndexesUnknown) computeHashGraph();   // finds the heads' change indexes (and leaves the history rebuilt)
+}
+
+// container (columnar.js:688-708 decodeContainerHeader), document header and column directory (columnar.js:1006-1038 decodeDocumentHeader)
+inline void Engine::readContainer(LoadCall& l) {
+  const u8* buf = l.buf; const size_t len = l.len; ByteReader& r = l.r;
   if (len < 10 || buf[0] != 0x85 || buf[1] != 0x6f || buf[2] != 0x4a || buf[3] != 0x83) throw Error(AMG_ERR_RANGE, "Data does not begin with magic bytes 85 6f 4a 83");
-  ByteReader r(buf, 8, (u32)len); const u32 chunkType = buf[8]; r.pos = 9; const u64 chunkLen = r.uleb();
+  const u32 chunkType = buf[8]; r.pos = 9; const u64 chunkLen = r.uleb();
   if (r.err || (u64)r.pos + chunkLen > len) throw Error(AMG_ERR_RANGE, "buffer ended with incomplete number");
   u8 digest[32]; host_sha256(buf + 8, r.pos + (size_t)chunkLen - 8, digest);
   if (memcmp(digest, buf + 4, 4) != 0) throw Error(AMG_ERR_RANGE, "checksum does not match data");
   if ((u64)r.pos + chunkLen != len) throw Error(AMG_ERR_RANGE, "Encoded document has trailing data");
   if (chunkType != 0) throw Error(AMG_ERR_RANGE, "Unexpected chunk type: " + std::to_string(chunkType));
-  lmark("container checksum");
-  // columnar.js:1006-1038 decodeDocumentHeader
-  std::vector<std::string> actors; const u64 numActors = r.uleb();
-  for (u64 i = 0; i < numActors && !r.err; i++) { const u64 l = r.uleb(); if ((u64)r.pos + l > len) { r.err = KE_SUBARRAY; break; } actors.emplace_back((const char*)buf + r.pos, l); r.skip(l); }
-  std::vector<std::array<u8, 32>> hs; const u64 numHeads = r.uleb();
-  for (u64 i = 0; i < numHeads && !r.err; i++) { if ((u64)r.pos + 32 > len) { r.err = KE_SUBARRAY; break; } std::array<u8, 32> h; memcpy(h.data(), buf + r.pos, 32); hs.push_back(h); r.skip(32); }
-  struct ColInfo { u32 id; u64 len; std::string data; };
-  auto readInfo = [&](std::vector<ColInfo>& cols) {
+  trace.print("load", "container checksum", l.t0);
+  const u64 numActors = r.uleb();
+  for (u64 i = 0; i < numActors && !r.err; i++) { const u64 n = r.uleb(); if ((u64)r.pos + n > len) { r.err = KE_SUBARRAY; break; } l.actors.emplace_back((const char*)buf + r.pos, n); r.skip(n); }
+  const u64 numHeads = r.uleb();
+  for (u64 i = 0; i < numHeads && !r.err; i++) { if ((u64)r.pos + 32 > len) { r.err = KE_SUBARRAY; break; } std::array<u8, 32> h; memcpy(h.data(), buf + r.pos, 32); l.heads.push_back(h); r.skip(32); }
+  auto readInfo = [&](std::vector<LoadCall::ColInfo>& cols) {
     const u64 n = r.uleb(); long long last = -1;
-    for (u64 i = 0; i < n && !r.err; i++) { const u64 id = r.uleb(), l = r.uleb(); if (last >= 0 && ((u32)id & ~8u) <= ((u32)last & ~8u)) throw Error(AMG_ERR_RANGE, "Columns must be in ascending order"); last = (long long)id; cols.push_back({(u32)id, l, std::string()}); }
+    for (u64 i = 0; i < n && !r.err; i++) { const u64 id = r.uleb(), cl = r.uleb(); if (last >= 0 && ((u32)id & ~8u) <= ((u32)last & ~8u)) throw Error(AMG_ERR_RANGE, "Columns must be in ascending order"); last = (long long)id; cols.push_back({(u32)id, cl, std::string()}); }
   };
-  std::vector<ColInfo> changeCols, opCols; readInfo(changeCols); readInfo(opCols);
-  std::vector<std::pair<ColInfo*, const u8*>> deflated;
-  auto readData = [&](std::vector<ColInfo>& cols) {
+  readInfo(l.changeCols); readInfo(l.opCols);
+  auto readData = [&](std::vector<LoadCall::ColInfo>& cols) {
     for (auto& c : cols) {
       if (r.err || (u64)r.pos + c.len > len) throw Error(AMG_ERR_RANGE, "subarray exceeds buffer size");
-      if (c.id & 8) deflated.emplace_back(&c, buf + r.pos); else c.data.assign((const char*)buf + r.pos, (size_t)c.len);
+      if (c.id & 8) l.deflated.emplace_back(&c, buf + r.pos); else c.data.assign((const char*)buf + r.pos, (size_t)c.len);
       r.skip(c.len);
     }
   };
-  readData(changeCols); readData(opCols);
-  {   // DEFLATEd columns (columnar.js:1022-1027): independent streams, one host thread each when there are several large ones
-    std::vector<std::string> errs(deflated.size()); std::vector<int> codes(deflated.size(), 0); std::vector<std::thread> ts;
-    auto one = [&](size_t k) { try { ColInfo& c = *deflated[k].first; c.data = inflateRawBytes(deflated[k].second, (size_t)c.len); c.id ^= 8; } catch (Error& e) { errs[k] = e.what(); codes[k] = e.code; } catch (std::exception& e) { errs[k] = e.what(); codes[k] = AMG_ERR_INTERNAL; } };
-    for (size_t k = 0; k < deflated.size(); k++) { if (deflated.size() > 1 && deflated[k].first->len >= (64u << 10)) ts.emplace_back(one, k); else one(k); }
-    for (auto& t : ts) t.join();
-    for (size_t k = 0; k < errs.size(); k++) if (codes[k]) throw Error(codes[k], errs[k]);   // the first in column order, as a sequential reader would meet it
-  }
-  lmark("columns inflated");
+  readData(l.changeCols); readData(l.opCols);
+}
+
+// DEFLATEd columns (columnar.js:1022-1027): independent streams, one host thread each when there are several large ones
+inline void Engine::inflateColumns(LoadCall& l) {
+  const auto& deflated = l.deflated;
+  std::vector<std::string> errs(deflated.size()); std::vector<int> codes(deflated.size(), 0); std::vector<std::thread> ts;
+  auto one = [&](size_t k) { try { LoadCall::ColInfo& c = *deflated[k].first; c.data = inflateRawBytes(deflated[k].second, (size_t)c.len); c.id ^= 8; } catch (Error& e) { errs[k] = e.what(); codes[k] = e.code; } catch (std::exception& e) { errs[k] = e.what(); codes[k] = AMG_ERR_INTERNAL; } };
+  for (size_t k = 0; k < deflated.size(); k++) { if (deflated.size() > 1 && deflated[k].first->len >= (64u << 10)) ts.emplace_back(one, k); else one(k); }
+  for (auto& t : ts) t.join();
+  for (size_t k = 0; k < errs.size(); k++) if (codes[k]) throw Error(codes[k], errs[k]);   // the first in column order, as a sequential reader would meet it
+  trace.print("load", "columns inflated", l.t0);
+}
+
+// actor ids, op columns and change metadata columns staged in the arena. First the head indexes that end the chunk: they
+// are read only now so that an error of the inflate above wins over "buffer ended with incomplete number".
+inline void Engine::stageColumns(LoadCall& l) {
+  ByteReader& r = l.r;
   if (r.err) throw Error(AMG_ERR_RANGE, "buffer ended with incomplete number");
-  std::vector<u32> headsIndexes; if (!r.done()) for (u64 i = 0; i < numHeads; i++) headsIndexes.push_back((u32)r.uleb());
-  if (actors.size() > 65535) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: more than 65535 actors in one document");
-  // ---- stage actor ids and op columns in the arena
-  static const u32 DOC_IDS[16] = {0x01, 0x02, 0x11, 0x13, 0x15, 0x21, 0x23, 0x34, 0x42, 0x56, 0x57, 0x61, 0x63, 0x80, 0x81, 0x83};
-  DocCols dc; memset(&dc, 0, sizeof(dc));
-  hostArena.resize(0); std::vector<std::pair<u32, u32>> reps;
-  { size_t total = 0; for (auto& a : actors) total += a.size(); for (auto& c : opCols) total += c.data.size(); for (auto& c : changeCols) total += c.data.size(); hostArena.reserve(total + 64); }   // one pinned allocation, not one per append
-  for (auto& a : actors) { reps.emplace_back((u32)hostArena.size(), (u32)a.size()); hostArena.append(a.data(), a.size()); }
-  for (auto& c : opCols) for (int k = 0; k < 16; k++) if (c.id == DOC_IDS[k]) { dc.off[k] = (u32)hostArena.size(); dc.len[k] = (u32)c.data.size(); hostArena.append(c.data.data(), c.data.size()); }
-  {   // the change metadata columns stay available for a later save() (new.js:1717 keeps them as encoders)
-    static const u32 CHANGE_IDS[9] = {0x01, 0x03, 0x13, 0x23, 0x35, 0x40, 0x43, 0x56, 0x57};
-    for (int k = 0; k < 9; k++) loadedCols[k] = HostChange{(u32)hostArena.size(), 0};
-    for (auto& c : changeCols) for (int k = 0; k < 9; k++) if (c.id == CHANGE_IDS[k]) { loadedCols[k] = HostChange{(u32)hostArena.size(), (u32)c.data.size()}; hostArena.append(c.data.data(), c.data.size()); }
-  }
-  const size_t cur = hostArena.size();
+  if (!r.done()) for (size_t i = 0; i < l.heads.size(); i++) l.headIdx.push_back((u32)r.uleb());
+  if (l.actors.size() > 65535) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: more than 65535 actors in one document");
+  hostArena.resize(0);
+  { size_t total = 0; for (auto& a : l.actors) total += a.size(); for (auto& c : l.opCols) total += c.data.size(); for (auto& c : l.changeCols) total += c.data.size(); hostArena.reserve(total + 64); }   // one pinned allocation, not one per append
+  for (auto& a : l.actors) { l.reps.emplace_back((u32)hostArena.size(), (u32)a.size()); hostArena.append(a.data(), a.size()); }
+  for (auto& c : l.opCols) for (int k = 0; k < NUM_DOC_COLS; k++) if (c.id == DOC_COL_IDS[k]) { l.dc.off[k] = (u32)hostArena.size(); l.dc.len[k] = (u32)c.data.size(); hostArena.append(c.data.data(), c.data.size()); }
+  // the change metadata columns stay available for a later save() (new.js:1717 keeps them as encoders)
+  for (int k = 0; k < NUM_CHANGE_COLS; k++) l.doc.cols[k] = HostChange{(u32)hostArena.size(), 0};
+  for (auto& c : l.changeCols) for (int k = 0; k < NUM_CHANGE_COLS; k++) if (c.id == CHANGE_COLS[k].id) { l.doc.cols[k] = HostChange{(u32)hostArena.size(), (u32)c.data.size()}; hostArena.append(c.data.data(), c.data.size()); }
+  const size_t cur = l.arenaLen = hostArena.size();
   if (cur + 64 >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: change arena limited to 4 GiB per document");
   arena.ensure(ctx, cur + 64); h2d(ctx, arena.p, hostArena.data(), cur); dev_memset(ctx, arena.p + cur, 0, 64);
-  lmark("staged + uploaded");
-  // ---- change metadata: clock (new.js:1645-1675 readDocumentChanges). A long history is decoded and checked on the device
-  // (doccols.cuh + one stable sort by actor); a short one, or one the device path declines (malformed columns, a sequence
-  // error to report), by the same readers on the host, which produce the reference's error messages.
-  std::vector<u64> clk(actors.size(), 0); size_t numChanges = 0;
-  auto hostClock = [&]()
-  {
-    const std::string* actorCol = nullptr; const std::string* seqCol = nullptr;
-    for (auto& c : changeCols) { if (c.id == 0x01) actorCol = &c.data; if (c.id == 0x03) seqCol = &c.data; }
-    static const std::string empty;
-    const std::string& ac = actorCol ? *actorCol : empty; const std::string& sc = seqCol ? *seqCol : empty;
-    RleReader ar((const u8*)ac.data(), 0, (u32)ac.size(), 0), sr((const u8*)sc.data(), 0, (u32)sc.size(), 1); long long seqAcc = 0;
+  trace.print("load", "staged + uploaded", l.t0);
+}
+
+// change metadata: clock (new.js:1645-1675 readDocumentChanges). A long history is decoded and checked on the device
+// (doccols.cuh + one stable sort by actor); a short one, or one the device path declines (malformed columns, a sequence
+// error to report), by the same readers on the host, which produce the reference's error messages. Then the change index
+// of every head.
+inline void Engine::loadClock(LoadCall& l) {
+  const std::vector<std::string>& actors = l.actors;
+  l.clock.assign(actors.size(), 0);
+  bool onDevice = false; const HostChange ac = l.doc.cols[CC_ACTOR], sc = l.doc.cols[CC_SEQ]; u32 total = 0;
+  if (ac.len >= parDocMinRows / 8 + 16 && sc.len > 0 && parCols.rleRecords(arena.p + ac.off, ac.len, &total) && total >= parDocMinRows) {
+    const size_t n = total; DBuf<long long> aV, sV; aV.ensure(ctx, n + 1); sV.ensure(ctx, n + 1);
+    if (parCols.toI64(arena.p + ac.off, ac.len, false, n, aV.p) && parCols.deltaToI64(arena.p + sc.off, sc.len, n, sV.p)) {
+      sortKeys.ensure(ctx, n + 1); sortVals.ensure(ctx, n + 1); DBuf<u64> clkD; clkD.ensure(ctx, actors.size() + 1); dev_memset(ctx, clkD.p, 0, (actors.size() + 1) * 8);
+      dev_memset(ctx, flagWord.p, 0, 16);
+      foreach(ctx, n, ClockKeyKernel{aV.p, (u32)actors.size(), sortKeys.p, sortVals.p, flagWord.p});
+      sortPairs(sortKeys, sortVals, n, bits_for(actors.size() > 1 ? actors.size() - 1 : 1));
+      foreach(ctx, n, ClockCheckKernel{sortKeys.p, sortVals.p, sV.p, (u32)n, clkD.p, flagWord.p});
+      u32 bad = 0; d2h(ctx, &bad, flagWord.p, 4); if (!actors.empty()) d2h(ctx, l.clock.data(), clkD.p, actors.size() * 8); sync(ctx);
+      if (!bad) { onDevice = true; l.doc.numChanges = n; } else std::fill(l.clock.begin(), l.clock.end(), 0);
+    }
+  }
+  if (!onDevice) {
+    RleReader ar(hostArena.data() + ac.off, 0, ac.len, 0), sr(hostArena.data() + sc.off, 0, sc.len, 1); long long seqAcc = 0;   // (their staged copies)
     while (!ar.done()) {
-      long long a = 0, d = 0; u32 o, l; const bool an = ar.next(a, o, l), sn = sr.next(d, o, l);
+      long long a = 0, d = 0; u32 o, n; const bool an = ar.next(a, o, n), sn = sr.next(d, o, n);
       if (ar.r.err || sr.r.err) throw Error(AMG_ERR_RANGE, "malformed change metadata columns");
       if (!an || (u64)a >= actors.size()) throw Error(AMG_ERR_RANGE, "actor index out of range");
       if (sn) seqAcc += d;
       const u64 seq = sn ? (u64)seqAcc : 0;
-      if (seq != 1 && seq != clk[a] + 1) throw Error(AMG_ERR_RANGE, "Expected seq " + std::to_string(clk[a] + 1) + ", got " + std::to_string(seq) + " for actor " + hex_of((const u8*)actors[a].data(), actors[a].size()));
-      clk[a] = seq; numChanges++;
+      if (seq != 1 && seq != l.clock[a] + 1) throw Error(AMG_ERR_RANGE, "Expected seq " + std::to_string(l.clock[a] + 1) + ", got " + std::to_string(seq) + " for actor " + hex_of((const u8*)actors[a].data(), actors[a].size()));
+      l.clock[a] = seq; l.doc.numChanges++;
     }
-  };
-  {
-    bool onDevice = false; const HostChange ac = loadedCols[0], sc = loadedCols[1]; u32 total = 0;
-    if (ac.len >= parDocMinRows / 8 + 16 && sc.len > 0 && parCols.rleRecords(arena.p + ac.off, ac.len, &total) && total >= parDocMinRows) {
-      const size_t n = total; DBuf<long long> aV, sV; aV.ensure(ctx, n + 1); sV.ensure(ctx, n + 1);
-      if (parCols.toI64(arena.p + ac.off, ac.len, false, n, aV.p) && parCols.deltaToI64(arena.p + sc.off, sc.len, n, sV.p)) {
-        sortKeys.ensure(ctx, n + 1); sortVals.ensure(ctx, n + 1); DBuf<u64> clkD; clkD.ensure(ctx, actors.size() + 1); dev_memset(ctx, clkD.p, 0, (actors.size() + 1) * 8);
-        dev_memset(ctx, flagWord.p, 0, 16);
-        foreach(ctx, n, ClockKeyKernel{aV.p, (u32)actors.size(), sortKeys.p, sortVals.p, flagWord.p});
-        sortPairs(sortKeys, sortVals, n, bits_for(actors.size() > 1 ? actors.size() - 1 : 1));
-        foreach(ctx, n, ClockCheckKernel{sortKeys.p, sortVals.p, sV.p, (u32)n, clkD.p, flagWord.p});
-        u32 bad = 0; d2h(ctx, &bad, flagWord.p, 4); if (!actors.empty()) d2h(ctx, clk.data(), clkD.p, actors.size() * 8); sync(ctx);
-        if (!bad) { onDevice = true; numChanges = n; } else std::fill(clk.begin(), clk.end(), 0);
-      }
-    }
-    if (!onDevice) hostClock();
   }
-  lmark("clock");
-  if (!headsIndexes.empty() && headsIndexes.size() != hs.size()) headsIndexes.clear();
+  trace.print("load", "clock", l.t0);
+  if (!l.headIdx.empty() && l.headIdx.size() != l.heads.size()) l.headIdx.clear();
   // several heads without indexes (new.js:1734-1737: the hashes are known, their change indexes are not): the indexes are
-  // found by reconstructing the change history right after the load (computeHashGraph below)
-  bool headIdxUnknown = false;
-  if (headsIndexes.empty()) { if (hs.size() == 1) headsIndexes.push_back((u32)(numChanges ? numChanges - 1 : 0)); else if (!hs.empty()) { headIdxUnknown = true; headsIndexes.assign(hs.size(), 0xffffffffu); } }
+  // found by reconstructing the change history right after the load (computeHashGraph)
+  if (l.headIdx.empty()) { if (l.heads.size() == 1) l.headIdx.push_back((u32)(l.doc.numChanges ? l.doc.numChanges - 1 : 0)); else if (!l.heads.empty()) { l.doc.headIndexesUnknown = true; l.headIdx.assign(l.heads.size(), 0xffffffffu); } }
+}
+
+inline void Engine::ensureLoadRows(size_t n) {
+  for (DBuf<u32>* b : {&r_objActor, &r_objCtr, &r_keyActor, &r_keyCtr, &r_keyStrOff, &r_keyStrLen, &r_insert, &r_action, &r_valLen, &r_valOff, &r_predNum, &r_predOff, &o_change, &o_time}) b->ensure(ctx, n + 1);
+}
+
+// Number of rows = values of the action column, number of succ entries = sum of succNum. Long columns take the parallel
+// decoder (doccols.cuh); short, malformed or non-canonical ones the serial walkers, which also report the errors.
+inline void Engine::countRows(LoadCall& l) {
+  const DocCols& dc = l.dc;
   dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull; dev_memset(ctx, flagWord.p, 0, 16);
-  // Number of rows = values of the action column, number of succ entries = sum of succNum. Long columns take the parallel
-  // decoder (doccols.cuh); short, malformed or non-canonical ones the serial walkers, which also report the errors.
   { const char* e = getenv("AMG_PAR_DOC_MIN"); if (e) parDocMinRows = (size_t)strtoull(e, nullptr, 10); }
-  size_t N = 0, S = 0; u32 serialMask = 0xffffu; bool counted = false;
-  auto colBytes = [&](int k) { return arena.p + dc.off[k]; };
-  auto ensureRows = [&]() {
-    for (DBuf<u32>* b : {&r_objActor, &r_objCtr, &r_keyActor, &r_keyCtr, &r_keyStrOff, &r_keyStrLen, &r_insert, &r_action, &r_valLen, &r_valOff, &r_predNum, &r_predOff, &o_change, &o_time}) b->ensure(ctx, N + 1);
+  auto succInParallel = [&](size_t rows) {   // many rows: the succ total in parallel too (succNum then needs no serial decode)
+    if (rows < parDocMinRows || rows >= (1u << 29)) return;
+    l.N = rows; ensureLoadRows(l.N); u64 sum = 0;
+    if (dc.len[OC_SUCC_NUM] == 0) { l.counted = true; l.S = 0; }
+    else if (parCols.countColumn(arena.p + dc.off[OC_SUCC_NUM], dc.len[OC_SUCC_NUM], l.N, r_predNum.p, r_predOff.p, &sum)) { l.counted = true; l.S = (size_t)sum; l.serialMask &= ~(1u << OC_SUCC_NUM); }
   };
-  if (dc.len[8] >= parDocMinRows / 8 + 16) {   // (a long column can still be a handful of records; then the serial count is instant anyway)
-    u32 total = 0;
-    if (parCols.rleRecords(colBytes(8), dc.len[8], &total) && total >= parDocMinRows && total < (1u << 29)) {
-      N = total; ensureRows();
-      u64 sum = 0;
-      if (dc.len[13] == 0) { counted = true; S = 0; }
-      else if (parCols.countColumn(colBytes(13), dc.len[13], N, r_predNum.p, r_predOff.p, &sum)) { counted = true; S = (size_t)sum; serialMask &= ~(1u << 13); }
-    }
-  }
-  if (!counted) {   // short action column: rows by the serial record walk, the succ total still in parallel if there are many rows
-    serialMask = 0xffffu;
+  u32 total = 0;   // (a long column can still be a handful of records; then the serial count is instant anyway)
+  if (dc.len[OC_ACTION] >= parDocMinRows / 8 + 16 && parCols.rleRecords(arena.p + dc.off[OC_ACTION], dc.len[OC_ACTION], &total)) succInParallel(total);
+  if (!l.counted) {   // short action column: rows by the serial record walk
     foreach(ctx, 1, DocCountRowsKernel{arena.p, dc, flagWord.p, errWord.p});
     u32 n32 = 0; d2h(ctx, &n32, flagWord.p, 4); sync(ctx); checkErr();
-    if (n32 >= parDocMinRows && n32 < (1u << 29)) {
-      N = n32; ensureRows(); u64 sum = 0;
-      if (dc.len[13] == 0) { counted = true; S = 0; }
-      else if (parCols.countColumn(colBytes(13), dc.len[13], N, r_predNum.p, r_predOff.p, &sum)) { counted = true; S = (size_t)sum; serialMask &= ~(1u << 13); }
-    }
+    succInParallel(n32);
   }
-  if (!counted) {
-    serialMask = 0xffffu;
+  if (!l.counted) {
     foreach(ctx, 1, DocCountKernel{arena.p, dc, flagWord.p, errWord.p});
     u32 cnt[2]; d2h(ctx, cnt, flagWord.p, 8); sync(ctx); checkErr();
-    N = cnt[0]; S = cnt[1];
+    l.N = cnt[0]; l.S = cnt[1];
   }
-  lmark("rows counted");
+  trace.print("load", "rows counted", l.t0);
+}
+
+// Columns of a long document through the parallel decoders; what they decline, and every column of a short document,
+// through DocColumnKernel (one launch, the columns selected by the mask).
+inline void Engine::decodeDocColumns(LoadCall& l) {
+  const size_t N = l.N, S = l.S; const DocCols& dc = l.dc;
   if (N >= (1u << 29)) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: more than 2^29 document rows");
-  ensureRows();
+  ensureLoadRows(N);
   r_predActor.ensure(ctx, S + 1); r_predCtr.ensure(ctx, S + 1);
-  RawRows raw{r_objActor.p, r_objCtr.p, r_keyActor.p, r_keyCtr.p, r_keyStrOff.p, r_keyStrLen.p, r_insert.p, r_action.p, r_valLen.p, r_valOff.p, r_predNum.p, r_predOff.p, r_predActor.p, r_predCtr.p};
+  const RawRows raw = l.raw = rawRows();
   if (N >= parDocMinRows) {
-    struct Plan { int k, col; u32* out; };   // document column -> row field, as DocColumnKernel maps them
-    const Plan plan[] = {{0, CX_OBJ_ACTOR, raw.objActor}, {1, CX_OBJ_CTR, raw.objCtr}, {2, CX_KEY_ACTOR, raw.keyActor}, {3, CX_KEY_CTR, raw.keyCtr}, {4, CX_KEY_STR, nullptr},
-                         {5, CX_OBJ_ACTOR, o_change.p}, {6, CX_KEY_CTR, o_time.p}, {7, CX_INSERT, raw.insert}, {8, CX_ACTION, raw.action}, {9, CX_VAL_LEN, raw.valLen},
-                         {13, CX_PRED_NUM, raw.predNum}, {14, CX_PRED_ACTOR, raw.predActor}, {15, CX_PRED_CTR, raw.predCtr}};
-    for (const Plan& pl : plan) {
-      if (!((serialMask >> pl.k) & 1u)) continue;
-      const size_t cnt = (pl.k == 14 || pl.k == 15) ? S : N; const u32 len = dc.len[pl.k]; const u8* bytes = colBytes(pl.k); bool done = false;
-      if (len == 0) {
-        RawRows rr = raw; if (pl.k == 5) rr.objActor = o_change.p; if (pl.k == 6) rr.keyCtr = o_time.p;
-        if (cnt > 0) foreach(ctx, cnt, DocAbsentKernel{pl.col, rr});
+    for (int k = 0; k < NUM_DOC_COLS; k++) {
+      const int cx = doc_col_decoder(k);
+      if (cx < 0 || !((l.serialMask >> k) & 1u)) continue;
+      const size_t cnt = (cx == CX_PRED_ACTOR || cx == CX_PRED_CTR) ? S : N; const RawRows rr = doc_col_rows(k, raw, o_change.p, o_time.p); bool done = false;
+      if (dc.len[k] == 0) {
+        if (cnt > 0) foreach(ctx, cnt, DocAbsentKernel{cx, rr});
         done = true;
-      } else if (cnt > 0) switch (pl.col) {
-        case CX_OBJ_ACTOR: case CX_OBJ_CTR: case CX_KEY_ACTOR: case CX_ACTION: case CX_PRED_ACTOR: done = parCols.toU32(bytes, len, cnt, pl.out); break;
-        case CX_KEY_CTR: case CX_PRED_CTR: done = parCols.deltaToU32(bytes, len, cnt, pl.out); break;
-        case CX_INSERT: done = parCols.boolean(bytes, len, cnt, pl.out); break;
-        case CX_VAL_LEN: { u64 sum = 0; done = parCols.lenColumn(bytes, len, cnt, raw.valLen, raw.valOff, dc.off[10], &sum) && sum <= dc.len[10]; } break;
-        case CX_PRED_NUM: { u64 sum = 0; done = parCols.countColumn(bytes, len, cnt, raw.predNum, raw.predOff, &sum) && sum == S; } break;
-        default: break;   // utf8 keys: below
+      } else if (cnt > 0) {   // (utf8 keys: below)
+        u64 sum = 0;
+        done = parCols.decode(CX_PAR_KIND[cx], arena.p + dc.off[k], dc.len[k], cnt, cx_outputs(rr, cx, 0, 0, dc.off[OC_VAL_RAW], &sum));
+        if (cx == CX_VAL_LEN) done = done && sum <= dc.len[OC_VAL_RAW];
+        if (cx == CX_PRED_NUM) done = done && sum == S;
       }
-      if (done) serialMask &= ~(1u << pl.k);
+      if (done) l.serialMask &= ~(1u << k);
     }
-    if ((serialMask >> 4) & 1u) {   // keyStr: serial over records, parallel over rows
+    if ((l.serialMask >> OC_KEY_STR) & 1u) {   // keyStr: serial over records, parallel over rows
       DBuf<u32>& recStart = parCols.recOff; DBuf<u32>& recStrOff = parCols.recTok; DBuf<u32>& recStrLen = parCols.recN;
       recStart.ensure(ctx, N + 3); recStrOff.ensure(ctx, N + 3); recStrLen.ensure(ctx, N + 3);
-      foreach_warp(ctx, 1, DocKeyStrRecordsKernel{arena.p, dc.off[4], dc.len[4], (u32)N, recStart.p, recStrOff.p, recStrLen.p, flagWord.p, errWord.p});
+      foreach_warp(ctx, 1, DocKeyStrRecordsKernel{arena.p, dc.off[OC_KEY_STR], dc.len[OC_KEY_STR], (u32)N, recStart.p, recStrOff.p, recStrLen.p, flagWord.p, errWord.p});
       u32 rc[2]; d2h(ctx, rc, flagWord.p, 8); sync(ctx); checkErr();
       foreach(ctx, N, DocKeyStrExpandKernel{recStart.p, recStrOff.p, recStrLen.p, rc[0], raw.keyStrOff, raw.keyStrLen});
-      serialMask &= ~(1u << 4);
+      l.serialMask &= ~(1u << OC_KEY_STR);
     }
   }
-  if (Trace::enabled()) fprintf(stderr, "amgpu load: %zu rows, %zu succ entries, columns left to the serial decoder: mask %04x (counted in parallel: %d)\n", N, S, serialMask & 0xe3ffu, counted ? 1 : 0);
-  if (serialMask & 0xe3ffu) foreach_warp(ctx, 16, DocColumnKernel{arena.p, dc, (u32)N, (u32)S, raw, o_change.p, o_time.p, errWord.p, serialMask});
-  lmark("columns decoded");
+  if (Trace::enabled()) fprintf(stderr, "amgpu load: %zu rows, %zu succ entries, columns left to the serial decoder: mask %04x (counted in parallel: %d)\n", N, S, l.serialMask & DECODED_DOC_COLS, l.counted ? 1 : 0);
+  if (l.serialMask & DECODED_DOC_COLS) foreach_warp(ctx, NUM_DOC_COLS, DocColumnKernel{arena.p, dc, (u32)N, (u32)S, raw, o_change.p, o_time.p, errWord.p, l.serialMask});
+  trace.print("load", "columns decoded", l.t0);
+}
+
+inline void Engine::finalizeRows(LoadCall& l) {
+  const size_t N = l.N, S = l.S;
   doc.ensure(ctx, N + 1); succOff.ensure(ctx, N + 2); succ.ensure(ctx, S + 1);
   DBuf<u64>& maxOpD = pairSucc; maxOpD.ensure(ctx, 1); dev_memset(ctx, maxOpD.p, 0, 8);
-  foreach(ctx, N, DocFinalizeKernel{raw, o_change.p, o_time.p, (u32)actors.size(), doc.view(), succOff.p, succ.p, maxOpD.p, errWord.p});
+  foreach(ctx, N, DocFinalizeKernel{l.raw, o_change.p, o_time.p, (u32)l.actors.size(), doc.view(), succOff.p, succ.p, maxOpD.p, errWord.p});
   { const u32 s32 = (u32)S; h2d(ctx, succOff.p + N, &s32, 4); }
-  u64 mx = 0; d2h(ctx, &mx, maxOpD.p, 8); sync(ctx); checkErr();
-  lmark("rows finalized");
-  {   // op columns with unknown ids: their values are kept per op (host; unknowncols.hpp) so that save() writes them again
-    bool anyUnknown = false; for (auto& c : opCols) if (!is_known_doc_column(c.id)) anyUnknown = true;
-    unknownCols.clear();
-    if (anyUnknown && N > 0) {
-      std::string all; std::vector<std::array<u32, 3>> cols;
-      for (auto& c : opCols) { cols.push_back({c.id, (u32)all.size(), (u32)c.data.size()}); all += c.data; }
-      std::vector<u64> ids(N); d2h(ctx, ids.data(), doc.id.p, N * 8); sync(ctx);
-      const u32 e = read_unknown_columns((const u8*)all.data(), cols, N, is_known_doc_column, [&](size_t i, UnknownRow& row) {
-        if (row.empty()) return;
-        for (auto& kv : row) unknownCols.colIds.insert(kv.first);
-        unknownCols.byOp[ids[i]] = row;
-      });
-      if (e == KE_UNSUPPORTED_OP) throw Error(AMG_ERR_RANGE, "unexpected VALUE_RAW column");
-      if (e) throwKernelError((u64)e);
-    }
-  }
-  // ---- change history placeholders: only the head hashes are known (new.js:1727-1739)
+  d2h(ctx, &l.maxOp, maxOpD.p, 8); sync(ctx); checkErr();
+  trace.print("load", "rows finalized", l.t0);
+}
+
+// op columns with unknown ids: their values are kept per op (host; unknowncols.hpp) so that save() writes them again
+inline void Engine::readUnknownOpColumns(LoadCall& l) {
+  const size_t N = l.N;
+  bool anyUnknown = false; for (auto& c : l.opCols) if (!is_known_doc_column(c.id)) anyUnknown = true;
+  unknownCols.clear();
+  if (!anyUnknown || N == 0) return;
+  std::string all; std::vector<std::array<u32, 3>> cols;
+  for (auto& c : l.opCols) { cols.push_back({c.id, (u32)all.size(), (u32)c.data.size()}); all += c.data; }
+  std::vector<u64> ids(N); d2h(ctx, ids.data(), doc.id.p, N * 8); sync(ctx);
+  const u32 e = read_unknown_columns((const u8*)all.data(), cols, N, is_known_doc_column, [&](size_t i, UnknownRow& row) {
+    if (row.empty()) return;
+    for (auto& kv : row) unknownCols.colIds.insert(kv.first);
+    unknownCols.byOp[ids[i]] = row;
+  });
+  if (e == KE_UNSUPPORTED_OP) throw Error(AMG_ERR_RANGE, "unexpected VALUE_RAW column");
+  if (e) throwKernelError((u64)e);
+}
+
+// change history placeholders: only the head hashes are known (new.js:1727-1739); then the document's host state
+inline void Engine::commitLoad(LoadCall& l) {
+  const size_t numChanges = l.doc.numChanges; const auto& hs = l.heads;
   hashes.ensure(ctx, numChanges * 32 + 64); dev_memset(ctx, hashes.p, 0, numChanges * 32 + 64);
-  if (!headIdxUnknown) for (size_t i = 0; i < hs.size(); i++) { if (headsIndexes[i] >= numChanges) throw Error(AMG_ERR_RANGE, "head index out of range"); h2d(ctx, hashes.p + (size_t)headsIndexes[i] * 32, hs[i].data(), 32); }
+  if (!l.doc.headIndexesUnknown) for (size_t i = 0; i < hs.size(); i++) { if (l.headIdx[i] >= numChanges) throw Error(AMG_ERR_RANGE, "head index out of range"); h2d(ctx, hashes.p + (size_t)l.headIdx[i] * 32, hs[i].data(), 32); }
   sync(ctx);
-  numRows = N; numSucc = S; numApplied = numChanges; arenaLen = cur;
+  numRows = l.N; numSucc = l.S; numApplied = numChanges; arenaLen = l.arenaLen;
   std::vector<size_t> o(hs.size()); for (size_t i = 0; i < o.size(); i++) o[i] = i; std::sort(o.begin(), o.end(), [&](size_t a, size_t b) { return hs[a] < hs[b]; });
-  st = DocState{actors, reps, clk, mx, {}, {}}; for (size_t i : o) { st.heads.push_back(hs[i]); st.headIdx.push_back(headsIndexes[i]); }
-  changes.assign(numChanges, HostChange{0, 0}); haveHashGraph = false; loadedDoc.assign((const char*)buf, len); numLoaded = numChanges; headIndexesUnknown = headIdxUnknown;
-  lmark("host state");
+  st = DocState{l.actors, l.reps, l.clock, l.maxOp, {}, {}}; for (size_t i : o) { st.heads.push_back(hs[i]); st.headIdx.push_back(l.headIdx[i]); }
+  changes.assign(numChanges, HostChange{0, 0});
+  l.doc.bytes.assign((const char*)l.buf, l.len); l.doc.haveHashGraph = false; loaded = std::move(l.doc);
+  trace.print("load", "host state", l.t0);
   while (actorCap < 2 * (st.actorIds.size() + 16)) actorCap *= 2;
   actorSlots.ensure(ctx, actorCap); rebuildActorTable();
-  if (headIndexesUnknown) computeHashGraph();   // finds the heads' change indexes (and leaves the history rebuilt)
 }
 
 }  // namespace amg

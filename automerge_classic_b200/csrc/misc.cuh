@@ -1,6 +1,7 @@
 // amgpu — small glue kernels of the pipeline (flags, compaction, sequence-number check, heads).
 #pragma once
 #include "patch.cuh"
+#include "doccols.cuh"
 namespace amg { struct HostChange; }
 
 namespace amg {
@@ -103,36 +104,28 @@ struct OffsetsToRangesKernel { const u64* offsets; u32 shift; u32* off; u32* len
 struct SplitPairsKernel { const HostChange* pairs; u32* off; u32* len; HD void operator()(size_t b) const { off[b] = pairs[b].off; len[b] = pairs[b].len; } };
 struct PatchPairsKernel { const u32* triples; u32* off; u32* len; HD void operator()(size_t i) const { const u32 c = triples[3 * i]; off[c] = triples[3 * i + 1]; len[c] = triples[3 * i + 2]; } };
 // ---------------------------------------------------------------- Backend.load: document chunk -> document table (new.js:1709-1750)
-struct DocCols { u32 off[16]; u32 len[16]; };   // objActor,objCtr,keyActor,keyCtr,keyStr,idActor,idCtr,insert,action,valLen,valRaw,chldActor,chldCtr,succNum,succActor,succCtr
 struct DocCountKernel {   // thread 0: number of rows (action column), then sum of succNum
   const u8* arena; DocCols c; u32* out /* [0] rows, [1] succ entries */; u64* errWord;
   HD void operator()(size_t) const {
-    u32 err = 0; const u32 n = rle_count_values(arena, c.off[8], c.off[8] + c.len[8], &err);
-    u64 s = 0; if (!err) s = rle_sum_values(arena, c.off[13], c.off[13] + c.len[13], n, &err);
+    u32 err = 0; const u32 n = rle_count_values(arena, c.off[OC_ACTION], c.off[OC_ACTION] + c.len[OC_ACTION], &err);
+    u64 s = 0; if (!err) s = rle_sum_values(arena, c.off[OC_SUCC_NUM], c.off[OC_SUCC_NUM] + c.len[OC_SUCC_NUM], n, &err);
     if (err) raise(errWord, err, 0); if (s > 0x7fffffffULL) { raise(errWord, KE_TOO_LARGE, 0); s = 0; }
     out[0] = n; out[1] = (u32)s;
   }
 };
 struct DocCountRowsKernel {   // rows only; the walk is by record, so a column of a few long runs costs nothing
   const u8* arena; DocCols c; u32* out; u64* errWord;
-  HD void operator()(size_t) const { u32 err = 0; out[0] = rle_count_values(arena, c.off[8], c.off[8] + c.len[8], &err); if (err) raise(errWord, err, 0); }
+  HD void operator()(size_t) const { u32 err = 0; out[0] = rle_count_values(arena, c.off[OC_ACTION], c.off[OC_ACTION] + c.len[OC_ACTION], &err); if (err) raise(errWord, err, 0); }
 };
 struct DocColumnKernel {   // one thread per document column; the change-column decoders are reused through a remapped row view
   const u8* arena; DocCols c; u32 n, numSucc; RawRows rows; u32* idActor; u32* idCtr; u64* errWord; u32 mask /* columns to decode here */;
   HD void operator()(size_t k) const {
-    if (!((mask >> k) & 1u)) return;
-    RawRows r = rows; int col = -1;
-    switch ((int)k) {
-      case 0: col = CX_OBJ_ACTOR; break; case 1: col = CX_OBJ_CTR; break; case 2: col = CX_KEY_ACTOR; break; case 3: col = CX_KEY_CTR; break; case 4: col = CX_KEY_STR; break;
-      case 5: col = CX_OBJ_ACTOR; r.objActor = idActor; break;      // idActor: plain RLE uint
-      case 6: col = CX_KEY_CTR; r.keyCtr = idCtr; break;            // idCtr: delta
-      case 7: col = CX_INSERT; break; case 8: col = CX_ACTION; break; case 9: col = CX_VAL_LEN; break;
-      case 13: col = CX_PRED_NUM; break; case 14: col = CX_PRED_ACTOR; break; case 15: col = CX_PRED_CTR; break;   // succ group == pred group layout
-      default: return;
-    }
+    const int col = doc_col_decoder((int)k);
+    if (!((mask >> k) & 1u) || col < 0) return;
+    const RawRows r = doc_col_rows((int)k, rows, idActor, idCtr);
     u32 e;
     if (c.len[k] == 0) { fill_absent_column(col, n, 0, 0, numSucc, r); e = 0; }
-    else e = decode_one_column(arena, col, n, 0, c.off[k], c.off[k] + c.len[k], c.off[10], c.len[10], 0, numSucc, r);
+    else e = decode_one_column(arena, col, n, 0, c.off[k], c.off[k] + c.len[k], c.off[OC_VAL_RAW], c.len[OC_VAL_RAW], 0, numSucc, r);
     if (e) raise(errWord, e, k);
   }
 };
@@ -177,20 +170,9 @@ struct ClockCheckKernel {
     if (j + 1 == n || key[j + 1] != key[j]) clock[key[j]] = (u64)s;
   }
 };
-struct DocAbsentKernel {   // fill_absent_column for a long document, one thread per row (col as in DocColumnKernel, rows already remapped)
+struct DocAbsentKernel {   // fill_absent_column for a long document, one thread per row (col as in DocColumnKernel, rows from doc_col_rows)
   int col; RawRows r;
-  HD void operator()(size_t i) const {
-    switch (col) {
-      case CX_OBJ_ACTOR: r.objActor[i] = NULL32; break; case CX_OBJ_CTR: r.objCtr[i] = NULL32; break; case CX_KEY_ACTOR: r.keyActor[i] = NULL32; break;
-      case CX_KEY_CTR: r.keyCtr[i] = NULL32; break; case CX_ACTION: r.action[i] = NULL32; break;
-      case CX_VAL_LEN: r.valLen[i] = NULL32; r.valOff[i] = 0; break;
-      case CX_KEY_STR: r.keyStrOff[i] = 0; r.keyStrLen[i] = NULL32; break;
-      case CX_INSERT: r.insert[i] = 0; break;
-      case CX_PRED_NUM: r.predNum[i] = 0; r.predOff[i] = 0; break;
-      case CX_PRED_ACTOR: r.predActor[i] = NULL32; break; case CX_PRED_CTR: r.predCtr[i] = NULL32; break;
-      default: break;
-    }
-  }
+  HD void operator()(size_t i) const { fill_absent_column(col, 1, (u32)i, col == CX_PRED_NUM ? 0u : (u32)i, 1, r); }   // row i (pred columns: entry i); an absent succNum gives offset 0
 };
 struct DebugColumnKernel {   // amg_debug_decode_column, serial side: the readers of the load path on one column
   int kind; const u8* bytes; u32 len; u32 n; long long* out; u32* tmp; u64* errWord;

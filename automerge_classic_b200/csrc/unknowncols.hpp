@@ -12,7 +12,7 @@
 #include <string>
 #include <unordered_map>
 #include <vector>
-#include "decode.cuh"
+#include "doccols.cuh"
 
 namespace amg {
 
@@ -27,7 +27,8 @@ struct UnknownStore {
 };
 
 inline bool is_known_change_column(u32 id) { return col_index_of(id) >= 0; }
-inline bool is_known_doc_column(u32 id) { return col_index_of(id) >= 0 || id == 0x21 || id == 0x23 || id == 0x80 || id == 0x81 || id == 0x83; }
+// an op column of the document format, or one of the change format's (a pred column in a document is skipped, not carried)
+inline bool is_known_doc_column(u32 id) { return std::count(DOC_COL_IDS, DOC_COL_IDS + NUM_DOC_COLS, id) > 0 || is_known_change_column(id); }
 
 // one value-at-a-time reader for a column of any type (what makeDecoders gives readOperation)
 struct AnyColumnReader {

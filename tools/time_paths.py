@@ -15,6 +15,7 @@ d2 = wall('load #1', lambda: GpuBackendDoc(s))
 wall('getPatch after load #1', d2.get_patch_flat); wall('getPatch after load #2', d2.get_patch_flat)
 d3 = wall('load #2', lambda: GpuBackendDoc(s))
 wall('save after load', d3.save)
+d5 = GpuBackendDoc(s); wall('getChanges([]) after load', lambda: d5.get_changes([]))   # rebuilds the change history
 # latency of small calls on a document that already holds 100k ops (the engine re-derives the document order per call)
 t2 = tracegen.generate('C3', 100000, 10)
 ch = t2.changes()
