@@ -166,6 +166,36 @@ napi_value HashByActor(napi_env env, napi_callback_info info) {
   if (!found) { napi_value u; napi_get_undefined(env, &u); return u; }
   return bytesToUint8Array(env, hash, 32);
 }
+// syncBloom(state, lastSync) — sync.js:234-238 makeBloomFilter(backend, lastSync).bloom; lastSync: Uint8Array of n x 32 bytes
+napi_value SyncBloom(napi_env env, napi_callback_info info) {
+  napi_value arr = hashListCall(env, info, amg_sync_bloom), el; if (!arr) return nullptr;
+  napi_get_element(env, arr, 0, &el); return el;
+}
+// syncChangesToSend(state, lastSync, filters, need) — sync.js:246-306 getChangesToSend for a non-empty `have`. lastSync, need:
+// Uint8Array of n x 32 bytes; filters: array of parsed Bloom filters {numEntries, numProbes, bits: Uint8Array}. Returns
+// [changes, hashes]: the changes to send in the reference's order, and one Uint8Array with their 32-byte hashes back to
+// back (to filter sentHashes with).
+napi_value SyncChangesToSend(napi_env env, napi_callback_info info) {
+  napi_value argv[4]; amg_backend* b; if (!getArgs(env, info, 4, argv) || !getBackend(env, argv[0], &b)) return nullptr;
+  const uint8_t *last, *need; size_t lastLen, needLen;
+  if (!getBytes(env, argv[1], &last, &lastLen) || !getBytes(env, argv[3], &need, &needLen)) return nullptr;
+  bool isArray = false; napi_is_array(env, argv[2], &isArray);
+  if (!isArray) { napi_throw_type_error(env, nullptr, "filters must be an array"); return nullptr; }
+  uint32_t n = 0; napi_get_array_length(env, argv[2], &n);
+  std::vector<amg_bloom> filters(n);
+  for (uint32_t i = 0; i < n; i++) {
+    napi_value f, v; napi_get_element(env, argv[2], i, &f);
+    napi_get_named_property(env, f, "numEntries", &v); if (napi_get_value_uint32(env, v, &filters[i].num_entries) != napi_ok) { napi_throw_type_error(env, nullptr, "numEntries must be a number"); return nullptr; }
+    napi_get_named_property(env, f, "numProbes", &v); if (napi_get_value_uint32(env, v, &filters[i].num_probes) != napi_ok) { napi_throw_type_error(env, nullptr, "numProbes must be a number"); return nullptr; }
+    napi_get_named_property(env, f, "bits", &v); if (!getBytes(env, v, &filters[i].bits, &filters[i].bits_len)) return nullptr;
+  }
+  amg_buffers *changes = nullptr, *hashes = nullptr; amg_error err;
+  if (amg_sync_changes_to_send(b, last, lastLen / 32, filters.data(), n, need, needLen / 32, &changes, &hashes, &err)) return throwAmg(env, err);
+  napi_value out, hs; napi_create_array_with_length(env, 2, &out);
+  napi_get_element(env, buffersToJs(env, hashes), 0, &hs);
+  napi_set_element(env, out, 0, buffersToJs(env, changes)); napi_set_element(env, out, 1, hs);
+  return out;
+}
 // Backend.free — backend/backend.js:16-19: releases the device memory now instead of at garbage collection
 napi_value Free(napi_env env, napi_callback_info info) {
   napi_value argv[1]; Holder* h; if (!getArgs(env, info, 1, argv) || !getHolder(env, argv[0], &h)) return nullptr;
@@ -177,7 +207,8 @@ napi_value InitModule(napi_env env, napi_value exports) {
   struct { const char* name; napi_callback fn; } fns[] = {
     {"init", Init}, {"load", Load}, {"clone", Clone}, {"free", Free}, {"applyChanges", ApplyChanges}, {"getPatch", GetPatch}, {"save", Save},
     {"getHeads", GetHeads}, {"getChanges", GetChanges}, {"getChangesAdded", GetChangesAdded}, {"getChangeByHash", GetChangeByHash},
-    {"getMissingDeps", GetMissingDeps}, {"clockOf", ClockOf}, {"hashByActor", HashByActor}};
+    {"getMissingDeps", GetMissingDeps}, {"clockOf", ClockOf}, {"hashByActor", HashByActor}, {"syncBloom", SyncBloom},
+    {"syncChangesToSend", SyncChangesToSend}};
   for (auto& f : fns) { napi_value fn; napi_create_function(env, f.name, NAPI_AUTO_LENGTH, f.fn, nullptr, &fn); napi_set_named_property(env, exports, f.name, fn); }
   return exports;
 }

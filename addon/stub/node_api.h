@@ -39,6 +39,8 @@ napi_status napi_create_double(napi_env env, double value, napi_value* result);
 napi_status napi_remove_wrap(napi_env env, napi_value js_object, void** result);
 napi_status napi_create_function(napi_env env, const char* utf8name, size_t length, napi_callback cb, void* data, napi_value* result);
 napi_status napi_set_named_property(napi_env env, napi_value object, const char* utf8name, napi_value value);
+napi_status napi_get_named_property(napi_env env, napi_value object, const char* utf8name, napi_value* result);
+napi_status napi_get_value_uint32(napi_env env, napi_value value, uint32_t* result);
 #define NAPI_MODULE(modname, regfunc) extern "C" napi_value napi_register_module_v1(napi_env env, napi_value exports) { return regfunc(env, exports); }
 #define NODE_GYP_MODULE_NAME amgpu_napi
 #ifdef __cplusplus

@@ -10,9 +10,10 @@ from .engine import GpuBackendDoc, AmgError, Unsupported
 from . import sync as _sync
 
 
-def bind_sync(facade):
-    """Adds the sync functions of backend/index.js:2, 7 to a Backend facade (the reference's sync.js is tied to its own backend)."""
-    s = _sync.Sync(facade)
+def bind_sync(facade, device=True):
+    """Adds the sync functions of backend/index.js:2, 7 to a Backend facade (the reference's sync.js is tied to its own backend).
+    device=False keeps the Bloom filters and the choice of changes to send in Python (see sync.Sync)."""
+    s = _sync.Sync(facade, device=device)
     facade.generateSyncMessage, facade.receiveSyncMessage = s.generateSyncMessage, s.receiveSyncMessage
     for name in ('encodeSyncMessage', 'decodeSyncMessage', 'encodeSyncState', 'decodeSyncState', 'initSyncState'):
         setattr(facade, name, getattr(_sync, name))

@@ -12,6 +12,8 @@ struct amg_buffers { std::vector<std::string> items; };
 namespace {
 typedef std::array<u8, 32> Hash;
 struct HashHasher { size_t operator()(const Hash& h) const { size_t v; memcpy(&v, h.data(), sizeof(v)); return v; } };
+Hash toHash(const u8* p) { Hash h; memcpy(h.data(), p, 32); return h; }
+std::string hashHex(const Hash& h) { return hex_of(h.data(), 32); }
 
 // Host hash graph, filled lazily from the applied changes' headers (the reference defers it too: new.js:1887-1912)
 struct HostGraph {
@@ -64,7 +66,43 @@ struct amg_backend {
     if (idx < eng.loaded.historyRebuilt && plain.size() >= 256) return deflateChange(plain);   // what encodeChange returns for a rebuilt change (columnar.js:738)
     return plain;
   }
+  // new.js:1921-1973 getChanges(haveDeps): the indexes of the changes it returns, in its order. n == 0: every applied change
+  // (the host graph is not needed for that; the caller makes sure the hashes are known).
+  std::vector<u32> changesSince(const u8* have_deps, size_t n);
 };
+
+std::vector<u32> amg_backend::changesSince(const u8* have_deps, size_t n) {
+  std::vector<u32> out;
+  if (n == 0) { out.resize(eng.changes.size()); for (size_t i = 0; i < out.size(); i++) out[i] = (u32)i; return out; }
+  ensureGraph();
+  std::vector<Hash> stack, toReturn; std::unordered_map<Hash, bool, HashHasher> seen;
+  for (size_t i = 0; i < n; i++) {
+    Hash h = toHash(have_deps + 32 * i); seen[h] = true;
+    auto it = g.dependents.find(h); if (it == g.dependents.end() || !g.indexByHash.count(h)) throw amg::Error(AMG_RANGE_ERROR, "hash not found: " + hashHex(h));
+    stack.insert(stack.end(), it->second.begin(), it->second.end());
+  }
+  // Reference quirk reproduced on purpose (new.js:1938-1955): the traversal stops at a change with an unseen dependency, but
+  // the test below only looks at the stack and the heads - when that change was the last one on the stack and the heads
+  // have all been seen, the fast path still answers, without the changes that are concurrent to `haveDeps`.
+  while (!stack.empty()) {
+    Hash h = stack.back(); stack.pop_back(); seen[h] = true; toReturn.push_back(h);
+    bool all = true; for (auto& d : g.deps[g.indexByHash[h]]) if (!seen.count(d)) all = false;
+    if (!all) break;
+    auto& ds = g.dependents[h]; stack.insert(stack.end(), ds.begin(), ds.end());
+  }
+  bool headsSeen = true; for (auto& h : eng.st.heads) if (!seen.count(h)) headsSeen = false;
+  if (stack.empty() && headsSeen) { for (auto& h : toReturn) out.push_back(g.indexByHash[h]); return out; }
+  stack.clear(); for (size_t i = 0; i < n; i++) stack.push_back(toHash(have_deps + 32 * i)); seen.clear();
+  while (!stack.empty()) {
+    Hash h = stack.back(); stack.pop_back();
+    if (!seen.count(h)) {
+      auto it = g.indexByHash.find(h); if (it == g.indexByHash.end()) throw amg::Error(AMG_RANGE_ERROR, "hash not found: " + hashHex(h));
+      auto& ds = g.deps[it->second]; stack.insert(stack.end(), ds.begin(), ds.end()); seen[h] = true;
+    }
+  }
+  for (size_t i = 0; i < eng.changes.size(); i++) if (!seen.count(g.hash[i])) out.push_back((u32)i);
+  return out;
+}
 
 namespace {
 void setErr(amg_error* err, int code, const std::string& msg) {
@@ -76,8 +114,6 @@ void setErr(amg_error* err, int code, const std::string& msg) {
   catch (std::exception& e) { amg::drop_pending_peeks(); setErr(err, AMG_INTERNAL_ERROR, e.what()); return AMG_INTERNAL_ERROR; }
 
 amg_patch* serialize(const PatchOut& p) { return new amg_patch{p.bytes, p.bytesLen}; }
-Hash toHash(const u8* p) { Hash h; memcpy(h.data(), p, 32); return h; }
-std::string hashHex(const Hash& h) { return hex_of(h.data(), 32); }
 }  // namespace
 
 extern "C" {
@@ -154,36 +190,49 @@ int amg_save(amg_backend* b, amg_buffers** out, amg_error* err) {
 // new.js:1921-1973
 int amg_get_changes(amg_backend* b, const uint8_t* have_deps, size_t n, amg_buffers** out, amg_error* err) {
   AMG_GUARD(
-    b->ensureGraph(); HostGraph& g = b->g; auto* l = new amg_buffers(); std::unique_ptr<amg_buffers> guard(l);
-    if (n == 0) { for (size_t i = 0; i < b->eng.changes.size(); i++) l->items.push_back(b->changeBytes((u32)i)); *out = guard.release(); return 0; }
-    std::vector<Hash> stack, toReturn; std::unordered_map<Hash, bool, HashHasher> seen;
-    for (size_t i = 0; i < n; i++) {
-      Hash h = toHash(have_deps + 32 * i); seen[h] = true;
-      auto it = g.dependents.find(h); if (it == g.dependents.end() || !g.indexByHash.count(h)) throw amg::Error(AMG_RANGE_ERROR, "hash not found: " + hashHex(h));
-      stack.insert(stack.end(), it->second.begin(), it->second.end());
-    }
-    // Reference quirk reproduced on purpose (new.js:1938-1955): the traversal stops at a change with an unseen dependency, but
-    // the test below only looks at the stack and the heads - when that change was the last one on the stack and the heads
-    // have all been seen, the fast path still answers, without the changes that are concurrent to `haveDeps`.
-    while (!stack.empty()) {
-      Hash h = stack.back(); stack.pop_back(); seen[h] = true; toReturn.push_back(h);
-      bool all = true; for (auto& d : g.deps[g.indexByHash[h]]) if (!seen.count(d)) all = false;
-      if (!all) break;
-      auto& ds = g.dependents[h]; stack.insert(stack.end(), ds.begin(), ds.end());
-    }
-    bool headsSeen = true; for (auto& h : b->eng.st.heads) if (!seen.count(h)) headsSeen = false;
-    if (stack.empty() && headsSeen) { for (auto& h : toReturn) l->items.push_back(b->changeBytes(g.indexByHash[h])); *out = guard.release(); return 0; }
-    stack.clear(); for (size_t i = 0; i < n; i++) stack.push_back(toHash(have_deps + 32 * i)); seen.clear();
-    while (!stack.empty()) {
-      Hash h = stack.back(); stack.pop_back();
-      if (!seen.count(h)) {
-        auto it = g.indexByHash.find(h); if (it == g.indexByHash.end()) throw amg::Error(AMG_RANGE_ERROR, "hash not found: " + hashHex(h));
-        auto& ds = g.deps[it->second]; stack.insert(stack.end(), ds.begin(), ds.end()); seen[h] = true;
-      }
-    }
-    for (size_t i = 0; i < b->eng.changes.size(); i++) if (!seen.count(g.hash[i])) l->items.push_back(b->changeBytes((u32)i));
+    b->ensureGraph(); auto* l = new amg_buffers(); std::unique_ptr<amg_buffers> guard(l);
+    for (u32 i : b->changesSince(have_deps, n)) l->items.push_back(b->changeBytes(i));
     *out = guard.release(); return 0;)
 }
+// sync.js:234-238 makeBloomFilter: Bloom filter over the hashes of getChanges(last_sync), built on the device
+int amg_sync_bloom(amg_backend* b, const uint8_t* last_sync, size_t n, amg_buffers** out, amg_error* err) {
+  AMG_GUARD(
+    Engine& e = b->eng; if (!e.loaded.haveHashGraph) e.computeHashGraph();   // the hashes of a loaded document (new.js:1922)
+    auto* l = new amg_buffers(); std::unique_ptr<amg_buffers> guard(l); l->items.emplace_back();
+    if (n == 0) e.syncBloom(nullptr, e.numApplied, l->items.back());   // every applied change: no host graph needed
+    else { const std::vector<u32> idx = b->changesSince(last_sync, n); e.syncBloom(idx.data(), idx.size(), l->items.back()); }
+    *out = guard.release(); return 0;)
+}
+// sync.js:246-306 getChangesToSend for a non-empty `have`
+int amg_sync_changes_to_send(amg_backend* b, const uint8_t* last_sync, size_t n_last, const amg_bloom* filters, size_t n_filters,
+                             const uint8_t* need, size_t n_need, amg_buffers** out_changes, amg_buffers** out_hashes, amg_error* err) {
+  AMG_GUARD(
+    Engine& e = b->eng; if (!e.loaded.haveHashGraph) e.computeHashGraph();
+    std::vector<u32> cand; if (n_last > 0) cand = b->changesSince(last_sync, n_last);
+    const u32* idx = n_last > 0 ? cand.data() : nullptr; const size_t count = n_last > 0 ? cand.size() : e.numApplied;
+    std::vector<Engine::BloomSpec> fs(n_filters);
+    for (size_t i = 0; i < n_filters; i++) fs[i] = Engine::BloomSpec{filters[i].num_entries, filters[i].num_probes, filters[i].bits, filters[i].bits_len};
+    std::vector<u8> send; e.syncChangesToSend(idx, count, fs, send);
+    // sync.js:291-305: first the needed changes that are not candidates (unknown ones are skipped), then, in candidate
+    // order, the candidates that were marked or are needed
+    std::vector<u32> outIdx;
+    if (n_need > 0) {
+      b->ensureGraph();
+      std::vector<u32> posOf(e.numApplied, EMPTY32);   // change index -> candidate position
+      for (size_t i = 0; i < count; i++) posOf[idx ? idx[i] : i] = (u32)i;
+      for (size_t k = 0; k < n_need; k++) {
+        auto it = b->g.indexByHash.find(toHash(need + 32 * k));
+        if (it == b->g.indexByHash.end()) continue;
+        if (posOf[it->second] != EMPTY32) send[posOf[it->second]] = 1; else outIdx.push_back(it->second);
+      }
+    }
+    for (size_t i = 0; i < count; i++) if (send[i]) outIdx.push_back(idx ? idx[i] : (u32)i);
+    auto* lc = new amg_buffers(); std::unique_ptr<amg_buffers> gc(lc); auto* lh = new amg_buffers(); std::unique_ptr<amg_buffers> gh(lh);
+    lh->items.emplace_back(); e.gatherHashes(outIdx, lh->items.back());
+    for (u32 i : outIdx) lc->items.push_back(b->changeBytes(i));
+    *out_changes = gc.release(); *out_hashes = gh.release(); return 0;)
+}
+float amg_last_sync_ms(amg_backend* b) { return b->eng.lastSyncMs; }
 // new.js:1979-1997
 int amg_get_changes_added(amg_backend* bn, amg_backend* bo, amg_buffers** out, amg_error* err) {
   AMG_GUARD(

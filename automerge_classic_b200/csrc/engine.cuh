@@ -27,6 +27,7 @@
 #include "domlocal.cuh"
 #include "doccols.cuh"
 #include "history.cuh"
+#include "sync.cuh"
 #include "unknowncols.hpp"
 
 namespace amg {
@@ -218,6 +219,7 @@ class Engine {
     if (ctx.evMirror) cudaEventDestroy(ctx.evMirror);
     if (ctx.evFork) cudaEventDestroy(ctx.evFork);
     if (ctx.evJoin) cudaEventDestroy(ctx.evJoin);
+    for (auto& e : syncEv) if (e) cudaEventDestroy(e);
 #endif
   }
 
@@ -421,6 +423,22 @@ class Engine {
   void computeHashGraph();   // change history of a loaded document (history.cuh); the sections, in order:
   void histChangeColumns(HistoryCall& h), histActorOrder(HistoryCall& h), histPredsAndDeletions(HistoryCall& h), histOpsToChanges(HistoryCall& h),
        histActorTables(HistoryCall& h), histEncode(HistoryCall& h), histHashes(HistoryCall& h), histCheckHeads(HistoryCall& h), histCommit(HistoryCall& h);
+
+  // ---------------------------------------------------------------- sync protocol (sync.cuh, engine_impl.cuh)
+  // Candidates are change indexes idx[0, count); idx == nullptr: every applied change, in application order. The change
+  // hashes must be known (computeHashGraph has run on a loaded document).
+  struct BloomSpec { u32 numEntries, numProbes; const u8* bits; size_t bitsLen; };   // a peer's parsed filter (sync.js:38-76)
+  void syncBloom(const u32* idx, size_t count, std::string& out);   // BloomFilter(hashes).bytes
+  void syncChangesToSend(const u32* idx, size_t count, const std::vector<BloomSpec>& filters, std::vector<u8>& send);   // send[i]: Bloom-negative or depends on one
+  void gatherHashes(const std::vector<u32>& idx, std::string& out);   // 32 bytes per change
+  float lastSyncMs = 0;   // device span (CUDA events on the main stream) of the last sync call's uploads, kernels and read-backs (0 in the emulation build)
+  DBuf<u32> syncIdx, syncBits; DBuf<u8> syncFilterBits, syncNeg, syncHashOut; DBuf<BloomRef> syncFilters;
+ private:
+  void uploadCandidates(const u32* idx, size_t count);
+  void syncTimer(bool start);
+#ifndef AMG_EMU
+  cudaEvent_t syncEv[2] = {nullptr, nullptr};
+#endif
 };
 
 }  // namespace amg

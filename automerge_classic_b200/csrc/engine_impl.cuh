@@ -1798,4 +1798,107 @@ inline void Engine::commitLoad(LoadCall& l) {
   actorSlots.ensure(ctx, actorCap); rebuildActorTable();
 }
 
+// ---------------------------------------------------------------- sync protocol (sync.js:234-306)
+inline void Engine::syncTimer(bool start) {
+#ifndef AMG_EMU
+  if (!syncEv[0]) for (auto& e : syncEv) CUDA_CHECK(cudaEventCreate(&e));
+  CUDA_CHECK(cudaEventRecord(syncEv[start ? 0 : 1], ctx.stream));
+  if (!start) { float ms = 0; CUDA_CHECK(cudaEventSynchronize(syncEv[1])); CUDA_CHECK(cudaEventElapsedTime(&ms, syncEv[0], syncEv[1])); lastSyncMs += ms; }
+#else
+  (void)start;
+#endif
+}
+
+inline void Engine::uploadCandidates(const u32* idx, size_t count) {
+  if (!idx) return;
+  syncIdx.ensure(ctx, count + 1); h2d(ctx, syncIdx.p, idx, count * 4);
+}
+
+// makeBloomFilter (sync.js:234-238): BloomFilter(hashes).bytes = LEB128 numEntries, 10, 7, then ceil(10 * count / 8) bytes
+inline void Engine::syncBloom(const u32* idx, size_t count, std::string& out) {
+  out.clear(); lastSyncMs = 0;
+  if (count == 0) return;   // BloomFilter([]).bytes is empty
+  const size_t bitsBytes = (BLOOM_BITS_PER_ENTRY * count + 7) / 8, words = (bitsBytes + 3) / 4;
+  syncTimer(true);
+  uploadCandidates(idx, count);
+  syncBits.ensure(ctx, words); dev_memset(ctx, syncBits.p, 0, words * 4);
+  foreach(ctx, count, BloomAddKernel{hashes.p, idx ? syncIdx.p : nullptr, 8 * (u64)bitsBytes, syncBits.p});
+  put_uleb(out, count); put_uleb(out, BLOOM_BITS_PER_ENTRY); put_uleb(out, BLOOM_NUM_PROBES);
+  const size_t at = out.size(); out.resize(at + words * 4);
+  d2h(ctx, &out[at], syncBits.p, words * 4); sync(ctx);
+  out.resize(at + bitsBytes);
+  syncTimer(false);
+}
+
+// getChangesToSend (sync.js:246-306) for a non-empty `have`: which candidates go out because of the peer's filters.
+inline void Engine::syncChangesToSend(const u32* idx, size_t count, const std::vector<BloomSpec>& filters, std::vector<u8>& send) {
+  send.assign(count, 0); lastSyncMs = 0;
+  if (count == 0) return;
+  for (auto& f : filters)
+    if (f.numProbes > BLOOM_MAX_PROBES) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: a Bloom filter with " + std::to_string(f.numProbes) + " probes (the device path takes at most " + std::to_string(BLOOM_MAX_PROBES) + ")");
+  syncTimer(true);
+  uploadCandidates(idx, count);
+  const u32* idxD = idx ? syncIdx.p : nullptr;
+  // sync.js:273-276: a candidate is negative when no filter contains it
+  std::vector<BloomRef> refs; std::string blob;
+  for (auto& f : filters) {
+    const bool empty = f.numEntries == 0 || f.bitsLen == 0;
+    refs.push_back(BloomRef{blob.size(), empty ? 0 : 8 * (u64)f.bitsLen, f.numProbes, 0});
+    if (!empty) blob.append((const char*)f.bits, f.bitsLen);
+  }
+  syncFilters.ensure(ctx, refs.size() + 1); h2d(ctx, syncFilters.p, refs.data(), refs.size() * sizeof(BloomRef));
+  syncFilterBits.ensure(ctx, blob.size() + 1); h2d(ctx, syncFilterBits.p, blob.data(), blob.size());
+  syncNeg.ensure(ctx, count);
+  foreach(ctx, count, BloomProbeKernel{hashes.p, idxD, syncFilterBits.p, syncFilters.p, (u32)refs.size(), syncNeg.p});
+  d2h(ctx, send.data(), syncNeg.p, count); sync(ctx);
+  size_t numNeg = 0; for (u8 v : send) numNeg += v;
+  if (numNeg == 0 || numNeg == count) { syncTimer(false); return; }   // a peer that has everything, or a new one: no closure needed
+  // sync.js:277-289: everything that depends on a Bloom-negative candidate goes too. The candidates' dependency indexes are
+  // resolved like save() does (ParseKernel over their headers, scan, HashInsertKernel, ResolveDepsKernelT<ChangeMeta>).
+  const size_t K = count, C = numApplied;
+  std::vector<HostChange> pairs(K); for (size_t i = 0; i < K; i++) pairs[i] = changes[idx ? idx[i] : i];
+  chPairs.ensure(ctx, K); chOff.ensure(ctx, K); chLen.ensure(ctx, K);
+  h2d(ctx, chPairs.p, pairs.data(), K * sizeof(HostChange));
+  foreach(ctx, K, SplitPairsKernel{chPairs.p, chOff.p, chLen.p});
+  meta.ensure(ctx, K); colOff.ensure(ctx, (size_t)NCOLS * K); colLen.ensure(ctx, (size_t)NCOLS * K);
+  nOps.ensure(ctx, K + 1); nPreds.ensure(ctx, K + 1); nDeps.ensure(ctx, K + 1); nActors.ensure(ctx, K + 1);
+  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+  foreach(ctx, K, ParseKernel{arena.p, chOff.p, chLen.p, K, meta.p, colOff.p, colLen.p, nOps.p, nPreds.p, nDeps.p, nActors.p, errWord.p, flagWord.p + 8});
+  depBase.ensure(ctx, K + 1); scan_exclusive(ctx, scanTmp, nDeps.p, depBase.p, K);
+  const u32 totalDeps = readU32(depBase.p + K);
+  checkErr();
+  depIdx.ensure(ctx, totalDeps + 1); primary.ensure(ctx, K);
+  const size_t tcap = pow2_at_least(2 * C + 2);
+  hashTable.ensure(ctx, tcap); dev_memset(ctx, hashTable.p, 0xff, tcap * 4);
+  foreach(ctx, C, HashInsertKernel{hashes.p, hashTable.p, (u64)tcap - 1});
+  // numApplied = 0: primary[b] looks up change b, which exists (b < K <= C); only depIdx is used here
+  foreach(ctx, K, ResolveDepsKernelT<ChangeMeta>{arena.p, hashes.p, hashTable.p, (u64)tcap - 1, meta.p, nDeps.p, 0, depBase.p, depIdx.p, primary.p});
+  std::vector<u32> base(K + 1), deps(totalDeps);
+  d2h(ctx, base.data(), depBase.p, (K + 1) * 4); d2h(ctx, deps.data(), depIdx.p, (size_t)totalDeps * 4); sync(ctx);
+  syncTimer(false);
+  // One forward pass in application order: a change is applied only after its dependencies (a loaded document stores its
+  // changes in topological order), so a candidate's candidate dependencies are decided before it is. This stays on the host
+  // on purpose: it is O(candidates + deps), while a device frontier walk needs one launch per dependency level, which on a
+  // history that is one long chain is one launch per change (up to 10^6).
+  std::vector<u32> order(K); for (size_t i = 0; i < K; i++) order[i] = (u32)i;
+  if (idx) std::sort(order.begin(), order.end(), [&](u32 a, u32 b) { return idx[a] < idx[b]; });
+  std::vector<u8> marked(C, 0);   // by change index; only candidates are ever marked
+  for (u32 p : order) {
+    u8 m = send[p];
+    for (u32 j = base[p]; j < base[p + 1] && !m; j++) if (deps[j] != DEP_MISSING && marked[deps[j]]) m = 1;
+    send[p] = m; marked[idx ? idx[p] : p] = m;
+  }
+}
+
+inline void Engine::gatherHashes(const std::vector<u32>& idx, std::string& out) {
+  out.assign(idx.size() * 32, '\0');
+  if (idx.empty()) return;
+  syncTimer(true);
+  syncIdx.ensure(ctx, idx.size() + 1); h2d(ctx, syncIdx.p, idx.data(), idx.size() * 4);
+  syncHashOut.ensure(ctx, idx.size() * 32);
+  foreach(ctx, idx.size(), SyncHashGatherKernel{hashes.p, syncIdx.p, syncHashOut.p});
+  d2h(ctx, &out[0], syncHashOut.p, out.size()); sync(ctx);
+  syncTimer(false);   // adds to the span of the syncChangesToSend call it follows
+}
+
 }  // namespace amg

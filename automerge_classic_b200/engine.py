@@ -41,6 +41,10 @@ class _ErrStruct(C.Structure):
     _fields_ = [('code', C.c_int), ('msg', C.c_char * 512)]
 
 
+class _Bloom(C.Structure):   # amg_bloom: a peer's parsed Bloom filter
+    _fields_ = [('num_entries', C.c_uint32), ('num_probes', C.c_uint32), ('bits', C.c_void_p), ('bits_len', C.c_size_t)]
+
+
 class Library:
     def __init__(self, path):
         if not os.path.exists(path):
@@ -71,8 +75,13 @@ class Library:
         L.amg_free_mem.argtypes = [vp]
         for name in ('amg_apply_changes', 'amg_apply_changes_packed', 'amg_get_patch', 'amg_get_state', 'amg_get_heads', 'amg_get_changes',
                      'amg_get_changes_added', 'amg_get_change_by_hash', 'amg_get_missing_deps', 'amg_clock_of', 'amg_hash_by_actor',
-                     'amg_debug_dump_ops', 'amg_debug_decode', 'amg_debug_decode_column', 'amg_bench_decode', 'amg_last_timings'):
+                     'amg_debug_dump_ops', 'amg_debug_decode', 'amg_debug_decode_column', 'amg_bench_decode', 'amg_last_timings',
+                     'amg_sync_bloom', 'amg_sync_changes_to_send'):
             getattr(L, name).restype = C.c_int
+        L.amg_sync_bloom.argtypes = [vp, vp, C.c_size_t, vp, vp]
+        L.amg_sync_changes_to_send.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, vp, C.c_size_t, vp, vp, vp]
+        L.amg_last_sync_ms.restype = C.c_float
+        L.amg_last_sync_ms.argtypes = [vp]
 
     def check(self, rc, err):
         if rc != 0:
@@ -294,7 +303,7 @@ class GpuBackendDoc:
         for i in range(L.amg_buffers_count(bl)):
             n = C.c_size_t()
             p = L.amg_buffers_get(bl, i, C.byref(n))
-            out.append(bytes((C.c_uint8 * n.value).from_address(p)) if n.value else b'')
+            out.append(C.string_at(p, n.value) if n.value else b'')
         L.amg_buffers_free(bl)
         return out
 
@@ -405,6 +414,37 @@ class GpuBackendDoc:
         bl, err = C.c_void_p(), _ErrStruct()
         self._lib.check(self._lib.L.amg_get_missing_deps(self.h, hs, C.c_size_t(len(heads)), C.byref(bl), C.byref(err)), err)
         return [b.hex() for b in self._buffers(bl)]
+
+    # ---- sync protocol (automerge_classic_b200/sync.py uses these when the document has them)
+    def sync_bloom(self, last_sync):
+        """makeBloomFilter(backend, lastSync) (sync.js:234-238): BloomFilter([hashes of getChanges(lastSync)]).bytes, built on
+        the device from the hashes the engine holds."""
+        hs = b''.join(bytes.fromhex(h) for h in last_sync)
+        bl, err = C.c_void_p(), _ErrStruct()
+        self._lib.check(self._lib.L.amg_sync_bloom(self.h, hs, C.c_size_t(len(last_sync)), C.byref(bl), C.byref(err)), err)
+        return self._buffers(bl)[0]
+
+    def sync_changes_to_send(self, last_sync, filters, need):
+        """getChangesToSend(backend, have, need) for a non-empty `have` (sync.js:246-306). last_sync: the union of the
+        have entries' lastSync hashes in first-seen order; filters: parsed Bloom filters (objects with num_entries,
+        num_probes and bits, like sync.BloomFilter). Returns (changes, hashes): the changes to send in the reference's
+        order and their hashes (hex). Raises Unsupported for a filter with more than 64 probes."""
+        hs = b''.join(bytes.fromhex(h) for h in last_sync)
+        nd = b''.join(bytes.fromhex(h) for h in need)
+        keep = [bytes(f.bits) for f in filters]   # alive until the call returns
+        arr = (_Bloom * max(len(filters), 1))()
+        for i, (f, bits) in enumerate(zip(filters, keep)):
+            arr[i].num_entries, arr[i].num_probes, arr[i].bits_len = f.num_entries, f.num_probes, len(bits)
+            arr[i].bits = C.cast(C.c_char_p(bits), C.c_void_p) if bits else None
+        bc, bh, err = C.c_void_p(), C.c_void_p(), _ErrStruct()
+        self._lib.check(self._lib.L.amg_sync_changes_to_send(self.h, hs, C.c_size_t(len(last_sync)), arr, C.c_size_t(len(filters)),
+                                                             nd, C.c_size_t(len(need)), C.byref(bc), C.byref(bh), C.byref(err)), err)
+        hx = self._buffers(bh)[0].hex()
+        return self._buffers(bc), [hx[i:i + 64] for i in range(0, len(hx), 64)]
+
+    def last_sync_ms(self):
+        """Device span of the last sync_bloom / sync_changes_to_send call (CUDA events), ms."""
+        return float(self._lib.L.amg_last_sync_ms(self.h))
 
     def dump_ops(self):
         rows, n, succ, m, err = C.c_void_p(), C.c_size_t(), C.c_void_p(), C.c_size_t(), _ErrStruct()

@@ -3,7 +3,8 @@
 The reference's sync.js hard-imports the JavaScript backend (sync.js:19), so a replacement backend has to bring these
 along (SURVEY.md section 8f, rank 3). This is host-side protocol logic: Bloom filter over change hashes, message and
 peer-state encoding, and the two state transitions; every document operation goes through the `Backend` facade
-(getHeads / getChanges / getChangeByHash / getMissingDeps / applyChanges), i.e. through the engine.
+(getHeads / getChanges / getChangeByHash / getMissingDeps / applyChanges), i.e. through the engine. The per-change work
+(the Bloom filter of a message, the changes to send) runs on the device when the document offers it (see Sync).
 
 Follows (paths relative to /root/reference): backend/sync.js:24-127 (BloomFilter), :130-227 (wire formats),
 :234-306 (makeBloomFilter, getChangesToSend), :308-478 (initSyncState, generateSyncMessage, advanceHeads,
@@ -11,7 +12,9 @@ receiveSyncMessage). Hashes are lowercase hex strings, messages and changes are 
 """
 import hashlib
 
+from .backend import backend_state
 from .columnar import inflate_change, uleb
+from .engine import Unsupported
 
 HASH_SIZE = 32
 MESSAGE_TYPE_SYNC = 0x42      # sync.js:25
@@ -200,15 +203,47 @@ def _change_meta(change):
 
 
 class Sync:
-    """The sync functions bound to a Backend facade (automerge_classic_b200.Backend or any object with its methods)."""
+    """The sync functions bound to a Backend facade (automerge_classic_b200.Backend or any object with its methods).
 
-    def __init__(self, backend_module):
+    With device=True (the default), the Bloom filter of a message and the choice of the changes to send run in the engine
+    when the document has the native methods (GpuBackendDoc.sync_bloom / sync_changes_to_send): from the change hashes it
+    already holds, instead of copying, inflating and hashing every change in Python. device=False, a document without
+    them (the oracle) or a filter the engine declines keep the host implementation below. Both give the same bytes."""
+
+    def __init__(self, backend_module, device=True):
         self.B = backend_module
+        self.device = device
+
+    def _native(self, backend, name):
+        if not self.device or not isinstance(backend, dict):
+            return None
+        fn = getattr(backend.get('state'), name, None)
+        if fn is not None:
+            backend_state(backend)   # an outdated handle fails as it does in the facade's getChanges
+        return fn
 
     # sync.js:234-238
     def _make_bloom_filter(self, backend, last_sync):
+        native = self._native(backend, 'sync_bloom')
+        if native is not None and isinstance(last_sync, (list, tuple)):
+            return {'lastSync': last_sync, 'bloom': native(list(last_sync))}
         new_changes = self.B.getChanges(backend, last_sync)
         return {'lastSync': last_sync, 'bloom': BloomFilter([_change_meta(c)['hash'] for c in new_changes]).bytes}
+
+    def _changes_to_send(self, backend, have, need):
+        """(changes, hashes) of getChangesToSend; hashes is None when the host path chose the changes."""
+        native = self._native(backend, 'sync_changes_to_send') if len(have) > 0 else None
+        if native is not None:
+            last_sync_hashes, bloom_filters = {}, []
+            for h in have:
+                for x in h['lastSync']:
+                    last_sync_hashes[x] = True
+                bloom_filters.append(BloomFilter(h['bloom']))   # parsing and its errors stay here
+            try:
+                return native(list(last_sync_hashes.keys()), bloom_filters, list(need))
+            except Unsupported:
+                pass   # a filter the device path declines (more than 64 probes): the host path answers
+        return self._get_changes_to_send(backend, have, need), None
 
     # sync.js:246-306
     def _get_changes_to_send(self, backend, have, need):
@@ -265,17 +300,22 @@ class Sync:
                 # the peer's last sync refers to changes we do not have (we lost state): ask for a fresh start
                 reset = {'heads': our_heads, 'need': [], 'have': [{'lastSync': [], 'bloom': b''}], 'changes': []}
                 return [sync_state, encodeSyncMessage(reset)]
-        changes_to_send = self._get_changes_to_send(backend, their_have, their_need) if isinstance(their_have, list) and isinstance(their_need, list) else []
+        changes_to_send, hashes = [], []
+        if isinstance(their_have, list) and isinstance(their_need, list):
+            changes_to_send, hashes = self._changes_to_send(backend, their_have, their_need)
         heads_unchanged = isinstance(last_sent_heads, list) and our_heads == last_sent_heads
         heads_equal = isinstance(their_heads, list) and our_heads == their_heads
         if heads_unchanged and heads_equal and len(changes_to_send) == 0:
             return [sync_state, None]
-        changes_to_send = [c for c in changes_to_send if _change_meta(c)['hash'] not in sent_hashes]
+        if hashes is None:
+            hashes = [_change_meta(c)['hash'] for c in changes_to_send]
+        keep = [k for k, h in enumerate(hashes) if h not in sent_hashes]
+        changes_to_send, hashes = [changes_to_send[k] for k in keep], [hashes[k] for k in keep]
         message = {'heads': our_heads, 'have': our_have, 'need': our_need, 'changes': changes_to_send}
         if changes_to_send:
             sent_hashes = dict(sent_hashes)
-            for c in changes_to_send:
-                sent_hashes[_change_meta(c)['hash']] = True
+            for h in hashes:
+                sent_hashes[h] = True
         new_state = dict(sync_state)
         new_state.update({'lastSentHeads': our_heads, 'sentHashes': sent_hashes})
         return [new_state, encodeSyncMessage(message)]

@@ -77,6 +77,20 @@ int amg_get_missing_deps(amg_backend* b, const uint8_t* heads, size_t n, amg_buf
 int amg_clock_of(amg_backend* b, const uint8_t* actor, size_t actor_len, uint64_t* seq_out, amg_error* err);
 int amg_hash_by_actor(amg_backend* b, const uint8_t* actor, size_t actor_len, uint64_t index, uint8_t hash_out[32], int* found, amg_error* err);
 
+/* sync.js:234-238 makeBloomFilter: the Bloom filter (BloomFilter(...).bytes, sync.js:38-76) over the hashes of
+ * getChanges(b, last_sync); last_sync = n hashes x 32 bytes. One buffer; empty when there are no such changes. The probes
+ * are set on the device from the hashes the engine holds; n == 0 (every change) does not build the host hash graph.
+ * An unknown hash fails like amg_get_changes ("hash not found"). */
+int amg_sync_bloom(amg_backend* b, const uint8_t* last_sync, size_t n, amg_buffers** out, amg_error* err);
+/* sync.js:246-306 getChangesToSend for have.length > 0. last_sync: the union of have[i].lastSync in first-seen order
+ * (n_last x 32 bytes); filters: n_filters already-parsed peer Bloom filters {num_entries, num_probes, bits, bits_len};
+ * need: n_need x 32 bytes. out_changes: the changes to send, in the reference's order; out_hashes: one buffer of
+ * 32-byte hashes back to back, one per returned change (the caller filters sentHashes with them). A filter with more than 64 probes
+ * fails with AMG_UNSUPPORTED (the caller answers from its host implementation instead). */
+typedef struct { uint32_t num_entries, num_probes; const uint8_t* bits; size_t bits_len; } amg_bloom;
+int amg_sync_changes_to_send(amg_backend* b, const uint8_t* last_sync, size_t n_last, const amg_bloom* filters, size_t n_filters,
+                             const uint8_t* need, size_t n_need, amg_buffers** out_changes, amg_buffers** out_hashes, amg_error* err);
+
 /* returned buffer lists */
 size_t amg_buffers_count(const amg_buffers* l);
 const uint8_t* amg_buffers_get(const amg_buffers* l, size_t i, size_t* len);
@@ -127,6 +141,9 @@ int amg_debug_dump_ops(amg_backend* b, uint64_t** rows_out, size_t* n, uint64_t*
  * the pieces, inflate + rest of the decode, gate, actors + seq + row finalisation, op set, patch groups + props, list index,
  * edits + copy-out, heads + commit), [12..23] host wall-clock marks (ms since the call started; [23] = the whole ABI call) */
 int amg_last_timings(amg_backend* b, float* ms_out, int n);
+/* device span of the last amg_sync_bloom / amg_sync_changes_to_send call in ms: CUDA events around its uploads, kernels and
+ * read-backs on the engine's main stream (host work in between included when the stream waits for it) */
+float amg_last_sync_ms(amg_backend* b);
 uint64_t amg_kernel_launches(amg_backend* b);
 /* labelled host wall-clock marks of the last applyChanges call ("label=ms ..."), development aid */
 size_t amg_debug_marks(amg_backend* b, char* buf, size_t cap);

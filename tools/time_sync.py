@@ -1,0 +1,109 @@
+"""Times the sync protocol on large documents: the device path (GpuBackendDoc.sync_bloom / sync_changes_to_send) against
+the host path (Sync(device=False)), which copies, inflates and hashes every change in Python.
+
+  (a) the first generateSyncMessage to a new peer (its Bloom filter covers every change)
+  (b) receiveSyncMessage + the next generateSyncMessage on the sender, when the peer's filter covers a random 99 % of the
+      changes (a few changes and their dependents go out; the filter in the reply is built again)
+  (c) (a) and (b) with device=False
+
+Wall clock per call: median of --reps repetitions (--host-reps for the host path) with the same sync state each time
+(neither call changes the document). Next to it: the device span of the engine's sync calls inside (CUDA events), and the
+one-time host hash graph (ensureGraph: getMissingDeps and getChangeByHash build it on their first call), timed on a fresh
+copy of the document.
+
+  python tools/time_sync.py [--c3-ops 1000000] [--c4-ops 100000] [--reps 5] [--host-reps 1] [--out FILE.json]
+"""
+import argparse
+import json
+import os
+import random
+import statistics
+import sys
+import time
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from automerge_classic_b200 import bind_sync, sync, tracegen   # noqa: E402
+from automerge_classic_b200.backend import Backend as Facade   # noqa: E402
+from automerge_classic_b200.engine import GpuBackendDoc   # noqa: E402
+
+
+class TimedDoc(GpuBackendDoc):
+    """Adds up the device span of every native sync call."""
+    device_ms = 0.0
+
+    def sync_bloom(self, last_sync):
+        out = super().sync_bloom(last_sync)
+        self.device_ms += self.last_sync_ms()
+        return out
+
+    def sync_changes_to_send(self, last_sync, filters, need):
+        out = super().sync_changes_to_send(last_sync, filters, need)
+        self.device_ms += self.last_sync_ms()
+        return out
+
+
+def timed(fn, doc, reps):
+    walls, devs, out = [], [], None
+    for _ in range(reps):
+        doc.device_ms = 0.0
+        t0 = time.perf_counter()
+        out = fn()
+        walls.append((time.perf_counter() - t0) * 1e3)
+        devs.append(doc.device_ms)
+    return {'wall_ms': statistics.median(walls), 'device_ms': statistics.median(devs), 'reps': reps}, out
+
+
+def run(cfg, n_ops, n_actors, reps, host_reps):
+    t = tracegen.generate(cfg, n_ops, n_actors)
+    def fresh():
+        d = TimedDoc()
+        d.apply_packed_flat(t.blob, t.offsets, t.n_changes, want_patch=False)
+        return {'state': d, 'heads': d.heads()}
+    res = {'config': cfg, 'ops': t.n_ops, 'changes': t.n_changes, 'change_bytes': int(t.offsets[-1])}
+    g = fresh()
+    t0 = time.perf_counter()
+    g['state'].get_missing_deps([])
+    res['ensure_graph_ms'] = (time.perf_counter() - t0) * 1e3
+    del g
+    a = fresh()
+    a['state'].get_missing_deps([])   # the graph is built once per document; (a) and (b) are timed after that
+    hashes = a['state'].sync_changes_to_send([], [sync.BloomFilter(b'')], [])[1]
+    rnd = random.Random(99)
+    peer = {'heads': [], 'need': [], 'changes': [],
+            'have': [{'lastSync': [], 'bloom': sync.BloomFilter([h for h in hashes if rnd.random() < 0.99]).bytes}]}
+    reply = sync.encodeSyncMessage(peer)
+    msgs = {}
+    for name, device, r in (('device', True, reps), ('host', False, host_reps)):
+        B = bind_sync(Facade(TimedDoc), device=device)
+        (ta, (s1, m1)) = timed(lambda: B.generateSyncMessage(a, B.initSyncState()), a['state'], r)
+        def step_b():
+            _, s2, _ = B.receiveSyncMessage(a, s1, reply)
+            return B.generateSyncMessage(a, s2)
+        (tb, (_, m2)) = timed(step_b, a['state'], r)
+        msgs[name] = (m1, m2)
+        res['a_' + name], res['b_' + name] = ta, tb
+        res['b_changes_sent'] = len(sync.decodeSyncMessage(m2)['changes'])
+        print('%s %s: (a) %.1f ms wall, %.2f ms device | (b) %.1f ms wall, %.2f ms device' % (cfg, name, ta['wall_ms'], ta['device_ms'], tb['wall_ms'], tb['device_ms']), flush=True)
+    res['messages_equal'] = msgs['device'] == msgs['host']
+    assert res['messages_equal'], 'device and host messages differ'
+    print('%s: %d changes, ensureGraph %.1f ms, (b) sends %d changes, messages identical' % (cfg, t.n_changes, res['ensure_graph_ms'], res['b_changes_sent']), flush=True)
+    return res
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--c3-ops', type=int, default=1000000)
+    ap.add_argument('--c4-ops', type=int, default=100000)
+    ap.add_argument('--reps', type=int, default=5)
+    ap.add_argument('--host-reps', type=int, default=1)
+    ap.add_argument('--out')
+    args = ap.parse_args()
+    out = [run('C3', args.c3_ops, 10, args.reps, args.host_reps), run('C4', args.c4_ops, 100, args.reps, args.host_reps)]
+    if args.out:
+        with open(args.out, 'w') as f:
+            json.dump(out, f, indent=1)
+    print(json.dumps(out))
+
+
+if __name__ == '__main__':
+    main()
