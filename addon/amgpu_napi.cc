@@ -196,6 +196,37 @@ napi_value SyncChangesToSend(napi_env env, napi_callback_info info) {
   napi_set_element(env, out, 0, buffersToJs(env, changes)); napi_set_element(env, out, 1, hs);
   return out;
 }
+// decodeChanges(Uint8Array[]) — columnar.js:770-776 decodeChange of every entry (one change container each), in one call on
+// a per-process backend handle. Returns the change table (layout: amgpu.h) as one Uint8Array; an error carries the index of
+// the failing change as `failedIndex`.
+napi_value DecodeChanges(napi_env env, napi_callback_info info) {
+  napi_value argv[1]; if (!getArgs(env, info, 1, argv)) return nullptr;
+  bool isArray = false; napi_is_array(env, argv[0], &isArray);
+  if (!isArray) { napi_throw_type_error(env, nullptr, "decodeChanges takes an array of Uint8Arrays"); return nullptr; }
+  uint32_t n = 0; napi_get_array_length(env, argv[0], &n);
+  std::string blob; std::vector<uint64_t> offsets(n + 1, 0);
+  for (uint32_t i = 0; i < n; i++) {
+    napi_value el; napi_get_element(env, argv[0], i, &el);
+    const uint8_t* p; size_t len; if (!getBytes(env, el, &p, &len)) return nullptr;
+    blob.append(reinterpret_cast<const char*>(p), len); offsets[i + 1] = blob.size();
+  }
+  static amg_backend* decoder = nullptr;
+  amg_error err;
+  if (!decoder && !(decoder = amg_init(deviceFromEnv(), &err))) return throwAmg(env, err);
+  amg_buffers* l = nullptr; size_t failed = 0;
+  if (amg_decode_changes(decoder, reinterpret_cast<const uint8_t*>(blob.data()), offsets.data(), n, &l, &failed, &err)) {
+    // the reference's error class and message, with the index of the failing change as `failedIndex`
+    napi_value msg, e, idx; napi_create_string_utf8(env, err.msg, NAPI_AUTO_LENGTH, &msg);
+    if (err.code == AMG_RANGE_ERROR) napi_create_range_error(env, nullptr, msg, &e);
+    else if (err.code == AMG_TYPE_ERROR) napi_create_type_error(env, nullptr, msg, &e);
+    else napi_create_error(env, nullptr, msg, &e);
+    napi_create_double(env, (double)failed, &idx); napi_set_named_property(env, e, "failedIndex", idx);
+    napi_throw(env, e); return nullptr;
+  }
+  napi_value el; napi_get_element(env, buffersToJs(env, l), 0, &el); return el;
+}
+// decodeHistory(state) — decodeChanges(getAllChanges(state)), read from device memory: the change table as one Uint8Array
+napi_value DecodeHistory(napi_env env, napi_callback_info info) { return listCall(env, info, amg_decode_history, true); }
 // Backend.free — backend/backend.js:16-19: releases the device memory now instead of at garbage collection
 napi_value Free(napi_env env, napi_callback_info info) {
   napi_value argv[1]; Holder* h; if (!getArgs(env, info, 1, argv) || !getHolder(env, argv[0], &h)) return nullptr;
@@ -208,7 +239,7 @@ napi_value InitModule(napi_env env, napi_value exports) {
     {"init", Init}, {"load", Load}, {"clone", Clone}, {"free", Free}, {"applyChanges", ApplyChanges}, {"getPatch", GetPatch}, {"save", Save},
     {"getHeads", GetHeads}, {"getChanges", GetChanges}, {"getChangesAdded", GetChangesAdded}, {"getChangeByHash", GetChangeByHash},
     {"getMissingDeps", GetMissingDeps}, {"clockOf", ClockOf}, {"hashByActor", HashByActor}, {"syncBloom", SyncBloom},
-    {"syncChangesToSend", SyncChangesToSend}};
+    {"syncChangesToSend", SyncChangesToSend}, {"decodeChanges", DecodeChanges}, {"decodeHistory", DecodeHistory}};
   for (auto& f : fns) { napi_value fn; napi_create_function(env, f.name, NAPI_AUTO_LENGTH, f.fn, nullptr, &fn); napi_set_named_property(env, exports, f.name, fn); }
   return exports;
 }

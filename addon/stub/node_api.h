@@ -36,6 +36,11 @@ napi_status napi_get_cb_info(napi_env env, napi_callback_info cbinfo, size_t* ar
 napi_status napi_get_value_bool(napi_env env, napi_value value, bool* result);
 napi_status napi_get_value_double(napi_env env, napi_value value, double* result);
 napi_status napi_create_double(napi_env env, double value, napi_value* result);
+napi_status napi_create_string_utf8(napi_env env, const char* str, size_t length, napi_value* result);
+napi_status napi_create_error(napi_env env, napi_value code, napi_value msg, napi_value* result);
+napi_status napi_create_range_error(napi_env env, napi_value code, napi_value msg, napi_value* result);
+napi_status napi_create_type_error(napi_env env, napi_value code, napi_value msg, napi_value* result);
+napi_status napi_throw(napi_env env, napi_value error);
 napi_status napi_remove_wrap(napi_env env, napi_value js_object, void** result);
 napi_status napi_create_function(napi_env env, const char* utf8name, size_t length, napi_callback cb, void* data, napi_value* result);
 napi_status napi_set_named_property(napi_env env, napi_value object, const char* utf8name, napi_value value);

@@ -5,7 +5,7 @@
 The module object `Backend` mirrors the module a caller hands to `Automerge.setDefaultBackend()`.
 """
 from .backend import Backend as _Facade
-from .engine import GpuBackendDoc, AmgError, Unsupported
+from .engine import GpuBackendDoc, AmgError, Unsupported, decode_changes as _decode_changes, _decoder_for
 
 from . import sync as _sync
 
@@ -20,5 +20,15 @@ def bind_sync(facade, device=True):
     return facade
 
 
+def decodeChanges(binary_changes):
+    """Automerge.decodeChanges (columnar.js:843-857) on the device: a list of change objects."""
+    return _decode_changes(binary_changes)
+
+
+def decodeChange(buf):
+    """Automerge.decodeChange (columnar.js:770-776, src/automerge.js:154): one binary change -> its change object."""
+    return _decoder_for(GpuBackendDoc).decode_changes_flat([buf]).to_changes()[0]
+
+
 Backend = bind_sync(_Facade(GpuBackendDoc))
-__all__ = ['Backend', 'GpuBackendDoc', 'AmgError', 'Unsupported', 'bind_sync']
+__all__ = ['Backend', 'GpuBackendDoc', 'AmgError', 'Unsupported', 'bind_sync', 'decodeChange', 'decodeChanges']

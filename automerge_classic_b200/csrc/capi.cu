@@ -233,6 +233,25 @@ int amg_sync_changes_to_send(amg_backend* b, const uint8_t* last_sync, size_t n_
     *out_changes = gc.release(); *out_hashes = gh.release(); return 0;)
 }
 float amg_last_sync_ms(amg_backend* b) { return b->eng.lastSyncMs; }
+// columnar.js:770-776 decodeChange over n change containers, into one change table
+int amg_decode_changes(amg_backend* b, const uint8_t* blob, const uint64_t* offsets, size_t n, amg_buffers** out, size_t* failed_index, amg_error* err) {
+  if (failed_index) *failed_index = 0;
+  try {
+    auto* l = new amg_buffers(); std::unique_ptr<amg_buffers> guard(l); l->items.emplace_back();
+    b->eng.decodeChanges(blob, (const u64*)offsets, n, false, l->items.back());
+    *out = guard.release(); return 0;
+  } catch (amg::Error& e) { amg::drop_pending_peeks(); if (failed_index) *failed_index = b->eng.decodeFailed; setErr(err, e.code, e.what()); return e.code; }
+  catch (std::exception& e) { amg::drop_pending_peeks(); setErr(err, AMG_INTERNAL_ERROR, e.what()); return AMG_INTERNAL_ERROR; }
+}
+// the same for every applied change, in getAllChanges order (new.js:1925-1927), read from device memory
+int amg_decode_history(amg_backend* b, amg_buffers** out, amg_error* err) {
+  AMG_GUARD(
+    auto* l = new amg_buffers(); std::unique_ptr<amg_buffers> guard(l); l->items.emplace_back();
+    if (!b->eng.loaded.haveHashGraph) b->eng.computeHashGraph();   // (new.js:1922) before the change count is taken
+    b->eng.decodeChanges(nullptr, nullptr, b->eng.changes.size(), true, l->items.back());
+    *out = guard.release(); return 0;)
+}
+float amg_last_decode_ms(amg_backend* b) { return b->eng.lastDecodeMs; }
 // new.js:1979-1997
 int amg_get_changes_added(amg_backend* bn, amg_backend* bo, amg_buffers** out, amg_error* err) {
   AMG_GUARD(

@@ -366,8 +366,8 @@ inline void sha_range(Ctx& c, const ShaTilesArgs& a, bool onSide) {
 }
 
 // number of values in an RLE column (record-level: runs are not expanded); *err receives a KErr
-template <class S> HD u32 rle_count_values_t(const S& src, u32 off, u32 end, u32* err) {
-  RleReaderT<S> a(src, off, end, 0); u64 n = 0;
+template <class S> HD u32 rle_count_values_t(const S& src, u32 off, u32 end, u32* err, int type = 0 /* 0 uint, 1 int, 2 utf8 */) {
+  RleReaderT<S> a(src, off, end, type); u64 n = 0;
   while (!a.done() && !a.r.err) {
     long long v; u32 o, l; a.next(v, o, l);
     u64 adv = 1;
@@ -390,6 +390,17 @@ template <class S> HD u64 rle_sum_values_t(const S& src, u32 off, u32 end, u32 l
   *err = pn.r.err; return sum;
 }
 HD u32 rle_count_values(const u8* arena, u32 off, u32 end, u32* err) { return rle_count_values_t(PtrSrc{arena}, off, end, err); }
+// decodeValue (columnar.js:300-329) of the payload arena[valOff, valOff + (valLen >> 4)): numbers must be complete LEB128
+// values within 53 bits, floating point payloads must be 8 bytes. Returns a KErr (0 = the value decodes).
+HD u32 decode_value_error(const u8* arena, u32 valLen, u32 valOff) {
+  const u32 tag = valLen & 15, n = valLen >> 4;
+  if (tag == 3 || tag == 4 || tag == 8 || tag == 9) {
+    ByteReader r(arena, valOff, valOff + n);
+    if (tag == 3) r.uleb(); else r.sleb();
+    return r.err;
+  }
+  return tag == 5 && n != 8 ? (u32)KE_FLOAT_LEN : 0u;
+}
 HD u64 rle_sum_values(const u8* arena, u32 off, u32 end, u32 limit, u32* err) { return rle_sum_values_t(PtrSrc{arena}, off, end, limit, err); }
 
 // ---------------------------------------------------------------- header / column directory parse, one thread per change

@@ -28,6 +28,7 @@
 #include "doccols.cuh"
 #include "history.cuh"
 #include "sync.cuh"
+#include "changes.cuh"
 #include "unknowncols.hpp"
 
 namespace amg {
@@ -433,6 +434,22 @@ class Engine {
   void gatherHashes(const std::vector<u32>& idx, std::string& out);   // 32 bytes per change
   float lastSyncMs = 0;   // device span (CUDA events on the main stream) of the last sync call's uploads, kernels and read-backs (0 in the emulation build)
   DBuf<u32> syncIdx, syncBits; DBuf<u8> syncFilterBits, syncNeg, syncHashOut; DBuf<BloomRef> syncFilters;
+
+  // ---------------------------------------------------------------- decodeChange / decodeChanges (changes.cuh)
+  // n change containers into one flat change table (layout: include/amgpu.h). Source: the caller's blob (staged into scratch,
+  // DEFLATEd changes inflated on the device behind it) or, with history, every applied change read in place from the arena.
+  // The document is not touched. On error, decodeFailed names the change.
+  struct DecodeCall {
+    size_t n = 0; const u8* ar = nullptr; bool history = false;
+    u32 tot[4] = {0, 0, 0, 0};   // ops, preds, actor table entries, bytes
+    size_t changesOff = 0, opsOff = 0, predsOff = 0, actorsOff = 0, bytesOff = 0, size = 0;   // sections of the table
+  };
+  void decodeChanges(const u8* blob, const u64* offsets, size_t n, bool history, std::string& out);
+  void stageDecodeInput(DecodeCall& d, const u8* blob, const u64* offsets), inflateDecodeInput(DecodeCall& d), decodeTable(DecodeCall& d, std::string& out);
+  [[noreturn]] void throwDecodeError(DecodeCall& d, const u64* words);
+  size_t decodeFailed = 0; float lastDecodeMs = 0;   // failing change of the last call; its device span (CUDA events; 0 in the emulation build)
+  DBuf<u8> dcArena, dcHash, dcOut; DBuf<u32> dcOff, dcLen, dcCLen, dcOps, dcPreds, dcActors, dcBytes, dcOpBase, dcPredBase, dcActorBase, dcByteBase, dcColOff, dcColLen, dcRows, dcChld;
+  DBuf<ChangeMeta> dcMeta; DBuf<u64> dcErr, dcTotals; DBuf<u32> dcDefl;
  private:
   void uploadCandidates(const u32* idx, size_t count);
   void syncTimer(bool start);

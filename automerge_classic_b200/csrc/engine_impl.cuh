@@ -1890,6 +1890,163 @@ inline void Engine::syncChangesToSend(const u32* idx, size_t count, const std::v
   }
 }
 
+// ------------------------------------------------------------ decodeChange / decodeChanges (changes.cuh)
+inline void Engine::decodeChanges(const u8* blob, const u64* offsets, size_t n, bool history, std::string& out) {
+  DecodeCall d; d.n = n; d.history = history; decodeFailed = 0; lastDecodeMs = 0;
+  const float keepSyncMs = lastSyncMs; lastSyncMs = 0;
+  struct Restore { Engine& e; float ms; ~Restore() { e.lastSyncMs = ms; } } restore{*this, keepSyncMs};   // the timer is shared with the sync calls
+  syncTimer(true);
+  dcErr.ensure(ctx, DP_NUM); dev_memset(ctx, dcErr.p, 0, DP_NUM * 8);
+  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+  dcOff.ensure(ctx, n + 1); dcLen.ensure(ctx, n + 1); dcHash.ensure(ctx, n * 32 + 64);
+  if (history) {   // every applied change (getAllChanges order), inflated copies in place; their hashes are the engine's
+    if (!loaded.haveHashGraph) computeHashGraph();
+    if (n) {
+      chPairs.ensure(ctx, n); h2d(ctx, chPairs.p, changes.data(), n * sizeof(HostChange));
+      foreach(ctx, n, SplitPairsKernel{chPairs.p, dcOff.p, dcLen.p});
+      d2d(ctx, dcHash.p, hashes.p, n * 32);
+    }
+    d.ar = arena.p;
+  } else {
+    stageDecodeInput(d, blob, offsets);
+    inflateDecodeInput(d);
+    d.ar = dcArena.p;
+  }
+  decodeTable(d, out);
+  syncTimer(false); lastDecodeMs = lastSyncMs;
+}
+
+// the caller's bytes into scratch (never into the document's arena): device memory is copied device to device, host
+// memory (pinned or pageable) uploaded
+inline void Engine::stageDecodeInput(DecodeCall& d, const u8* blob, const u64* offsets) {
+  const size_t n = d.n; const u64 total = n ? offsets[n] - offsets[0] : 0;
+  if (total + 64 >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: change arena limited to 4 GiB per call");
+  dcArena.ensure(ctx, total + 64);
+  bool onDevice = false;
+#ifndef AMG_EMU
+  if (n) { cudaPointerAttributes at; if (cudaPointerGetAttributes(&at, blob + offsets[0]) == cudaSuccess) onDevice = at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged; else cudaGetLastError(); }
+#endif
+  if (onDevice) d2d(ctx, dcArena.p, blob + offsets[0], total); else h2d(ctx, dcArena.p, blob + offsets[0], total);
+  dev_memset(ctx, dcArena.p + total, 0, 64);
+  std::vector<u32> ol(2 * n + 2);
+  for (size_t i = 0; i < n; i++) { ol[i] = (u32)(offsets[i] - offsets[0]); ol[n + i] = (u32)(offsets[i + 1] - offsets[i]); }
+  h2d(ctx, dcOff.p, ol.data(), n * 4); h2d(ctx, dcLen.p, ol.data() + n, n * 4);
+  d.tot[3] = (u32)total;   // bytes staged so far: DEFLATEd changes are inflated behind them
+}
+
+// DEFLATEd entries (columnar.js:742) inflated on the device, behind the staged bytes: the sequence of inflateBatch (flag ->
+// scan -> list -> k_inflate into scratch -> scan -> k_inflate in place). Their offsets are re-pointed to the inflated copies.
+inline void Engine::inflateDecodeInput(DecodeCall& d) {
+  const size_t B = d.n; if (B == 0) return;
+  emit.ensure(ctx, B + 1); slot.ensure(ctx, B + 2); dcDefl.ensure(ctx, B + 1);   // (own list: benchDecode re-reads the apply path's deflList)
+  dev_memset(ctx, flagWord.p + 8, 0, 4);
+  foreach(ctx, B, DeflateFlagKernel{dcArena.p, dcOff.p, dcLen.p, emit.p, flagWord.p + 8});
+  scan_exclusive(ctx, scanTmp, emit.p, slot.p, B);
+  u32 nd32 = 0, deflBytes = 0; readU32x2(slot.p + B, flagWord.p + 8, &nd32, &deflBytes);
+  const size_t nd = nd32; if (nd == 0) return;
+  foreach(ctx, B, CompactKernel{emit.p, slot.p, dcDefl.p});
+  inflLen.ensure(ctx, nd + 1); inflOff.ensure(ctx, nd + 2); patchTriples.ensure(ctx, 2 * nd + 2); inflCap.ensure(ctx, nd + 2); inflCapOff.ensure(ctx, nd + 2); inflOvf.ensure(ctx, nd + 1);
+  u32 factor = 4; while (factor > 1 && (u64)factor * deflBytes + 1024ull * nd >= 0xf0000000ULL) factor--;
+  inflScratch.ensure(ctx, (size_t)factor * deflBytes + 1024 * nd + 64);
+  foreach(ctx, nd, InflateCapKernel{dcDefl.p, dcLen.p, factor, inflCap.p});
+  scan_exclusive(ctx, scanTmp, inflCap.p, inflCapOff.p, nd);
+  InflateArgs ia{dcArena.p, dcOff.p, dcLen.p, dcDefl.p, nd, inflLen.p, nullptr, 0u, patchTriples.p, patchTriples.p + nd, inflScratch.p, inflCapOff.p, inflOvf.p, dcErr.p + DP_INFLATE};
+  inflate_changes(ctx, INFL_SPECULATE, ia);
+  scan_exclusive(ctx, scanTmp, inflLen.p, inflOff.p, nd);
+  const size_t extra = readU32(inflOff.p + nd), start = d.tot[3];
+  if ((u64)start + extra + 64 >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: change arena limited to 4 GiB per call");
+  dcArena.ensure(ctx, start + extra + 64, start);
+  ia.arena = dcArena.p; ia.outOff = inflOff.p; ia.extraStart = (u32)start;
+  inflate_changes(ctx, INFL_PLACE, ia);
+  dev_memset(ctx, dcArena.p + start + extra, 0, 64);
+  foreach(ctx, nd, InflatePatchKernel{dcDefl.p, inflLen.p, inflOff.p, (u32)start, dcOff.p, dcLen.p});
+  d.tot[3] = (u32)(start + extra);
+}
+
+inline void Engine::decodeTable(DecodeCall& d, std::string& out) {
+  const size_t n = d.n; const u8* ar = d.ar;
+  dcCLen.ensure(ctx, n + 1); dcMeta.ensure(ctx, n + 1); dcColOff.ensure(ctx, (size_t)CHG_COLS * n + 1); dcColLen.ensure(ctx, (size_t)CHG_COLS * n + 1);
+  for (auto* b : {&dcOps, &dcPreds, &dcActors, &dcBytes, &dcOpBase, &dcPredBase, &dcActorBase, &dcByteBase}) b->ensure(ctx, n + 2);
+  foreach(ctx, n, ChgContainerKernel{ar, dcOff.p, dcLen.p, dcCLen.p, dcErr.p + DP_CONTAINER});
+  if (!d.history) foreach(ctx, n, ShaKernel{ar, dcOff.p, dcCLen.p, dcHash.p, dcErr.p + DP_SHA, nullptr, nullptr});
+  foreach(ctx, n, ChgHeaderKernel{ar, dcOff.p, dcLen.p, dcCLen.p, dcHash.p, dcMeta.p, dcColOff.p, dcColLen.p, dcOps.p, dcPreds.p, dcActors.p, dcBytes.p, n, dcErr.p + DP_HEADER});
+  scan_exclusive(ctx, scanTmp, dcOps.p, dcOpBase.p, n); scan_exclusive(ctx, scanTmp, dcPreds.p, dcPredBase.p, n);
+  scan_exclusive(ctx, scanTmp, dcActors.p, dcActorBase.p, n); scan_exclusive(ctx, scanTmp, dcBytes.p, dcByteBase.p, n);
+  // the scans are 32-bit: their totals are only used once the 64-bit sums show that nothing wrapped (bytes: at most the
+  // staged input or the arena, both below 4 GiB)
+  dcTotals.ensure(ctx, 3); dev_memset(ctx, dcTotals.p, 0, 3 * 8);
+  foreach(ctx, n, ChgTotalsKernel{dcOps.p, dcPreds.p, dcActors.p, dcTotals.p});
+  u64 t64[3] = {0, 0, 0}; void* dst[4] = {&t64[0], &t64[1], &t64[2], &d.tot[3]};
+  readWords({{dcTotals.p, 8}, {dcTotals.p + 1, 8}, {dcTotals.p + 2, 8}, {dcByteBase.p + n, 4}}, dst);
+  if (t64[0] >= 0x7fffffffULL || t64[1] >= 0x7fffffffULL || t64[2] >= 0x7fffffffULL)
+    throw Error(AMG_ERR_UNSUPPORTED, "amgpu: more than 2^31 operations, preds or actor table entries in one decodeChanges call");
+  for (int k = 0; k < 3; k++) d.tot[k] = (u32)t64[k];
+  const size_t M = d.tot[0], P = d.tot[1], A = d.tot[2], Bt = d.tot[3];
+  auto align8 = [](size_t v) { return (v + 7) & ~(size_t)7; };
+  d.changesOff = CHG_HDR_WORDS * 8; d.opsOff = d.changesOff + n * sizeof(ChangeRec); d.predsOff = d.opsOff + M * sizeof(OpRec);
+  d.actorsOff = d.predsOff + P * 8; d.bytesOff = d.actorsOff + A * sizeof(ActorRef); d.size = align8(d.bytesOff + Bt);
+  if (d.size >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: a change table is limited to 4 GiB");
+  dcOut.ensure(ctx, d.size + 64);
+  const u64 hdr[CHG_HDR_WORDS] = {CHG_MAGIC, n, d.changesOff, M, d.opsOff, P, d.predsOff, A, d.actorsOff, d.bytesOff, Bt, 0};
+  h2d(ctx, dcOut.p, hdr, sizeof(hdr)); sync(ctx);   // (hdr lives on this stack frame)
+  // SoA rows: the 12 columns of RawRows over M ops, then predActor / predCtr over P preds; child columns
+  dcRows.ensure(ctx, 12 * (M + 1) + 2 * (P + 1)); dcChld.ensure(ctx, 2 * (M + 1));
+  u32* r = dcRows.p; const size_t Ms = M + 1;
+  RawRows raw{r, r + Ms, r + 2 * Ms, r + 3 * Ms, r + 4 * Ms, r + 5 * Ms, r + 6 * Ms, r + 7 * Ms, r + 8 * Ms, r + 9 * Ms, r + 10 * Ms, r + 11 * Ms, r + 12 * Ms, r + 12 * Ms + P + 1};
+  foreach(ctx, (size_t)NCOLS * n, ChgColumnsKernel{ar, dcColOff.p, dcColLen.p, dcOps.p, dcPreds.p, dcOpBase.p, dcPredBase.p, n, raw, dcChld.p, dcChld.p + Ms, dcErr.p + DP_COLUMNS});
+  u8* o = dcOut.p;
+  foreach(ctx, n, ChgRecordKernel{ar, dcMeta.p, dcHash.p, dcOps.p, dcActors.p, dcOpBase.p, dcPredBase.p, dcActorBase.p, dcByteBase.p, (u64)d.bytesOff,
+                                  reinterpret_cast<ChangeRec*>(o + d.changesOff), reinterpret_cast<ActorRef*>(o + d.actorsOff)});
+  foreach(ctx, (Bt + 63) / 64, ChgBytesKernel{ar, dcOff.p, dcByteBase.p, n, (u32)Bt, o + d.bytesOff});
+  foreach(ctx, M, ChgOpKernel{ar, dcOff.p, dcOpBase.p, n, raw, dcChld.p, dcChld.p + Ms, dcColOff.p, dcColLen.p, dcActors.p, dcActorBase.p, dcByteBase.p, (u64)d.bytesOff,
+                              o, reinterpret_cast<const ActorRef*>(o + d.actorsOff), reinterpret_cast<OpRec*>(o + d.opsOff), reinterpret_cast<u32*>(o + d.predsOff), dcErr.p + DP_OPS});
+  u64 w[DP_NUM] = {0}; void* wd[DP_NUM]; for (int k = 0; k < DP_NUM; k++) wd[k] = &w[k];
+  readWords({{dcErr.p, 8}, {dcErr.p + 1, 8}, {dcErr.p + 2, 8}, {dcErr.p + 3, 8}, {dcErr.p + 4, 8}, {dcErr.p + 5, 8}}, wd);
+  for (int k = 0; k < DP_NUM; k++) if (w[k]) throwDecodeError(d, w);
+  out.resize(d.size);
+  d2h(ctx, &out[0], dcOut.p, d.size); sync(ctx);
+}
+
+// The change the sequential reference fails on first: the smallest failing change over all phases (op errors are keyed by
+// op: mapped to their change), and for it the error of its earliest phase.
+inline void Engine::throwDecodeError(DecodeCall& d, const u64* w) {
+  const size_t n = d.n; std::vector<u32> opBase(n + 1); d2h(ctx, opBase.data(), dcOpBase.p, (n + 1) * 4); sync(ctx);
+  size_t best = SIZE_MAX; int phase = -1;
+  for (int k = 0; k < DP_NUM; k++) {
+    if (!w[k]) continue;
+    size_t c = (size_t)(w[k] >> 8);
+    if (k == DP_OPS) c = (size_t)(std::upper_bound(opBase.begin(), opBase.end(), (u32)c) - opBase.begin()) - 1;
+    if (c < best) { best = c; phase = k; }
+  }
+  decodeFailed = best; const u32 code = (u32)(w[phase] & 0xff);
+  auto actorIndex = [](u32 a) { return "No actor index " + std::to_string(a); };
+  if (code == DE_CHUNK_TYPE_N) {
+    u32 off = 0; d2h(ctx, &off, dcOff.p + best, 4); sync(ctx); u8 t = 0; d2h(ctx, &t, d.ar + off + 8, 1); sync(ctx);
+    throw Error(AMG_ERR_RANGE, "Unexpected chunk type: " + std::to_string(t));
+  }
+  if (phase == DP_OPS) {
+    const size_t g = (size_t)(w[phase] >> 8); OpRec o; d2h(ctx, &o, dcOut.p + d.opsOff + g * sizeof(OpRec), sizeof(OpRec)); sync(ctx);
+    auto txt = [](u32 v) { return v == NULL32 ? std::string("None") : std::to_string(v); };
+    switch (code) {
+      case DE_OBJ_ACTOR: throw Error(AMG_ERR_RANGE, actorIndex(o.objActor));
+      case DE_KEY_ACTOR: throw Error(AMG_ERR_RANGE, actorIndex(o.keyActor));
+      case DE_CHLD_ACTOR: throw Error(AMG_ERR_RANGE, actorIndex(o.chldActor));
+      case DE_PRED_ACTOR: {
+        std::vector<u32> pr(2 * (size_t)o.predNum + 2); d2h(ctx, pr.data(), dcOut.p + d.predsOff + (size_t)o.predFirst * 8, (size_t)o.predNum * 8);
+        u32 na = 0; d2h(ctx, &na, dcActors.p + o.change, 4); sync(ctx);
+        for (u32 j = 0; j < o.predNum; j++) if (pr[2 * j] != NULL32 && pr[2 * j] >= na) throw Error(AMG_ERR_RANGE, actorIndex(pr[2 * j]));
+        break;
+      }
+      case DE_CHLD_MISMATCH: throw Error(AMG_ERR_RANGE, "Mismatched child columns: " + txt(o.chldCtr) + " and " + txt(o.chldActor));
+      case DE_PRED_ORDER: throw Error(AMG_ERR_RANGE, "operation IDs are not in ascending order");
+      case DE_PRED_NULL: throw Error(AMG_ERR_UNSUPPORTED, "amgpu: a pred list that orders a null operation ID (the reference compares null with a number)");
+      case KE_FLOAT_LEN: throw Error(AMG_ERR_RANGE, "Invalid length for floating point number: " + std::to_string(o.valLen >> 4));
+      default: break;
+    }
+  }
+  throwKernelError(w[phase]);
+}
+
 inline void Engine::gatherHashes(const std::vector<u32>& idx, std::string& out) {
   out.assign(idx.size() * 32, '\0');
   if (idx.empty()) return;

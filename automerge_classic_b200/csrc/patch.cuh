@@ -41,12 +41,7 @@ struct PatchBytesGatherKernel {
   // decodeValue (columnar.js:300-329) runs in the reference whenever a value reaches a patch: numbers must be complete
   // LEB128 values within 53 bits, floating point payloads must be 8 bytes
   HD void validate(u32 valLen, u32 valOff, size_t i) const {
-    const u32 tag = valLen & 15, n = valLen >> 4;
-    if (tag == 3 || tag == 4 || tag == 8 || tag == 9) {
-      ByteReader r(arena, valOff, valOff + n);
-      if (tag == 3) r.uleb(); else r.sleb();
-      if (r.err) raise(errWord, r.err, i);
-    } else if (tag == 5 && n != 8) raise(errWord, KE_FLOAT_LEN, i);
+    if (const u32 e = decode_value_error(arena, valLen, valOff)) raise(errWord, e, i);
   }
   HD void operator()(size_t i) const {
     u32 at = off[i];

@@ -82,6 +82,12 @@ class Library:
         L.amg_sync_changes_to_send.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, vp, C.c_size_t, vp, vp, vp]
         L.amg_last_sync_ms.restype = C.c_float
         L.amg_last_sync_ms.argtypes = [vp]
+        L.amg_decode_changes.restype = C.c_int
+        L.amg_decode_changes.argtypes = [vp, vp, vp, C.c_size_t, vp, vp, vp]
+        L.amg_decode_history.restype = C.c_int
+        L.amg_decode_history.argtypes = [vp, vp, vp]
+        L.amg_last_decode_ms.restype = C.c_float
+        L.amg_last_decode_ms.argtypes = [vp]
 
     def check(self, rc, err):
         if rc != 0:
@@ -246,6 +252,83 @@ class FlatPatch:
                 edits.append({'action': 'insert', 'index': index, 'elemId': self.op_id(self.edit_elem[j]), 'opId': self.op_id(rec['opId']), 'value': value})
         out = self.header()
         out['diffs'] = patches['_root']
+        return out
+
+
+NULL32 = 0xffffffff
+CHANGE_DT = np.dtype([('hash', 'u1', 32), ('seq', '<u8'), ('startOp', '<u8'), ('time', '<i8'), ('msgOff', '<u4'), ('msgLen', '<u4'),
+                      ('depsOff', '<u4'), ('nDeps', '<u4'), ('actorFirst', '<u4'), ('nActors', '<u4'), ('extraOff', '<u4'), ('extraLen', '<u4'),
+                      ('hasExtra', '<u4'), ('pad', '<u4'), ('firstOp', '<u8'), ('nOps', '<u8'), ('firstPred', '<u8'), ('nPreds', '<u8')])
+OP_DT = np.dtype([(f, '<u4') for f in ('objActor', 'objCtr', 'keyActor', 'keyCtr', 'keyStrOff', 'keyStrLen', 'insert', 'action', 'valLen', 'valOff',
+                                       'chldActor', 'chldCtr', 'predFirst', 'predNum', 'change', 'pad')])
+PRED_DT = np.dtype([('actor', '<u4'), ('ctr', '<u4')])
+ACTOR_DT = np.dtype([('off', '<u4'), ('len', '<u4')])
+
+
+class FlatChanges:
+    """Zero-copy view of a change table (amg_decode_changes / amg_decode_history; layout in include/amgpu.h)."""
+
+    def __init__(self, raw):
+        self.raw = raw
+        h = self.hdr = np.frombuffer(raw, dtype='<u8', count=12)
+        assert int(h[0]) == 0x31474843474d41, 'bad change table magic'
+        self.changes = np.frombuffer(raw, dtype=CHANGE_DT, count=int(h[1]), offset=int(h[2]))
+        self.ops = np.frombuffer(raw, dtype=OP_DT, count=int(h[3]), offset=int(h[4]))
+        self.preds = np.frombuffer(raw, dtype=PRED_DT, count=int(h[5]), offset=int(h[6]))
+        self.actors = np.frombuffer(raw, dtype=ACTOR_DT, count=int(h[7]), offset=int(h[8]))
+
+    def __len__(self):
+        return len(self.changes)
+
+    def hashes(self):
+        return [bytes(h).hex() for h in self.changes['hash']]
+
+    def to_changes(self):
+        """The dicts columnar.decode_change returns (columnar.js:770-776 decodeChange), one per change."""
+        from .columnar import decode_value, ACTIONS as ACTION_NAMES
+        raw, out = self.raw, []
+        ops, preds, actor_refs = self.ops.tolist(), self.preds.tolist(), self.actors.tolist()
+        for rec in self.changes:
+            a0, na = int(rec['actorFirst']), int(rec['nActors'])
+            actors = [bytes(raw[o:o + ln]).hex() for o, ln in actor_refs[a0:a0 + na]]
+            d0 = int(rec['depsOff'])
+            mo = int(rec['msgOff'])
+            change = {'actor': actors[0], 'seq': int(rec['seq']), 'startOp': int(rec['startOp']), 'time': int(rec['time']),
+                      'message': bytes(raw[mo:mo + int(rec['msgLen'])]).decode('utf-8', 'replace'),
+                      'deps': [bytes(raw[d0 + 32 * k:d0 + 32 * k + 32]).hex() for k in range(int(rec['nDeps']))]}
+            if int(rec['hasExtra']):
+                eo = int(rec['extraOff'])
+                change['extraBytes'] = bytes(raw[eo:eo + int(rec['extraLen'])])
+
+            def actor(i):
+                return None if i == NULL32 else actors[i]
+
+            def num(v):
+                return None if v == NULL32 else v
+            change_ops = []
+            f0 = int(rec['firstOp'])
+            for (obj_a, obj_c, key_a, key_c, ks_off, ks_len, insert, action, val_len, val_off, ch_a, ch_c, p0, pn, _, _) in ops[f0:f0 + int(rec['nOps'])]:
+                obj = '_root' if obj_c == NULL32 else '%d@%s' % (obj_c, actor(obj_a))
+                act = None if action == NULL32 else (ACTION_NAMES[action] if action < len(ACTION_NAMES) else action)
+                key = None if ks_len == NULL32 else bytes(raw[ks_off:ks_off + ks_len]).decode('utf-8', 'replace')
+                if key:
+                    op = {'obj': obj, 'key': key, 'action': act}
+                else:
+                    op = {'obj': obj, 'elemId': '_head' if key_c == 0 else '%s@%s' % (num(key_c), actor(key_a)), 'action': act}
+                op['insert'] = bool(insert)
+                tag = 0 if val_len == NULL32 else val_len
+                if act in ('set', 'inc'):
+                    value, datatype = decode_value(tag, raw[val_off:val_off + (tag >> 4)])
+                    op['value'] = value
+                    if datatype:
+                        op['datatype'] = datatype
+                if ch_c != NULL32:
+                    op['child'] = '%d@%s' % (ch_c, actor(ch_a))
+                op['pred'] = ['%s@%s' % (num(c), actor(a)) for a, c in preds[p0:p0 + pn]]
+                change_ops.append(op)
+            change['ops'] = change_ops
+            change['hash'] = bytes(rec['hash']).hex()
+            out.append(change)
         return out
 
 
@@ -446,6 +529,44 @@ class GpuBackendDoc:
         """Device span of the last sync_bloom / sync_changes_to_send call (CUDA events), ms."""
         return float(self._lib.L.amg_last_sync_ms(self.h))
 
+    # ---- decodeChange / decodeChanges (columnar.js:770-776), on the device
+    def decode_packed_flat(self, blob, offs, n):
+        """amg_decode_changes over change i = blob[offs[i]:offs[i+1]] (bytes, a numpy array, or a pointer to pinned or device
+        memory). Raises AmgError with `.failed_index` = the change the reference fails on first."""
+        if isinstance(blob, (bytes, bytearray)):
+            buf = (C.c_uint8 * max(len(blob), 1)).from_buffer_copy(bytes(blob) if len(blob) else b'\0')
+        elif isinstance(blob, np.ndarray):
+            buf = blob.ctypes.data_as(C.c_void_p)
+        else:
+            buf = blob
+        offs = np.ascontiguousarray(offs, dtype=np.uint64)
+        bl, failed, err = C.c_void_p(), C.c_size_t(), _ErrStruct()
+        rc = self._lib.L.amg_decode_changes(self.h, buf, offs.ctypes.data_as(C.c_void_p), C.c_size_t(n), C.byref(bl), C.byref(failed), C.byref(err))
+        try:
+            self._lib.check(rc, err)
+        except AmgError as e:
+            e.failed_index = failed.value
+            raise
+        return FlatChanges(self._buffers(bl)[0])
+
+    def decode_changes_flat(self, changes):
+        """decodeChange of every binary change in `changes` (chunk type 1 or 2), in one device call: a FlatChanges view.
+        The document is not touched."""
+        n = len(changes)
+        offs = np.zeros(n + 1, dtype=np.uint64)
+        np.cumsum([len(c) for c in changes], out=offs[1:])
+        return self.decode_packed_flat(b''.join(bytes(c) for c in changes), offs, n)
+
+    def decode_history_flat(self):
+        """decodeChanges(getAllChanges()) of this document, read from device memory: a FlatChanges view."""
+        bl, err = C.c_void_p(), _ErrStruct()
+        self._lib.check(self._lib.L.amg_decode_history(self.h, C.byref(bl), C.byref(err)), err)
+        return FlatChanges(self._buffers(bl)[0])
+
+    def last_decode_ms(self):
+        """Device span of the last decode_*_flat call (CUDA events), ms."""
+        return float(self._lib.L.amg_last_decode_ms(self.h))
+
     def dump_ops(self):
         rows, n, succ, m, err = C.c_void_p(), C.c_size_t(), C.c_void_p(), C.c_size_t(), _ErrStruct()
         self._lib.check(self._lib.L.amg_debug_dump_ops(self.h, C.byref(rows), C.byref(n), C.byref(succ), C.byref(m), C.byref(err)), err)
@@ -495,6 +616,71 @@ class GpuBackendDoc:
 
     def launches(self):
         return int(self._lib.L.amg_kernel_launches(self.h))
+
+
+def split_containers(buf):
+    """columnar.js:829-837 splitContainers: the chunks of a buffer that holds several containers back to back."""
+    from .columnar import _Dec, MAGIC, DecodeError
+    d, chunks, start = _Dec(buf), [], 0
+    while not d.done:   # decodeContainerHeader(decoder, false), columnar.js:688-708
+        if d.raw(4) != MAGIC:
+            raise DecodeError('Data does not begin with magic bytes 85 6f 4a 83')
+        d.raw(4)
+        d.raw(1)
+        d.raw(d.uleb())
+        chunks.append(d.buf[start:d.off])
+        start = d.off
+    return chunks
+
+
+_decoders = {}
+
+
+def _decoder_for(doc_class):
+    """The per-process document handle that decodeChange / decodeChanges run on (created on first use, on AMG_DEVICE)."""
+    if doc_class not in _decoders:
+        _decoders[doc_class] = doc_class()
+    return _decoders[doc_class]
+
+
+def decode_changes(binary_changes, doc_class=None):
+    """columnar.js:843-857 decodeChanges: every buffer may hold several containers; change chunks (type 1 or 2) of the whole
+    list are decoded in one device call, a document chunk (type 0) contributes its changes (load, then the history decoded on
+    the device), other chunk types are skipped. The error of the first failing chunk in input order is raised."""
+    from .columnar import DecodeError
+    doc_class = doc_class or GpuBackendDoc
+    pieces, split_error = [], None   # ('change', chunk) / ('doc', chunk) in input order
+    for b in binary_changes:
+        try:
+            chunks = split_containers(bytes(b))
+        except DecodeError as e:
+            split_error = AmgError(1, str(e))
+            break
+        for chunk in chunks:
+            if chunk[8] == 0:
+                pieces.append(('doc', chunk))
+            elif chunk[8] in (1, 2):
+                pieces.append(('change', chunk))
+    changes = [c for kind, c in pieces if kind == 'change']
+    table, failed, change_error = None, None, None
+    if changes:
+        try:
+            table = _decoder_for(doc_class).decode_changes_flat(changes).to_changes()
+        except AmgError as e:
+            failed, change_error = e.failed_index, e
+    out, k = [], 0
+    for kind, chunk in pieces:
+        if kind == 'doc':
+            out.extend(doc_class(chunk).decode_history_flat().to_changes())
+            continue
+        if k == failed:
+            raise change_error
+        if table is not None:   # (after a failure only the chunks in front of the failing one are walked: for their errors)
+            out.append(table[k])
+        k += 1
+    if split_error is not None:
+        raise split_error
+    return out
 
 
 def doc_class_for(library_path):

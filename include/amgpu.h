@@ -91,6 +91,33 @@ typedef struct { uint32_t num_entries, num_probes; const uint8_t* bits; size_t b
 int amg_sync_changes_to_send(amg_backend* b, const uint8_t* last_sync, size_t n_last, const amg_bloom* filters, size_t n_filters,
                              const uint8_t* need, size_t n_need, amg_buffers** out_changes, amg_buffers** out_hashes, amg_error* err);
 
+/* columnar.js:770-776 decodeChange over n change containers (chunk type 1 or 2, one per entry, as in amg_apply_changes_packed:
+ * change i is blob[offsets[i] .. offsets[i+1]); blob may be pinned, pageable or device memory). The bytes are staged into
+ * scratch, DEFLATEd changes inflated on the device; the document is not touched. One buffer: the change table (layout below).
+ * On error, *failed_index is the change the reference's sequential loop fails on first, and err carries its message. */
+int amg_decode_changes(amg_backend* b, const uint8_t* blob, const uint64_t* offsets, size_t n,
+                       amg_buffers** out, size_t* failed_index, amg_error* err);
+/* the same for every applied change of b, in getAllChanges order (new.js:1925-1927), read in place from device memory (a
+ * loaded document's history is rebuilt first, as getChanges does). Queued changes are not included. */
+int amg_decode_history(amg_backend* b, amg_buffers** out, amg_error* err);
+/* device span of the last amg_decode_changes / amg_decode_history call in ms (CUDA events on the engine's main stream) */
+float amg_last_decode_ms(amg_backend* b);
+/* Change table layout (little endian). A header of 12 uint64:
+ *   [0] 0x31474843474d41 ("AMGCHG1") [1] nChanges [2] changesOff [3] nOps [4] opsOff [5] nPreds [6] predsOff
+ *   [7] nActors [8] actorsOff [9] bytesOff [10] bytesLen [11] 0
+ * followed by the sections (offsets relative to the start of the buffer):
+ *   changes: nChanges x { uint8 hash[32]; uint64 seq, startOp; int64 time; uint32 msgOff, msgLen, depsOff, nDeps, actorFirst,
+ *            nActors, extraOff, extraLen, hasExtra, pad; uint64 firstOp, nOps, firstPred, nPreds }          (128 bytes)
+ *   ops    : nOps x { uint32 objActor, objCtr, keyActor, keyCtr, keyStrOff, keyStrLen, insert, action, valLen, valOff,
+ *            chldActor, chldCtr, predFirst, predNum, change, pad }                                             (64 bytes)
+ *   preds  : nPreds x { uint32 actor, ctr }
+ *   actors : nActors x { uint32 off, len }: per change, entries actorFirst .. actorFirst + nActors - 1 are its actor table
+ *            (entry 0 is the author); the op and pred actor numbers index it
+ *   bytes  : the decoded change containers back to back (inflated)
+ * 0xffffffff is null (keyStrLen null: no key string column value; an empty string has length 0). msgOff, depsOff (nDeps x 32
+ * bytes), extraOff, keyStrOff, valOff and the actor entries' off are offsets INTO THE TABLE. action is the raw action number,
+ * valLen the VALUE_LEN tag (length << 4 | type, columnar.js:46-49); every value has been checked like decodeValue does. */
+
 /* returned buffer lists */
 size_t amg_buffers_count(const amg_buffers* l);
 const uint8_t* amg_buffers_get(const amg_buffers* l, size_t i, size_t* len);
