@@ -196,6 +196,21 @@ napi_value SyncChangesToSend(napi_env env, napi_callback_info info) {
   napi_set_element(env, out, 0, buffersToJs(env, changes)); napi_set_element(env, out, 1, hs);
   return out;
 }
+// the per-process backend handle decodeChanges and encodeChanges run on (created on first use)
+amg_backend* codecBackend(amg_error* err) {
+  static amg_backend* codec = nullptr;
+  if (!codec) codec = amg_init(deviceFromEnv(), err);
+  return codec;
+}
+// the reference's error class and message, with the index of the failing change as `failedIndex`
+napi_value throwFailed(napi_env env, const amg_error& err, size_t failed) {
+  napi_value msg, e, idx; napi_create_string_utf8(env, err.msg, NAPI_AUTO_LENGTH, &msg);
+  if (err.code == AMG_RANGE_ERROR) napi_create_range_error(env, nullptr, msg, &e);
+  else if (err.code == AMG_TYPE_ERROR) napi_create_type_error(env, nullptr, msg, &e);
+  else napi_create_error(env, nullptr, msg, &e);
+  napi_create_double(env, (double)failed, &idx); napi_set_named_property(env, e, "failedIndex", idx);
+  napi_throw(env, e); return nullptr;
+}
 // decodeChanges(Uint8Array[]) — columnar.js:770-776 decodeChange of every entry (one change container each), in one call on
 // a per-process backend handle. Returns the change table (layout: amgpu.h) as one Uint8Array; an error carries the index of
 // the failing change as `failedIndex`.
@@ -210,20 +225,26 @@ napi_value DecodeChanges(napi_env env, napi_callback_info info) {
     const uint8_t* p; size_t len; if (!getBytes(env, el, &p, &len)) return nullptr;
     blob.append(reinterpret_cast<const char*>(p), len); offsets[i + 1] = blob.size();
   }
-  static amg_backend* decoder = nullptr;
-  amg_error err;
-  if (!decoder && !(decoder = amg_init(deviceFromEnv(), &err))) return throwAmg(env, err);
+  amg_error err; amg_backend* decoder = codecBackend(&err);
+  if (!decoder) return throwAmg(env, err);
   amg_buffers* l = nullptr; size_t failed = 0;
-  if (amg_decode_changes(decoder, reinterpret_cast<const uint8_t*>(blob.data()), offsets.data(), n, &l, &failed, &err)) {
-    // the reference's error class and message, with the index of the failing change as `failedIndex`
-    napi_value msg, e, idx; napi_create_string_utf8(env, err.msg, NAPI_AUTO_LENGTH, &msg);
-    if (err.code == AMG_RANGE_ERROR) napi_create_range_error(env, nullptr, msg, &e);
-    else if (err.code == AMG_TYPE_ERROR) napi_create_type_error(env, nullptr, msg, &e);
-    else napi_create_error(env, nullptr, msg, &e);
-    napi_create_double(env, (double)failed, &idx); napi_set_named_property(env, e, "failedIndex", idx);
-    napi_throw(env, e); return nullptr;
-  }
+  if (amg_decode_changes(decoder, reinterpret_cast<const uint8_t*>(blob.data()), offsets.data(), n, &l, &failed, &err)) return throwFailed(env, err, failed);
   napi_value el; napi_get_element(env, buffersToJs(env, l), 0, &el); return el;
+}
+// encodeChanges(Uint8Array) — columnar.js:710-739 encodeChange of every change of a change table (layout: amgpu.h), in one
+// call on the same per-process backend handle. Returns {changes: Uint8Array[], hashes: Uint8Array (n x 32 bytes)}; an error
+// carries the index of the failing change as `failedIndex`.
+napi_value EncodeChanges(napi_env env, napi_callback_info info) {
+  napi_value argv[1]; if (!getArgs(env, info, 1, argv)) return nullptr;
+  const uint8_t* p; size_t len; if (!getBytes(env, argv[0], &p, &len)) return nullptr;
+  amg_error err; amg_backend* encoder = codecBackend(&err);
+  if (!encoder) return throwAmg(env, err);
+  amg_buffers *changes = nullptr, *hashes = nullptr; size_t failed = 0;
+  if (amg_encode_changes(encoder, p, len, &changes, &hashes, &failed, &err)) return throwFailed(env, err, failed);
+  napi_value out, hs; napi_create_object(env, &out);
+  napi_get_element(env, buffersToJs(env, hashes), 0, &hs);
+  napi_set_named_property(env, out, "changes", buffersToJs(env, changes)); napi_set_named_property(env, out, "hashes", hs);
+  return out;
 }
 // decodeHistory(state) — decodeChanges(getAllChanges(state)), read from device memory: the change table as one Uint8Array
 napi_value DecodeHistory(napi_env env, napi_callback_info info) { return listCall(env, info, amg_decode_history, true); }
@@ -239,7 +260,8 @@ napi_value InitModule(napi_env env, napi_value exports) {
     {"init", Init}, {"load", Load}, {"clone", Clone}, {"free", Free}, {"applyChanges", ApplyChanges}, {"getPatch", GetPatch}, {"save", Save},
     {"getHeads", GetHeads}, {"getChanges", GetChanges}, {"getChangesAdded", GetChangesAdded}, {"getChangeByHash", GetChangeByHash},
     {"getMissingDeps", GetMissingDeps}, {"clockOf", ClockOf}, {"hashByActor", HashByActor}, {"syncBloom", SyncBloom},
-    {"syncChangesToSend", SyncChangesToSend}, {"decodeChanges", DecodeChanges}, {"decodeHistory", DecodeHistory}};
+    {"syncChangesToSend", SyncChangesToSend}, {"decodeChanges", DecodeChanges}, {"decodeHistory", DecodeHistory},
+    {"encodeChanges", EncodeChanges}};
   for (auto& f : fns) { napi_value fn; napi_create_function(env, f.name, NAPI_AUTO_LENGTH, f.fn, nullptr, &fn); napi_set_named_property(env, exports, f.name, fn); }
   return exports;
 }

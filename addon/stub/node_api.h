@@ -29,6 +29,7 @@ napi_status napi_create_arraybuffer(napi_env env, size_t byte_length, void** dat
 napi_status napi_create_typedarray(napi_env env, napi_typedarray_type type, size_t length, napi_value arraybuffer, size_t byte_offset, napi_value* result);
 napi_status napi_get_undefined(napi_env env, napi_value* result);
 napi_status napi_create_array_with_length(napi_env env, size_t length, napi_value* result);
+napi_status napi_create_object(napi_env env, napi_value* result);
 napi_status napi_set_element(napi_env env, napi_value object, uint32_t index, napi_value value);
 napi_status napi_get_element(napi_env env, napi_value object, uint32_t index, napi_value* result);
 napi_status napi_get_array_length(napi_env env, napi_value value, uint32_t* result);

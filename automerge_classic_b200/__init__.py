@@ -5,7 +5,7 @@
 The module object `Backend` mirrors the module a caller hands to `Automerge.setDefaultBackend()`.
 """
 from .backend import Backend as _Facade
-from .engine import GpuBackendDoc, AmgError, Unsupported, decode_changes as _decode_changes, _decoder_for
+from .engine import GpuBackendDoc, AmgError, Unsupported, FlatChanges, decode_changes as _decode_changes, _decoder_for
 
 from . import sync as _sync
 
@@ -30,5 +30,19 @@ def decodeChange(buf):
     return _decoder_for(GpuBackendDoc).decode_changes_flat([buf]).to_changes()[0]
 
 
+def encodeChanges(changes):
+    """Automerge.encodeChange over a list of change objects, in one device call: their binary changes."""
+    return _decoder_for(GpuBackendDoc).encode_flat(FlatChanges.from_changes(changes))[0]
+
+
+def encodeChange(change):
+    """Automerge.encodeChange (columnar.js:710-739, src/automerge.js:153): a change object -> its binary change. A `hash` that
+    differs from the encoding's raises the reference's RangeError (columnar.js:735-737)."""
+    out, hashes = _decoder_for(GpuBackendDoc).encode_flat(FlatChanges.from_changes([change]))
+    if change.get('hash') and change['hash'] != hashes[0]:
+        raise AmgError(1, 'Change hash does not match encoding: %s != %s' % (change['hash'], hashes[0]))
+    return out[0]
+
+
 Backend = bind_sync(_Facade(GpuBackendDoc))
-__all__ = ['Backend', 'GpuBackendDoc', 'AmgError', 'Unsupported', 'bind_sync', 'decodeChange', 'decodeChanges']
+__all__ = ['Backend', 'GpuBackendDoc', 'AmgError', 'Unsupported', 'bind_sync', 'decodeChange', 'decodeChanges', 'encodeChange', 'encodeChanges']

@@ -252,6 +252,35 @@ int amg_decode_history(amg_backend* b, amg_buffers** out, amg_error* err) {
     *out = guard.release(); return 0;)
 }
 float amg_last_decode_ms(amg_backend* b) { return b->eng.lastDecodeMs; }
+// columnar.js:710-739 encodeChange over the changes of a change table: plain changes from the device, the ones of 256 bytes
+// or more DEFLATEd here (columnar.js:738), over a few host threads when there are many
+int amg_encode_changes(amg_backend* b, const uint8_t* table, size_t table_len, amg_buffers** out_changes, amg_buffers** out_hashes,
+                       size_t* failed_index, amg_error* err) {
+  if (failed_index) *failed_index = 0;
+  try {
+    std::string bytes, hs; std::vector<u64> offs;
+    b->eng.encodeChanges(table, table_len, bytes, offs, hs);
+    auto* lc = new amg_buffers(); std::unique_ptr<amg_buffers> gc(lc); auto* lh = new amg_buffers(); std::unique_ptr<amg_buffers> gh(lh);
+    const size_t n = offs.size() - 1; lc->items.resize(n);
+    auto fill = [&](size_t from, size_t to) {
+      for (size_t i = from; i < to; i++) {
+        const u64 len = offs[i + 1] - offs[i];
+        if (len >= 256) lc->items[i] = amg_backend::deflateChange(std::string(bytes, offs[i], len)); else lc->items[i].assign(bytes, offs[i], len);
+      }
+    };
+    const size_t nThreads = std::min<size_t>(std::max(1u, std::thread::hardware_concurrency()), std::min<size_t>(16, n / 4096 + 1));
+    if (nThreads <= 1) fill(0, n);
+    else {
+      std::vector<std::thread> th; const size_t per = (n + nThreads - 1) / nThreads;
+      for (size_t t = 0; t < nThreads; t++) th.emplace_back(fill, std::min(n, t * per), std::min(n, (t + 1) * per));
+      for (auto& x : th) x.join();
+    }
+    lh->items.push_back(std::move(hs));
+    *out_changes = gc.release(); *out_hashes = gh.release(); return 0;
+  } catch (amg::Error& e) { amg::drop_pending_peeks(); if (failed_index) *failed_index = b->eng.encodeFailed; setErr(err, e.code, e.what()); return e.code; }
+  catch (std::exception& e) { amg::drop_pending_peeks(); setErr(err, AMG_INTERNAL_ERROR, e.what()); return AMG_INTERNAL_ERROR; }
+}
+float amg_last_encode_ms(amg_backend* b) { return b->eng.lastEncodeMs; }
 // new.js:1979-1997
 int amg_get_changes_added(amg_backend* bn, amg_backend* bo, amg_buffers** out, amg_error* err) {
   AMG_GUARD(

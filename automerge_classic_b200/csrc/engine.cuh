@@ -29,6 +29,7 @@
 #include "history.cuh"
 #include "sync.cuh"
 #include "changes.cuh"
+#include "encchg.cuh"
 #include "unknowncols.hpp"
 
 namespace amg {
@@ -450,6 +451,26 @@ class Engine {
   size_t decodeFailed = 0; float lastDecodeMs = 0;   // failing change of the last call; its device span (CUDA events; 0 in the emulation build)
   DBuf<u8> dcArena, dcHash, dcOut; DBuf<u32> dcOff, dcLen, dcCLen, dcOps, dcPreds, dcActors, dcBytes, dcOpBase, dcPredBase, dcActorBase, dcByteBase, dcColOff, dcColLen, dcRows, dcChld;
   DBuf<ChangeMeta> dcMeta; DBuf<u64> dcErr, dcTotals; DBuf<u32> dcDefl;
+
+  // ---------------------------------------------------------------- encodeChange over a change table (encchg.cuh)
+  // The n changes of a change table (layout: include/amgpu.h) into plain binary changes and their hashes. The table is
+  // staged like decodeChanges' input; the document is not touched. On error, encodeFailed names the change. Its tables live
+  // as long as the call.
+  struct EncodeCall {
+    size_t n = 0; u64 len = 0; u64 hdr[CHG_HDR_WORDS] = {}; EncTable T{};
+    size_t M = 0, P = 0, E = 0, Q = 0, U = 0; u32 maxActorLen = 0; u64 total = 0;   // ops, preds, actor entries, actor slots, (change, actor) pairs; output bytes
+    DBuf<u64> err, totals; DBuf<u32> nOps, nPreds, nActors, opBase, predBase, actorBase, slotCnt, slotBase;
+    DBuf<u32> entOff, entLen, entRank, rep, head, headScan, sortVals, uniq, uniqSlot, otherStart; DBuf<u64> sortKeys, slotKeys, other;
+    DBuf<u32> objA, keyA, chA, predA, colLen, outLen; DBuf<long long> keyDelta, chDelta, predDelta; DBuf<u64> predKey, outOff, dataAt, depsAt, bodyAt;
+    DBuf<u8> out, hashes;
+  };
+  // out: the changes back to back, offs: n + 1 offsets into it, hashes: n x 32 bytes
+  void encodeChanges(const u8* table, size_t len, std::string& out, std::vector<u64>& offs, std::string& hashesOut);   // the phases, in order:
+  void stageEncodeInput(EncodeCall& e, const u8* table), validateTable(EncodeCall& e), encodeActorTables(EncodeCall& e), encodePrep(EncodeCall& e),
+       encodeColumns(EncodeCall& e), encodeHashes(EncodeCall& e);
+  void copyEncodeOutput(EncodeCall& e, std::string& out, std::vector<u64>& offs, std::string& hashesOut);
+  [[noreturn]] void throwEncodeError(EncodeCall& e, const u64* words);
+  size_t encodeFailed = 0; float lastEncodeMs = 0;   // failing change of the last call; its device span (CUDA events; 0 in the emulation build)
  private:
   void uploadCandidates(const u32* idx, size_t count);
   void syncTimer(bool start);

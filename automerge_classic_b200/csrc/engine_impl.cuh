@@ -2047,6 +2047,190 @@ inline void Engine::throwDecodeError(DecodeCall& d, const u64* w) {
   throwKernelError(w[phase]);
 }
 
+// ------------------------------------------------------------ encodeChange over a change table (encchg.cuh)
+inline void Engine::encodeChanges(const u8* table, size_t len, std::string& out, std::vector<u64>& offs, std::string& hashesOut) {
+  EncodeCall e; e.len = len; encodeFailed = 0; lastEncodeMs = 0;
+  const float keepSyncMs = lastSyncMs; lastSyncMs = 0;
+  struct Restore { Engine& e; float ms; ~Restore() { e.lastSyncMs = ms; } } restore{*this, keepSyncMs};   // the timer is shared with the sync calls
+  syncTimer(true);
+  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+  stageEncodeInput(e, table);
+  if (e.n) { validateTable(e); encodeActorTables(e); encodePrep(e); encodeColumns(e); encodeHashes(e); }
+  copyEncodeOutput(e, out, offs, hashesOut);
+  syncTimer(false); lastEncodeMs = lastSyncMs;
+}
+
+// 1. the table into scratch as decodeChanges stages its input (pinned, pageable or device memory); the header's sections
+// checked on the host: inside the table and aligned for their records
+inline void Engine::stageEncodeInput(EncodeCall& e, const u8* table) {
+  auto bad = [](const std::string& what) { throw Error(AMG_ERR_RANGE, "change table: " + what); };
+  if (e.len < CHG_HDR_WORDS * 8) bad("shorter than its header");
+  DecodeCall d; d.n = 1; const u64 offs[2] = {0, (u64)e.len};
+  dcOff.ensure(ctx, 2); dcLen.ensure(ctx, 2);
+  stageDecodeInput(d, table, offs);
+  d2h(ctx, e.hdr, dcArena.p, sizeof(e.hdr)); sync(ctx);
+  const u64* h = e.hdr;
+  if (h[0] != CHG_MAGIC) bad("bad magic");
+  auto section = [&](u64 count, u64 off, u64 size, u64 align, const char* what) {
+    if (off % align || off > e.len || count > (e.len - off) / size) bad(std::string(what) + " section out of range");
+  };
+  section(h[1], h[2], sizeof(ChangeRec), 8, "changes"); section(h[3], h[4], sizeof(OpRec), 8, "ops");
+  section(h[5], h[6], 8, 4, "preds"); section(h[7], h[8], sizeof(ActorRef), 4, "actors");
+  e.n = (size_t)h[1];
+  const u8* t = dcArena.p;
+  e.T = EncTable{t, e.len, h[3], h[5], h[7], reinterpret_cast<const ChangeRec*>(t + h[2]), reinterpret_cast<const OpRec*>(t + h[4]),
+                 reinterpret_cast<const u32*>(t + h[6]), reinterpret_cast<const ActorRef*>(t + h[8])};
+}
+
+// 2. change records (thread per change), then ops (thread per op); every error of the call is known before anything is sized
+inline void Engine::validateTable(EncodeCall& e) {
+  const size_t n = e.n;
+  e.err.ensure(ctx, EP_NUM); dev_memset(ctx, e.err.p, 0, EP_NUM * 8);
+  e.totals.ensure(ctx, 4); dev_memset(ctx, e.totals.p, 0, 4 * 8);
+  for (auto* b : {&e.nOps, &e.nPreds, &e.nActors, &e.opBase, &e.predBase, &e.actorBase}) b->ensure(ctx, n + 2);
+  foreach(ctx, n, EncChangeKernel{e.T, e.nOps.p, e.nPreds.p, e.nActors.p, reinterpret_cast<u32*>(e.totals.p + 3), e.err.p + EP_CHANGES, e.err.p + EP_SIZE});
+  foreach(ctx, n, ChgTotalsKernel{e.nOps.p, e.nPreds.p, e.nActors.p, e.totals.p});
+  u64 t[4] = {0, 0, 0, 0}; void* dst[4] = {&t[0], &t[1], &t[2], &t[3]};
+  readWords({{e.totals.p, 8}, {e.totals.p + 1, 8}, {e.totals.p + 2, 8}, {e.totals.p + 3, 8}}, dst);
+  // the scans are 32-bit, and every op takes 3 + predNum actor slots
+  if (t[0] >= 0x7fffffffULL || t[1] >= 0x7fffffffULL || t[2] >= 0x7fffffffULL || 3 * t[0] + t[1] >= 0x7fffffffULL)
+    throw Error(AMG_ERR_UNSUPPORTED, "amgpu: more than 2^31 operations, preds or actor table entries in one encodeChanges call");
+  e.M = t[0]; e.P = t[1]; e.E = t[2]; e.maxActorLen = (u32)t[3];
+  scan_exclusive(ctx, scanTmp, e.nOps.p, e.opBase.p, n); scan_exclusive(ctx, scanTmp, e.nPreds.p, e.predBase.p, n); scan_exclusive(ctx, scanTmp, e.nActors.p, e.actorBase.p, n);
+  e.slotCnt.ensure(ctx, e.M + 2); e.slotBase.ensure(ctx, e.M + 3);
+  if (e.M) foreach(ctx, e.M, EncOpKernel{e.T, e.opBase.p, n, e.slotCnt.p, e.err.p + EP_OPS});
+  u64 w[EP_NUM] = {0, 0, 0}; void* wd[EP_NUM] = {&w[0], &w[1], &w[2]};
+  readWords({{e.err.p, 8}, {e.err.p + 1, 8}, {e.err.p + 2, 8}}, wd);
+  if (w[EP_CHANGES] || w[EP_OPS] || w[EP_SIZE]) throwEncodeError(e, w);   // nothing is sized before every change is known to fit
+}
+
+// 3. actor ids ranked over the call (LSD radix sort: length, then 8-byte chunks from the last), then every change's other
+// actors: its sorted, unique (change, rank) pairs (the history kernels)
+inline void Engine::encodeActorTables(EncodeCall& e) {
+  const size_t n = e.n, E = e.E, M = e.M;   // (every change has its author: E >= n > 0)
+  for (auto* b : {&e.entOff, &e.entLen, &e.entRank, &e.rep, &e.head, &e.headScan}) b->ensure(ctx, E + 2);
+  e.sortKeys.ensure(ctx, E + 1); e.sortVals.ensure(ctx, E + 1);
+  foreach(ctx, n, EncActorListKernel{e.T, e.nActors.p, e.actorBase.p, e.entOff.p, e.entLen.p});
+  foreach(ctx, E, EncActorKeyKernel{e.T.t, e.entOff.p, e.entLen.p, nullptr, -1, e.sortKeys.p, e.sortVals.p});
+  radix_sort_pairs(ctx, sortTmp, e.sortKeys, e.sortVals, E, 0, bits_for(e.maxActorLen));
+  for (int q = (int)((e.maxActorLen + 7) / 8) - 1; q >= 0; q--) {
+    foreach(ctx, E, EncActorKeyKernel{e.T.t, e.entOff.p, e.entLen.p, e.sortVals.p, q, e.sortKeys.p, nullptr});
+    radix_sort_pairs(ctx, sortTmp, e.sortKeys, e.sortVals, E, 0, 64);
+  }
+  foreach(ctx, E, EncActorHeadKernel{e.T.t, e.entOff.p, e.entLen.p, e.sortVals.p, e.head.p});
+  scan_exclusive(ctx, scanTmp, e.head.p, e.headScan.p, E);
+  foreach(ctx, E, EncActorRankKernel{e.sortVals.p, e.head.p, e.headScan.p, e.entRank.p, e.rep.p});
+  if (M) { scan_exclusive(ctx, scanTmp, e.slotCnt.p, e.slotBase.p, M); e.Q = readU32(e.slotBase.p + M); }
+  const size_t Q = e.Q;
+  e.slotKeys.ensure(ctx, Q + 1); e.sortVals.ensure(ctx, Q + 1); e.uniq.ensure(ctx, Q + 2); e.uniqSlot.ensure(ctx, Q + 3);
+  if (Q) {
+    foreach(ctx, M, EncActorPairKernel{e.T, e.opBase.p, n, e.actorBase.p, e.entRank.p, e.slotBase.p, e.slotKeys.p});
+    foreach(ctx, Q, HistIotaKernel{e.sortVals.p});
+    radix_sort_pairs(ctx, sortTmp, e.slotKeys, e.sortVals, Q, 0, std::min(64, 32 + bits_for(n)));   // (~0 = no actor: all ones, sorts last)
+    foreach(ctx, Q, HistUniqueKernel{e.slotKeys.p, e.uniq.p});
+    scan_exclusive(ctx, scanTmp, e.uniq.p, e.uniqSlot.p, Q);
+    e.U = readU32(e.uniqSlot.p + Q);
+  }
+  e.other.ensure(ctx, e.U + 1); e.otherStart.ensure(ctx, n + 2);
+  if (e.U) foreach(ctx, Q, HistOtherFillKernel{e.slotKeys.p, e.uniq.p, e.uniqSlot.p, e.other.p});
+  foreach(ctx, n + 1, HistLowerBoundKernel{e.other.p, (u32)e.U, 32, e.otherStart.p});
+}
+
+// 4. local actor numbers, delta values, sorted preds (thread per change)
+inline void Engine::encodePrep(EncodeCall& e) {
+  const size_t M = e.M, P = e.P;
+  for (auto* b : {&e.objA, &e.keyA, &e.chA}) b->ensure(ctx, M + 1);
+  for (auto* b : {&e.keyDelta, &e.chDelta}) b->ensure(ctx, M + 1);
+  e.predA.ensure(ctx, P + 1); e.predDelta.ensure(ctx, P + 1); e.predKey.ensure(ctx, P + 1);
+  foreach(ctx, e.n, EncPrepKernel{e.T, e.opBase.p, e.predBase.p, e.actorBase.p, e.entRank.p, e.other.p, e.otherStart.p, e.objA.p, e.keyA.p, e.keyDelta.p, e.chA.p, e.chDelta.p,
+                                  e.predKey.p, e.predA.p, e.predDelta.p});
+}
+
+// 5. column lengths (thread per (column, change)), container lengths, offsets (64-bit scan), headers, then the columns
+inline void Engine::encodeColumns(EncodeCall& e) {
+  const size_t n = e.n;
+  const EncCols cols{e.opBase.p, e.predBase.p, e.objA.p, e.keyA.p, e.keyDelta.p, e.chA.p, e.chDelta.p, e.predA.p, e.predDelta.p};
+  e.colLen.ensure(ctx, (size_t)HC_NUM * n + 1); e.outLen.ensure(ctx, n + 1); e.outOff.ensure(ctx, n + 2);
+  for (auto* b : {&e.dataAt, &e.depsAt, &e.bodyAt}) b->ensure(ctx, n + 1);
+  foreach(ctx, (size_t)HC_NUM * n, EncColSizeKernel{e.T, cols, n, e.colLen.p});
+  EncChangeHeadKernel hk{0, e.T, n, e.colLen.p, e.actorBase.p, e.entOff.p, e.entLen.p, e.rep.p, e.other.p, e.otherStart.p, e.outLen.p, e.outOff.p, nullptr, e.dataAt.p, e.depsAt.p, e.bodyAt.p};
+  foreach(ctx, n, hk);
+  scan_exclusive64(ctx, scanTmp, EncOutLen64{e.outLen.p}, e.outOff.p, n);
+  u64 total = 0; void* dst[1] = {&total}; readWords({{e.outOff.p + n, 8}}, dst);
+  if (total + 64 >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: the changes of one encodeChanges call are limited to 4 GiB");
+  e.total = total; e.out.ensure(ctx, total + 64);
+  hk.pass = 1; hk.out = e.out.p; foreach(ctx, n, hk);
+  foreach(ctx, (size_t)HC_NUM * n, EncColWriteKernel{e.T, cols, n, e.colLen.p, e.dataAt.p, e.out.p});
+}
+
+// 6. hashes and checksums (thread per change: the dependencies are given as hashes)
+inline void Engine::encodeHashes(EncodeCall& e) {
+  e.hashes.ensure(ctx, e.n * 32 + 64);
+  foreach(ctx, e.n, EncHashKernel{e.T, e.outOff.p, e.outLen.p, e.depsAt.p, e.bodyAt.p, e.out.p, e.hashes.p});
+}
+
+// 7. to the host (the caller DEFLATEs the large ones)
+inline void Engine::copyEncodeOutput(EncodeCall& e, std::string& out, std::vector<u64>& offs, std::string& hashesOut) {
+  const size_t n = e.n;
+  out.resize(e.total); offs.assign(n + 1, 0); hashesOut.resize(n * 32);
+  if (!n) return;
+  if (e.total) d2h(ctx, &out[0], e.out.p, e.total);
+  d2h(ctx, offs.data(), e.outOff.p, (n + 1) * 8); d2h(ctx, &hashesOut[0], e.hashes.p, n * 32); sync(ctx);
+}
+
+// The smallest failing change over both phases (op errors are keyed by op: mapped to their change), and for it the error
+// of its earliest phase
+inline void Engine::throwEncodeError(EncodeCall& e, const u64* w) {
+  const size_t n = e.n; std::vector<u32> opBase(n + 1); d2h(ctx, opBase.data(), e.opBase.p, (n + 1) * 4); sync(ctx);
+  size_t best = SIZE_MAX; int phase = -1;
+  for (int k = 0; k < EP_NUM; k++) {
+    if (!w[k]) continue;
+    size_t c = (size_t)(w[k] >> 8);
+    if (k == EP_OPS) c = (size_t)(std::upper_bound(opBase.begin(), opBase.end(), (u32)c) - opBase.begin()) - 1;
+    if (c < best) { best = c; phase = k; }
+  }
+  encodeFailed = best; const u32 code = (u32)(w[phase] & 0xff);
+  const std::string at = "change table: change " + std::to_string(best) + ": ";
+  switch (code) {
+    case EE_CHG_OPS: throw Error(AMG_ERR_RANGE, at + "ops out of range");
+    case EE_CHG_PREDS: throw Error(AMG_ERR_RANGE, at + "preds out of range");
+    case EE_CHG_ACTORS: throw Error(AMG_ERR_RANGE, at + "actor table out of range");
+    case EE_ACTOR_ENTRY: throw Error(AMG_ERR_RANGE, at + "actor id out of range");
+    case EE_CHG_MSG: throw Error(AMG_ERR_RANGE, at + "message out of range");
+    case EE_CHG_DEPS: throw Error(AMG_ERR_RANGE, at + "deps out of range");
+    case EE_CHG_EXTRA: throw Error(AMG_ERR_RANGE, at + "extra bytes out of range");
+    case EE_NUM_RANGE: throw Error(AMG_ERR_RANGE, "number out of range");
+    case EE_TOO_LARGE: throw Error(AMG_ERR_UNSUPPORTED, "amgpu: more than 2^31 preds in one change");
+    case EE_CHANGE_SIZE: throw Error(AMG_ERR_UNSUPPORTED, "amgpu: change " + std::to_string(best) + " may encode to 4 GiB or more (its ops' key and value bytes are counted once per op)");
+    case EE_OP_KEYSTR: throw Error(AMG_ERR_RANGE, at + "key string out of range");
+    case EE_OP_VALUE: throw Error(AMG_ERR_RANGE, at + "value out of range");
+    case EE_OP_PREDS: throw Error(AMG_ERR_RANGE, at + "op preds out of range");
+    case EE_OBJ: throw Error(AMG_ERR_RANGE, "Unexpected objectId reference");
+    case EE_KEY: throw Error(AMG_ERR_RANGE, "Unexpected operation key");
+    case EE_ACTION: throw Error(AMG_ERR_RANGE, "Unexpected operation action");
+    default: break;
+  }
+  if (phase == EP_OPS) {   // the messages that name a value of the op
+    const size_t j = (size_t)(w[phase] >> 8); ChangeRec r; d2h(ctx, &r, e.T.ch + best, sizeof(r)); sync(ctx);
+    OpRec o; d2h(ctx, &o, e.T.ops + r.firstOp + (j - opBase[best]), sizeof(o)); sync(ctx);
+    auto actorIndex = [](u32 a) { return "No actor index " + std::to_string(a); };
+    switch (code) {
+      case EE_KEY_ACTOR: throw Error(AMG_ERR_RANGE, actorIndex(o.keyActor));
+      case EE_CHLD_ACTOR: throw Error(AMG_ERR_RANGE, actorIndex(o.chldActor));
+      case EE_CHLD_NULL: throw Error(AMG_ERR_RANGE, "Mismatched child columns: " + std::to_string(o.chldCtr) + " and None");
+      case EE_PRED_NULL: throw Error(AMG_ERR_RANGE, "Not a valid opId: a pred counter is null");
+      case EE_PRED_ACTOR: {
+        std::vector<u32> pr(2 * (size_t)o.predNum + 2); d2h(ctx, pr.data(), e.T.preds + 2 * (size_t)o.predFirst, (size_t)o.predNum * 8); sync(ctx);
+        for (u32 k = 0; k < o.predNum; k++) if (pr[2 * k] >= r.nActors) throw Error(AMG_ERR_RANGE, actorIndex(pr[2 * k]));
+        break;
+      }
+      case KE_FLOAT_LEN: throw Error(AMG_ERR_RANGE, "Invalid length for floating point number: " + std::to_string(o.valLen >> 4));
+      default: break;
+    }
+  }
+  throwKernelError(w[phase]);
+}
+
 inline void Engine::gatherHashes(const std::vector<u32>& idx, std::string& out) {
   out.assign(idx.size() * 32, '\0');
   if (idx.empty()) return;

@@ -10,6 +10,8 @@
 // list; one thread per change then encodes its own columns (canonical RLE / delta / boolean records; a change is a few
 // ops, and changes are independent) in two passes (size, bytes). A change's bytes contain the hashes of its
 // dependencies, so hashing goes level by level through the dependency graph (level = longest path from a root).
+// The column writer (hist_column over an op source), the change header writer (write_change_head) and hist_sha256 are
+// shared with encodeChanges (encchg.cuh), which reads its ops from a change table instead of the document's rows.
 #pragma once
 #include "encode.cuh"
 #include "prims.cuh"
@@ -156,62 +158,102 @@ template <class Acc> HD void hist_rle(ByteSink& out, const Acc& acc, u32 n) {
   }
 }
 
-enum { HC_OBJ_ACTOR, HC_OBJ_CTR, HC_KEY_ACTOR, HC_KEY_CTR, HC_KEY_STR, HC_INSERT, HC_ACTION, HC_VAL_LEN, HC_VAL_RAW, HC_PRED_NUM, HC_PRED_ACTOR, HC_PRED_CTR, HC_NUM };
+enum { HC_OBJ_ACTOR, HC_OBJ_CTR, HC_KEY_ACTOR, HC_KEY_CTR, HC_KEY_STR, HC_INSERT, HC_ACTION, HC_VAL_LEN, HC_VAL_RAW, HC_CHLD_ACTOR, HC_CHLD_CTR,
+       HC_PRED_NUM, HC_PRED_ACTOR, HC_PRED_CTR, HC_NUM };
 
-// everything one change's encoder reads
-struct HistChangeCtx {
-  HistOpView v; const u8* arena; u32 k; u32 opStart, nOps, predBase, nPreds;
-  const u32* objA; const u32* keyA; const long long* keyDelta; const u32* predA; const long long* predDelta;   // local actor indexes / delta values (HistPrepKernel)
+// The column writer reads one change's ops through an op source (Src):
+//   u32 nOps, nPreds;
+//   bool num(int col, u32 i, long long& x)   numeric column value of op i (pred columns: pred i); false = null. Delta
+//                                            columns (keyCtr, chldCtr, predCtr) hold the differences already.
+//   bool keyNull(u32 i); bool keySame(u32 a, u32 b); void keyPut(ByteSink&, u32 i)   the keyStr column
+//   bool insert(u32 i); void valRaw(ByteSink&, u32 i)                              the insert and valRaw columns
+// HistChangeCtx is the source over the document's rows (history rebuild), EncChangeSrc (encchg.cuh) the one over a change table.
+template <class Src> struct ColNumAcc {   // numeric columns
+  const Src& s; int col;
+  HD bool isNull(u32 i) const { long long x; return !s.num(col, i, x); }
+  HD bool same(u32 a, u32 b) const { long long x = 0, y = 0; s.num(col, a, x); s.num(col, b, y); return x == y; }
+  HD void put(ByteSink& out, u32 i) const { long long x = 0; s.num(col, i, x); if (col == HC_KEY_CTR || col == HC_CHLD_CTR || col == HC_PRED_CTR) out.sleb(x); else out.uleb((u64)x); }
 };
-struct HistNumAcc {   // numeric columns
-  const HistChangeCtx& c; int col;
-  HD bool get(u32 i, long long& x) const {   // false = null
-    if (col == HC_PRED_ACTOR) { x = c.predA[c.predBase + i]; return true; }
-    if (col == HC_PRED_CTR) { x = c.predDelta[c.predBase + i]; return true; }
-    const u32 j = c.opStart + i, m = c.v.op(j);
-    switch (col) {
-      case HC_OBJ_ACTOR: if (c.objA[j] == NULL32) return false; x = c.objA[j]; return true;
-      case HC_OBJ_CTR: { const u64 o = c.v.objOf(m); if (!o) return false; x = (long long)id_ctr(o); return true; }
-      case HC_KEY_ACTOR: if (c.keyA[j] == NULL32) return false; x = c.keyA[j]; return true;
-      case HC_KEY_CTR: if (c.keyDelta[j] == NULLV) return false; x = c.keyDelta[j]; return true;
-      case HC_ACTION: x = c.v.actionOf(m); return true;
-      case HC_VAL_LEN: x = c.v.valLenOf(m); return true;
-      case HC_PRED_NUM: x = c.v.opPredNum[m]; return true;
-      default: return false;
-    }
-  }
-  HD bool isNull(u32 i) const { long long x; return !get(i, x); }
-  HD bool same(u32 a, u32 b) const { long long x = 0, y = 0; get(a, x); get(b, y); return x == y; }
-  HD void put(ByteSink& out, u32 i) const { long long x = 0; get(i, x); if (col == HC_KEY_CTR || col == HC_PRED_CTR) out.sleb(x); else out.uleb((u64)x); }
-};
-struct HistStrAcc {   // keyStr
-  const HistChangeCtx& c;
-  HD bool isNull(u32 i) const { return !c.v.isMapKey(c.v.op(c.opStart + i)); }
-  HD bool same(u32 a, u32 b) const {
-    const u32 ra = c.v.opSrc[c.v.op(c.opStart + a)], rb = c.v.opSrc[c.v.op(c.opStart + b)];
-    const u32 la = c.v.d.keyStrLen[ra], lb = c.v.d.keyStrLen[rb]; if (la != lb) return false;
-    const u8* pa = c.arena + c.v.d.keyStrOff[ra]; const u8* pb = c.arena + c.v.d.keyStrOff[rb];
-    for (u32 t = 0; t < la; t++) if (pa[t] != pb[t]) return false;
-    return true;
-  }
-  HD void put(ByteSink& out, u32 i) const { const u32 r = c.v.opSrc[c.v.op(c.opStart + i)]; out.uleb(c.v.d.keyStrLen[r]); out.bytes(c.arena + c.v.d.keyStrOff[r], c.v.d.keyStrLen[r]); }
+template <class Src> struct ColStrAcc {   // keyStr
+  const Src& s;
+  HD bool isNull(u32 i) const { return s.keyNull(i); }
+  HD bool same(u32 a, u32 b) const { return s.keySame(a, b); }
+  HD void put(ByteSink& out, u32 i) const { s.keyPut(out, i); }
 };
 // bytes of column `col` of the change (nothing for a column that encodes to nothing)
-HD void hist_column(ByteSink& out, const HistChangeCtx& c, int col) {
+template <class Src> HD void hist_column(ByteSink& out, const Src& s, int col) {
   switch (col) {
-    case HC_KEY_STR: hist_rle(out, HistStrAcc{c}, c.nOps); break;
+    case HC_KEY_STR: hist_rle(out, ColStrAcc<Src>{s}, s.nOps); break;
     case HC_INSERT: {   // BooleanEncoder (encoding.js:1061-1135): run lengths, starting with false
       bool last = false; u32 cnt = 0;
-      for (u32 i = 0; i < c.nOps; i++) { const bool b = c.v.insertOf(c.v.op(c.opStart + i)); if (b == last) cnt++; else { out.uleb(cnt); last = b; cnt = 1; } }
+      for (u32 i = 0; i < s.nOps; i++) { const bool b = s.insert(i); if (b == last) cnt++; else { out.uleb(cnt); last = b; cnt = 1; } }
       if (cnt > 0) out.uleb(cnt);
       break;
     }
-    case HC_VAL_RAW: for (u32 i = 0; i < c.nOps; i++) { const u32 m = c.v.op(c.opStart + i); if (!c.v.isDel(m)) { const u32 r = c.v.opSrc[m]; out.bytes(c.arena + c.v.d.valOff[r], c.v.d.valLen[r] >> 4); } } break;
-    case HC_PRED_ACTOR: case HC_PRED_CTR: hist_rle(out, HistNumAcc{c, col}, c.nPreds); break;
-    default: hist_rle(out, HistNumAcc{c, col}, c.nOps); break;
+    case HC_VAL_RAW: for (u32 i = 0; i < s.nOps; i++) s.valRaw(out, i); break;
+    case HC_PRED_ACTOR: case HC_PRED_CTR: hist_rle(out, ColNumAcc<Src>{s, col}, s.nPreds); break;
+    default: hist_rle(out, ColNumAcc<Src>{s, col}, s.nOps); break;
   }
 }
-HD u32 hist_column_id(int col) { const u32 ids[HC_NUM] = {0x01, 0x02, 0x11, 0x13, 0x15, 0x34, 0x42, 0x56, 0x57, 0x70, 0x71, 0x73}; return ids[col]; }
+HD u32 hist_column_id(int col) { const u32 ids[HC_NUM] = {0x01, 0x02, 0x11, 0x13, 0x15, 0x34, 0x42, 0x56, 0x57, 0x61, 0x63, 0x70, 0x71, 0x73}; return ids[col]; }
+
+// The change header (columnar.js:710-739 encodeChange, 659-686 encodeContainer), shared by both encoders. Others writes
+// the other actors: n(), put(ByteSink&, q) (length-prefixed id bytes). The dependency hashes are left as zeros: the hash
+// kernels write them in sorted order before hashing.
+struct ChangeHead { u32 nDeps; const u8* author; u32 authorLen; u64 seq, startOp; long long time; const u8* msg; u32 msgLen; };
+template <class Others> HD void change_body_head(ByteSink& b, const ChangeHead& h, const Others& others, const u32* colLen, u32* depsAt) {
+  b.uleb(h.nDeps); if (depsAt) *depsAt = b.n; b.zeros(32 * h.nDeps);
+  b.uleb(h.authorLen); b.bytes(h.author, h.authorLen); b.uleb(h.seq); b.uleb(h.startOp); b.sleb(h.time); b.uleb(h.msgLen); b.bytes(h.msg, h.msgLen);
+  b.uleb(others.n()); for (u32 q = 0; q < others.n(); q++) others.put(b, q);
+  u32 nCols = 0; for (int col = 0; col < HC_NUM; col++) if (colLen[col]) nCols++;
+  b.uleb(nCols);
+  for (int col = 0; col < HC_NUM; col++) if (colLen[col]) { b.uleb(hist_column_id(col)); b.uleb(colLen[col]); }
+}
+// Container header and body up to the column data into w (a sizing sink writes nothing). Returns the length of the whole
+// container (columns and extra bytes included); *depsAt, *bodyAt (the chunk type byte: where the hashed part starts) and
+// *dataAt (the first column's bytes) are offsets relative to the container.
+template <class Others> HD u32 write_change_head(ByteSink& w, const ChangeHead& h, const Others& others, const u32* colLen, u32 extraLen, u32* depsAt, u32* bodyAt, u32* dataAt) {
+  ByteSink s{nullptr, 0}; change_body_head(s, h, others, colLen, nullptr);
+  u32 dataLen = 0; for (int col = 0; col < HC_NUM; col++) dataLen += colLen[col];
+  const u32 bodyLen = s.n + dataLen + extraLen;
+  const u32 start = w.n;
+  w.put(0x85); w.put(0x6f); w.put(0x4a); w.put(0x83); w.zeros(4);
+  *bodyAt = w.n - start; w.put(1); w.uleb(bodyLen);
+  u32 d = 0; change_body_head(w, h, others, colLen, &d); *depsAt = d - start; *dataAt = w.n - start;
+  return 8 + 1 + uleb_size(bodyLen) + bodyLen;
+}
+
+// everything one change's encoder reads (op source over the document's rows)
+struct HistChangeCtx {
+  HistOpView v; const u8* arena; u32 k; u32 opStart, nOps, predBase, nPreds;
+  const u32* objA; const u32* keyA; const long long* keyDelta; const u32* predA; const long long* predDelta;   // local actor indexes / delta values (HistPrepKernel)
+  HD bool num(int col, u32 i, long long& x) const {   // false = null
+    if (col == HC_PRED_ACTOR) { x = predA[predBase + i]; return true; }
+    if (col == HC_PRED_CTR) { x = predDelta[predBase + i]; return true; }
+    const u32 j = opStart + i, m = v.op(j);
+    switch (col) {
+      case HC_OBJ_ACTOR: if (objA[j] == NULL32) return false; x = objA[j]; return true;
+      case HC_OBJ_CTR: { const u64 o = v.objOf(m); if (!o) return false; x = (long long)id_ctr(o); return true; }
+      case HC_KEY_ACTOR: if (keyA[j] == NULL32) return false; x = keyA[j]; return true;
+      case HC_KEY_CTR: if (keyDelta[j] == NULLV) return false; x = keyDelta[j]; return true;
+      case HC_ACTION: x = v.actionOf(m); return true;
+      case HC_VAL_LEN: x = v.valLenOf(m); return true;
+      case HC_PRED_NUM: x = v.opPredNum[m]; return true;
+      default: return false;   // (the document keeps no child columns: always null)
+    }
+  }
+  HD bool keyNull(u32 i) const { return !v.isMapKey(v.op(opStart + i)); }
+  HD bool keySame(u32 a, u32 b) const {
+    const u32 ra = v.opSrc[v.op(opStart + a)], rb = v.opSrc[v.op(opStart + b)];
+    const u32 la = v.d.keyStrLen[ra], lb = v.d.keyStrLen[rb]; if (la != lb) return false;
+    const u8* pa = arena + v.d.keyStrOff[ra]; const u8* pb = arena + v.d.keyStrOff[rb];
+    for (u32 t = 0; t < la; t++) if (pa[t] != pb[t]) return false;
+    return true;
+  }
+  HD void keyPut(ByteSink& out, u32 i) const { const u32 r = v.opSrc[v.op(opStart + i)]; out.uleb(v.d.keyStrLen[r]); out.bytes(arena + v.d.keyStrOff[r], v.d.keyStrLen[r]); }
+  HD bool insert(u32 i) const { return v.insertOf(v.op(opStart + i)); }
+  HD void valRaw(ByteSink& out, u32 i) const { const u32 m = v.op(opStart + i); if (!v.isDel(m)) { const u32 r = v.opSrc[m]; out.bytes(arena + v.d.valOff[r], v.d.valLen[r] >> 4); } }
+};
 
 struct HistChanges {   // decoded change metadata of the loaded document (one entry per change)
   const long long* actor; const long long* seq; const long long* maxOp; const long long* time; const u32* msgOff; const u32* msgLen;
@@ -248,6 +290,11 @@ struct HistPrepKernel {
     }
   }
 };
+struct HistOthers {   // the other actors of one change: document actors by rank (other: (change << 16 | rank), sorted)
+  const u64* other; u32 count; const u32* actorOfRank; const u32* repOff; const u32* repLen; const u8* arena;
+  HD u32 n() const { return count; }
+  HD void put(ByteSink& b, u32 q) const { const u32 a = actorOfRank[(u32)(other[q] & 0xffff)]; b.uleb(repLen[a]); b.bytes(arena + repOff[a], repLen[a]); }
+};
 // pass 0: size of the encoded change (container header + body); pass 1: the bytes (dependency hashes left as zeros)
 struct HistEncodeKernel {
   int pass; HistOpView v; HistChanges ch; const u8* arena; const u32* chOpStart; const u32* chNOps; const u32* opPredBase; u32 numOpsTotal; u32 numPredsTotal;
@@ -260,29 +307,17 @@ struct HistEncodeKernel {
     const u32 predEnd = nOps ? ((opStart + nOps < numOpsTotal) ? opPredBase[opStart + nOps] : numPredsTotal) : 0;
     HistChangeCtx c{v, arena, (u32)k, opStart, nOps, predBase, predEnd - predBase, objA, keyA, keyDelta, predA, predDelta};
     // column sizes first (the directory precedes the data)
-    u32 colLen[HC_NUM]; u32 nCols = 0, dataLen = 0, dirLen = 0;
-    for (int col = 0; col < HC_NUM; col++) { ByteSink s{nullptr, 0}; hist_column(s, c, col); colLen[col] = s.n; if (s.n) { nCols++; dataLen += s.n; dirLen += uleb_size(hist_column_id(col)) + uleb_size(s.n); } }
-    const u32 author = (u32)ch.actor[k]; const u32 nDeps = (u32)ch.depsNum[k];
-    const u32 nOther = otherStart[k + 1] - otherStart[k];
-    const u64 startOp = (u64)ch.maxOp[k] - nOps + 1;
+    u32 colLen[HC_NUM];
+    for (int col = 0; col < HC_NUM; col++) { ByteSink s{nullptr, 0}; hist_column(s, c, col); colLen[col] = s.n; }
+    const u32 author = (u32)ch.actor[k];
     const u32 msgLen = ch.msgLen[k] == NULL32 ? 0 : ch.msgLen[k];
-    // body size
-    ByteSink b{nullptr, 0};
-    b.uleb(nDeps); b.zeros(32 * nDeps); b.uleb(actorRepLen[author]); b.zeros(actorRepLen[author]); b.uleb((u64)ch.seq[k]); b.uleb(startOp); b.sleb(ch.time[k]); b.uleb(msgLen); b.zeros(msgLen);
-    b.uleb(nOther); for (u32 q = otherStart[k]; q < otherStart[k + 1]; q++) { const u32 a = actorOfRank[(u32)(other[q] & 0xffff)]; b.uleb(actorRepLen[a]); b.zeros(actorRepLen[a]); }
-    b.uleb(nCols); b.zeros(dirLen + dataLen + ch.extraLen[k]);
-    const u32 bodyLen = b.n; const u32 total = 8 + 1 + uleb_size(bodyLen) + bodyLen;
+    const ChangeHead h{(u32)ch.depsNum[k], arena + actorRepOff[author], actorRepLen[author], (u64)ch.seq[k], (u64)ch.maxOp[k] - nOps + 1, ch.time[k], arena + ch.msgOff[k], msgLen};
+    const HistOthers others{other + otherStart[k], otherStart[k + 1] - otherStart[k], actorOfRank, actorRepOff, actorRepLen, arena};
+    ByteSink w{pass ? outArena + outBase + outOff[k] : nullptr, 0};
+    u32 dAt = 0, bAt = 0, dataAt = 0;
+    const u32 total = write_change_head(w, h, others, colLen, ch.extraLen[k], &dAt, &bAt, &dataAt);
     if (pass == 0) { outLen[k] = total; return; }
-    ByteSink w{outArena + outBase + outOff[k], 0};
-    w.put(0x85); w.put(0x6f); w.put(0x4a); w.put(0x83); w.zeros(4); w.put(1); w.uleb(bodyLen);
-    bodyAt[k] = outBase + outOff[k] + 8;   // the hashed part starts at the chunk type byte
-    w.uleb(nDeps); depsAt[k] = outBase + outOff[k] + w.n; w.zeros(32 * nDeps);
-    w.uleb(actorRepLen[author]); w.bytes(arena + actorRepOff[author], actorRepLen[author]);
-    w.uleb((u64)ch.seq[k]); w.uleb(startOp); w.sleb(ch.time[k]);
-    w.uleb(msgLen); w.bytes(arena + ch.msgOff[k], msgLen);
-    w.uleb(nOther); for (u32 q = otherStart[k]; q < otherStart[k + 1]; q++) { const u32 a = actorOfRank[(u32)(other[q] & 0xffff)]; w.uleb(actorRepLen[a]); w.bytes(arena + actorRepOff[a], actorRepLen[a]); }
-    w.uleb(nCols);
-    for (int col = 0; col < HC_NUM; col++) if (colLen[col]) { w.uleb(hist_column_id(col)); w.uleb(colLen[col]); }
+    bodyAt[k] = outBase + outOff[k] + bAt; depsAt[k] = outBase + outOff[k] + dAt;
     for (int col = 0; col < HC_NUM; col++) if (colLen[col]) hist_column(w, c, col);
     w.bytes(arena + ch.extraOff[k], ch.extraLen[k]);
   }

@@ -88,6 +88,10 @@ class Library:
         L.amg_decode_history.argtypes = [vp, vp, vp]
         L.amg_last_decode_ms.restype = C.c_float
         L.amg_last_decode_ms.argtypes = [vp]
+        L.amg_encode_changes.restype = C.c_int
+        L.amg_encode_changes.argtypes = [vp, vp, C.c_size_t, vp, vp, vp, vp]
+        L.amg_last_encode_ms.restype = C.c_float
+        L.amg_last_encode_ms.argtypes = [vp]
 
     def check(self, rc, err):
         if rc != 0:
@@ -279,6 +283,116 @@ class FlatChanges:
 
     def __len__(self):
         return len(self.changes)
+
+    @classmethod
+    def from_changes(cls, changes):
+        """The inverse of to_changes(): the change table of a list of change dicts (the form columnar.encode_change takes).
+        Multi-ops are expanded, op ids parsed and values encoded by columnar's expand_multi_ops / parse_op_id / encode_value,
+        which raise their errors for what is wrong at the dict level; everything else is checked by the encoder. Each change's
+        actor table lists its actors in first-use order (the encoder writes the canonical one); preds and deps keep their order."""
+        from .columnar import expand_multi_ops, parse_op_id as _parse, encode_value, hex_bytes, ACTIONS as ACTION_NAMES
+
+        def parse_op_id(s):   # the table's counters are 32-bit, and 0xffffffff is its null
+            ctr, actor = _parse(s)
+            if ctr >= NULL32:
+                raise Unsupported(4, "amgpu: an operation counter beyond the change table's 32-bit fields: %s" % s)
+            return ctr, actor
+        blob = bytearray()   # the bytes section; offsets are relative to it until the layout is known
+
+        def put(b):
+            off = len(blob)
+            blob.extend(b)
+            return off
+        ch_cols = {f: [] for f in ('seq', 'startOp', 'time', 'msgOff', 'msgLen', 'depsOff', 'nDeps', 'actorFirst', 'nActors',
+                                   'extraOff', 'extraLen', 'hasExtra', 'firstOp', 'nOps', 'firstPred', 'nPreds')}
+        ops, preds, actors = [], [], []
+        for change in changes:
+            author = change['actor']
+            ids, order = {author: 0}, [author]
+
+            def num(a):
+                if a not in ids:
+                    ids[a] = len(order)
+                    order.append(a)
+                return ids[a]
+            first_op, first_pred = len(ops), len(preds)
+            for op in expand_multi_ops(change['ops'], change['startOp'], author):
+                if op['obj'] == '_root':
+                    oa = oc = NULL32
+                else:
+                    oc, a = parse_op_id(op['obj'])
+                    oa = num(a)
+                ka = kc = ks_off = ks_len = NULL32
+                if op.get('key'):
+                    k = op['key'].encode('utf-8')
+                    ks_off, ks_len = put(k), len(k)
+                elif op.get('elemId') == '_head':
+                    kc = 0
+                elif op.get('elemId') is not None:
+                    kc, a = parse_op_id(op['elemId'])
+                    if kc == 0:   # a counter-0 element id is not _head (columnar.js:193): the table cannot hold it
+                        raise ValueError('Unexpected operation key: %r' % (op,))
+                    ka = num(a)
+                act = op.get('action')
+                if act in ACTION_NAMES:
+                    act = ACTION_NAMES.index(act)
+                elif not isinstance(act, int):
+                    raise ValueError('Unexpected operation action: %r' % (act,))
+                val_len, raw = [], bytearray()
+                encode_value(op, val_len, raw)
+                ca = cc = NULL32
+                if op.get('child'):
+                    cc, a = parse_op_id(op['child'])
+                    ca = num(a)
+                p0 = len(preds)
+                for p in op.get('pred', []):
+                    c, a = parse_op_id(p)
+                    preds.append((num(a), c))
+                ops.append((oa, oc, ka, kc, ks_off, ks_len, 1 if op.get('insert') else 0, act, val_len[0], put(raw), ca, cc,
+                            p0, len(preds) - p0, len(ch_cols['seq']), 0))
+            deps = [hex_bytes(d) for d in change.get('deps', [])]
+            if any(len(d) != 32 for d in deps):
+                raise ValueError('a dependency is not a 32-byte hash')
+            msg = (change.get('message') or '').encode('utf-8')
+            extra = bytes(change.get('extraBytes') or b'')
+            for k, v in (('seq', change['seq']), ('startOp', change['startOp']), ('time', change.get('time', 0)),
+                         ('msgOff', put(msg)), ('msgLen', len(msg)), ('depsOff', put(b''.join(deps))), ('nDeps', len(deps)),
+                         ('actorFirst', len(actors)), ('nActors', len(order)), ('extraOff', put(extra)), ('extraLen', len(extra)),
+                         ('hasExtra', 1 if extra else 0), ('firstOp', first_op), ('nOps', len(ops) - first_op),
+                         ('firstPred', first_pred), ('nPreds', len(preds) - first_pred)):
+                ch_cols[k].append(v)
+            for a in order:
+                b = hex_bytes(a)
+                actors.append((put(b), len(b)))
+        n, M, P, A = len(ch_cols['seq']), len(ops), len(preds), len(actors)
+        changes_off = 96
+        ops_off = changes_off + n * CHANGE_DT.itemsize
+        preds_off = ops_off + M * OP_DT.itemsize
+        actors_off = preds_off + P * PRED_DT.itemsize
+        bytes_off = actors_off + A * ACTOR_DT.itemsize
+        size = (bytes_off + len(blob) + 7) & ~7
+        raw = bytearray(size)
+        np.frombuffer(raw, dtype='<u8', count=12)[:] = [0x31474843474d41, n, changes_off, M, ops_off, P, preds_off, A, actors_off,
+                                                        bytes_off, len(blob), 0]
+        ch = np.frombuffer(raw, dtype=CHANGE_DT, count=n, offset=changes_off)
+        for k, v in ch_cols.items():
+            ch[k] = v
+        for k in ('msgOff', 'depsOff', 'extraOff'):
+            ch[k] += bytes_off
+        if M:
+            o = np.frombuffer(raw, dtype=OP_DT, count=M, offset=ops_off)
+            o[:] = np.array(ops, dtype=np.uint32).view(OP_DT).reshape(M)
+            for k, nk in (('keyStrOff', 'keyStrLen'), ('valOff', None)):
+                sel = o[nk] != NULL32 if nk else slice(None)
+                o[k][sel] += bytes_off
+        if P:
+            np.frombuffer(raw, dtype=PRED_DT, count=P, offset=preds_off)[:] = np.array(preds, dtype=np.uint32).view(PRED_DT).reshape(P)
+        if A:
+            a = np.frombuffer(raw, dtype=ACTOR_DT, count=A, offset=actors_off)
+            a[:] = np.array(actors, dtype=np.uint32).view(ACTOR_DT).reshape(A)
+            a['off'] += bytes_off
+        raw[bytes_off:bytes_off + len(blob)] = blob
+        return cls(bytes(raw))
 
     def hashes(self):
         return [bytes(h).hex() for h in self.changes['hash']]
@@ -566,6 +680,36 @@ class GpuBackendDoc:
     def last_decode_ms(self):
         """Device span of the last decode_*_flat call (CUDA events), ms."""
         return float(self._lib.L.amg_last_decode_ms(self.h))
+
+    # ---- encodeChange (columnar.js:710-739), on the device
+    def encode_flat(self, table, length=None):
+        """amg_encode_changes: encodeChange of every change of a change table - a FlatChanges, the table's bytes, a numpy array
+        or a pointer (int) to pinned or device memory with `length`. Returns (binary changes, hashes as hex strings); the
+        document is not touched. Raises AmgError with `.failed_index` = the first failing change."""
+        if isinstance(table, FlatChanges):
+            table = table.raw
+        if isinstance(table, bytes):
+            n, buf = len(table), C.cast(C.c_char_p(table), C.c_void_p)
+        elif isinstance(table, (bytearray, memoryview)):
+            table = bytes(table)
+            n, buf = len(table), C.cast(C.c_char_p(table), C.c_void_p)
+        elif isinstance(table, np.ndarray):
+            n, buf = table.nbytes, table.ctypes.data_as(C.c_void_p)
+        else:
+            n, buf = int(length), C.c_void_p(int(table))
+        bc, bh, failed, err = C.c_void_p(), C.c_void_p(), C.c_size_t(), _ErrStruct()
+        rc = self._lib.L.amg_encode_changes(self.h, buf, C.c_size_t(n), C.byref(bc), C.byref(bh), C.byref(failed), C.byref(err))
+        try:
+            self._lib.check(rc, err)
+        except AmgError as e:
+            e.failed_index = failed.value
+            raise
+        hx = self._buffers(bh)[0].hex()
+        return self._buffers(bc), [hx[i:i + 64] for i in range(0, len(hx), 64)]
+
+    def last_encode_ms(self):
+        """Device span of the last encode_flat call (CUDA events), ms."""
+        return float(self._lib.L.amg_last_encode_ms(self.h))
 
     def dump_ops(self):
         rows, n, succ, m, err = C.c_void_p(), C.c_size_t(), C.c_void_p(), C.c_size_t(), _ErrStruct()

@@ -116,7 +116,26 @@ float amg_last_decode_ms(amg_backend* b);
  *   bytes  : the decoded change containers back to back (inflated)
  * 0xffffffff is null (keyStrLen null: no key string column value; an empty string has length 0). msgOff, depsOff (nDeps x 32
  * bytes), extraOff, keyStrOff, valOff and the actor entries' off are offsets INTO THE TABLE. action is the raw action number,
- * valLen the VALUE_LEN tag (length << 4 | type, columnar.js:46-49); every value has been checked like decodeValue does. */
+ * valLen the VALUE_LEN tag (length << 4 | type, columnar.js:46-49); every value has been checked like decodeValue does.
+ *
+ * What amg_encode_changes reads of a table: the header's changes, ops, preds and actors sections; per change seq, startOp,
+ * time, the message, the deps (hashes, any order), the extra bytes when hasExtra is set, actorFirst / nActors and firstOp /
+ * nOps; per op every field but `change` and `pad`; preds (any order). It ignores the hash, the bytes section (bytesOff /
+ * bytesLen: the offsets point anywhere into the table), pad and the change's firstPred / nPreds beyond a range check (the ops'
+ * predFirst / predNum say which preds are theirs). A change's actor table is only the mapping from its actor numbers to
+ * actor ids: the encoder writes the canonical one (author first, then the actors the ops use, sorted by id bytes), so
+ * unused, repeated or unsorted entries encode like the canonical table. keyStrLen > 0 is a map key; otherwise keyCtr 0 with
+ * insert is _head and keyCtr > 0 an element id. A value is written for action 1 (set) and 5 (inc) only. */
+/* columnar.js:710-739 encodeChange over the n changes of a change table in the layout amg_decode_changes returns (table may
+ * be pinned, pageable or device memory; table_len bytes). out_changes: n binary changes as encodeChange returns them, i.e.
+ * chunk type 2 (zlib level 6, columnar.js:738, 798-808) when the plain change is >= 256 bytes; out_hashes: one buffer of
+ * n x 32 bytes. On error *failed_index is the smallest failing change (a damaged table is AMG_RANGE_ERROR naming the change;
+ * a damaged header names change 0). A change whose encoding may reach 4 GiB (its ops may share one value or key
+ * string) is AMG_UNSUPPORTED, found before anything is sized. The document is not touched. */
+int amg_encode_changes(amg_backend* b, const uint8_t* table, size_t table_len, amg_buffers** out_changes,
+                       amg_buffers** out_hashes, size_t* failed_index, amg_error* err);
+/* device span of the last amg_encode_changes call in ms (CUDA events on the engine's main stream, like amg_last_decode_ms) */
+float amg_last_encode_ms(amg_backend* b);
 
 /* returned buffer lists */
 size_t amg_buffers_count(const amg_buffers* l);
