@@ -248,6 +248,23 @@ napi_value EncodeChanges(napi_env env, napi_callback_info info) {
 }
 // decodeHistory(state) — decodeChanges(getAllChanges(state)), read from device memory: the change table as one Uint8Array
 napi_value DecodeHistory(napi_env env, napi_callback_info info) { return listCall(env, info, amg_decode_history, true); }
+// historyPatches(state, prefixLengths) — src/automerge.js:105-118 getHistory's snapshots: for every k of the array, the flat
+// patch (layout: amgpu.h) of getPatch(loadChanges(init(), getAllChanges(state).slice(0, k))), one Uint8Array each
+napi_value HistoryPatches(napi_env env, napi_callback_info info) {
+  napi_value argv[2]; amg_backend* b; if (!getArgs(env, info, 2, argv) || !getBackend(env, argv[0], &b)) return nullptr;
+  bool isArray = false; napi_is_array(env, argv[1], &isArray);
+  if (!isArray) { napi_throw_type_error(env, nullptr, "prefixLengths must be an array of numbers"); return nullptr; }
+  uint32_t n = 0; napi_get_array_length(env, argv[1], &n);
+  std::vector<uint64_t> lens(n);
+  for (uint32_t i = 0; i < n; i++) {
+    napi_value el; double k = 0; napi_get_element(env, argv[1], i, &el);
+    if (napi_get_value_double(env, el, &k) != napi_ok || !(k >= 0) || k != (double)(uint64_t)k) { napi_throw_type_error(env, nullptr, "prefixLengths must be an array of non-negative integers"); return nullptr; }
+    lens[i] = (uint64_t)k;
+  }
+  amg_buffers* l = nullptr; amg_error err;
+  if (amg_get_history_patches(b, lens.data(), n, &l, &err)) return throwAmg(env, err);
+  return buffersToJs(env, l);
+}
 // Backend.free — backend/backend.js:16-19: releases the device memory now instead of at garbage collection
 napi_value Free(napi_env env, napi_callback_info info) {
   napi_value argv[1]; Holder* h; if (!getArgs(env, info, 1, argv) || !getHolder(env, argv[0], &h)) return nullptr;
@@ -261,7 +278,7 @@ napi_value InitModule(napi_env env, napi_value exports) {
     {"getHeads", GetHeads}, {"getChanges", GetChanges}, {"getChangesAdded", GetChangesAdded}, {"getChangeByHash", GetChangeByHash},
     {"getMissingDeps", GetMissingDeps}, {"clockOf", ClockOf}, {"hashByActor", HashByActor}, {"syncBloom", SyncBloom},
     {"syncChangesToSend", SyncChangesToSend}, {"decodeChanges", DecodeChanges}, {"decodeHistory", DecodeHistory},
-    {"encodeChanges", EncodeChanges}};
+    {"encodeChanges", EncodeChanges}, {"historyPatches", HistoryPatches}};
   for (auto& f : fns) { napi_value fn; napi_create_function(env, f.name, NAPI_AUTO_LENGTH, f.fn, nullptr, &fn); napi_set_named_property(env, exports, f.name, fn); }
   return exports;
 }

@@ -4,7 +4,7 @@
 
 The module object `Backend` mirrors the module a caller hands to `Automerge.setDefaultBackend()`.
 """
-from .backend import Backend as _Facade
+from .backend import Backend as _Facade, backend_state as _backend_state
 from .engine import GpuBackendDoc, AmgError, Unsupported, FlatChanges, decode_changes as _decode_changes, _decoder_for
 
 from . import sync as _sync
@@ -44,5 +44,37 @@ def encodeChange(change):
     return out[0]
 
 
+class HistoryEntry:
+    """One entry of getHistory: `change` and `snapshot` are computed when first read, like the reference's getters."""
+
+    def __init__(self, history, index):
+        self._history, self._index = history, index
+
+    @property
+    def change(self):
+        """decodeChange of the entry's change (all of the list's changes are decoded in one device call, once)."""
+        h = self._history
+        if h['changes'] is None:
+            h['changes'] = h['doc'].decode_history_flat().to_changes()
+        return h['changes'][self._index]
+
+    @property
+    def snapshot(self):
+        """The patch getPatch(loadChanges(init(), history[:index + 1])) returns, filtered on the device from the document's op
+        table. There is no frontend here, so it is the patch, not a document."""
+        return self._history['doc'].history_patches([self._index + 1])[0]
+
+
+def getHistory(backend):
+    """Automerge.getHistory (src/automerge.js:105-118) at the backend level: one entry per change of getAllChanges(backend).
+    No change bytes leave the device. Later changes to the document only append to getAllChanges order, so the entries
+    stay valid."""
+    doc = _backend_state(backend)
+    n = sum(doc.clock().values())   # every actor's changes have seq 1 .. clock[actor]
+    history = {'doc': doc, 'changes': None}
+    return [HistoryEntry(history, i) for i in range(n)]
+
+
 Backend = bind_sync(_Facade(GpuBackendDoc))
-__all__ = ['Backend', 'GpuBackendDoc', 'AmgError', 'Unsupported', 'bind_sync', 'decodeChange', 'decodeChanges', 'encodeChange', 'encodeChanges']
+__all__ = ['Backend', 'GpuBackendDoc', 'AmgError', 'Unsupported', 'bind_sync', 'decodeChange', 'decodeChanges', 'encodeChange', 'encodeChanges',
+           'getHistory', 'HistoryEntry']

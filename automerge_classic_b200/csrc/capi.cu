@@ -281,6 +281,14 @@ int amg_encode_changes(amg_backend* b, const uint8_t* table, size_t table_len, a
   catch (std::exception& e) { amg::drop_pending_peeks(); setErr(err, AMG_INTERNAL_ERROR, e.what()); return AMG_INTERNAL_ERROR; }
 }
 float amg_last_encode_ms(amg_backend* b) { return b->eng.lastEncodeMs; }
+// src/automerge.js:105-118 getHistory's snapshots: getPatch(loadChanges(init(), getAllChanges()[0, k))) for every k
+int amg_get_history_patches(amg_backend* b, const uint64_t* prefix_lens, size_t n, amg_buffers** out, amg_error* err) {
+  AMG_GUARD(
+    auto* l = new amg_buffers(); std::unique_ptr<amg_buffers> guard(l);
+    b->eng.historyPatches((const u64*)prefix_lens, n, l->items);
+    *out = guard.release(); return 0;)
+}
+float amg_last_history_ms(amg_backend* b) { return b->eng.lastHistoryMs; }
 // new.js:1979-1997
 int amg_get_changes_added(amg_backend* bn, amg_backend* bo, amg_buffers** out, amg_error* err) {
   AMG_GUARD(

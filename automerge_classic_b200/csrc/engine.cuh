@@ -30,6 +30,7 @@
 #include "sync.cuh"
 #include "changes.cuh"
 #include "encchg.cuh"
+#include "snapshot.cuh"
 #include "unknowncols.hpp"
 
 namespace amg {
@@ -409,6 +410,13 @@ class Engine {
   };
   void saveDocument(std::string& result);   // the phases, in order:
   void saveChangeColumns(SaveCall& s), saveOpColumns(SaveCall& s); void packDocument(SaveCall& s, std::string& result);
+  // Change metadata of every applied change (save() and historyPatches): the first L from the loaded document's columns, the
+  // K = C - L later ones from their headers in the arena (ParseKernel, their dependency hashes resolved to change indexes).
+  // parseChangeMeta fills the engine's meta / depIdx scratch; changeMetaColumn then writes column `col` (CHANGE_COLS
+  // index) for all C changes, or for the loadedDeps + laterDeps dependency indexes.
+  struct ChangeMetaCall { size_t C, L, K; u32 loadedDeps = 0, laterDeps = 0; };
+  void parseChangeMeta(ChangeMetaCall& m);
+  void changeMetaColumn(const ChangeMetaCall& m, int col, long long* out, u32* strOff, u32* strLen);
   // computeHashGraph's tables live as long as the call (they go back to the pool when it ends)
   struct HistoryCall {
     size_t L, N, S, A; DocRows d; HostClock t0;
@@ -471,6 +479,24 @@ class Engine {
   void copyEncodeOutput(EncodeCall& e, std::string& out, std::vector<u64>& offs, std::string& hashesOut);
   [[noreturn]] void throwEncodeError(EncodeCall& e, const u64* words);
   size_t encodeFailed = 0; float lastEncodeMs = 0;   // failing change of the last call; its device span (CUDA events; 0 in the emulation build)
+
+  // ---------------------------------------------------------------- getHistory snapshots (snapshot.cuh)
+  // The whole-document patch of the first k applied changes (getAllChanges order) for every k of a list: the op table
+  // filtered to the prefix's rows and succ entries, then buildPatch as getPatch runs it. The per-change tables are built
+  // once per call and shared by its prefix lengths; the document is not touched.
+  struct HistoryPatchCall {
+    size_t C = 0, A = 0, N = 0, S = 0, D = 0;   // applied changes, actors, rows, succ entries, dependency edges
+    ChangeMetaCall m{};
+    DBuf<long long> cActor, cSeq, cMaxOp, cDepsNum, depIdxV; DBuf<u32> strOff, strLen, depsNum32, depBase, depIdx;
+    DBuf<u64> chKey; DBuf<u32> changeOrder, actorStart, rowChange, succChange, firstDep;
+    DBuf<u32> keep, rowPos, cnt, cntPos, headFlag, headPos, headIdx; DBuf<u64> clock; DBuf<u8> headHashes;   // per prefix length
+  };
+  void historyPatches(const u64* prefixLens, size_t n, std::vector<std::string>& out);   // the phases, in order:
+  void snapChangeMeta(HistoryPatchCall& h), snapActorOrder(HistoryPatchCall& h), snapChangeIndexes(HistoryPatchCall& h);
+  size_t snapFilter(HistoryPatchCall& h, size_t k);   // per prefix length: the prefix document into snapDoc (returns its rows)
+  void snapHeader(HistoryPatchCall& h, size_t k, PatchOut& out);
+  float lastHistoryMs = 0;   // device span of the last historyPatches call (CUDA events; 0 in the emulation build)
+  DocBufs snapDoc; DBuf<u32> snapSuccOff, snapSuccCnt; DBuf<u64> snapSucc;   // the prefix document (grow-only; never the document's own)
  private:
   void uploadCandidates(const u32* idx, size_t count);
   void syncTimer(bool start);

@@ -53,6 +53,7 @@ inline void Engine::finishPatch(PatchOut& out) {
   size_t small = 64 + out.actor.size(); for (auto& a : out.actors) small += 8 + a.size(); small += out.clock.size() * 16 + out.deps.size() * 32 + 64;
   patchBuf.ensure(out.bigEnd + small);   // growth preserves what is already there
   u8* b = patchBuf.p; size_t at = out.bigEnd;
+  for (size_t i = out.valBytesOff + out.valBytesLen; i < out.bigEnd; i++) b[i] = 0;   // the bytes section's padding: equal patches are equal bytes
   auto pad8 = [&]() { while (at % 8) b[at++] = 0; };
   u64 hdr[PATCH_HDR_WORDS] = {0}; hdr[0] = 0x31504747414d41ULL; hdr[1] = out.maxOp; hdr[2] = out.pendingChanges; hdr[3] = out.hasActorSeq ? 1 : 0; hdr[4] = out.seq;
   pad8(); hdr[5] = at; hdr[6] = out.actor.size(); memcpy(b + at, out.actor.data(), out.actor.size()); at += out.actor.size(); pad8();
@@ -1457,10 +1458,30 @@ inline void Engine::saveDocument(std::string& result) {
 
 // change metadata (new.js:1680-1692 appendChange); the first L rows come from the loaded document's own columns
 inline void Engine::saveChangeColumns(SaveCall& s) {
-  const size_t C = s.C, N = s.N, L = s.L, K = s.K;
+  const size_t C = s.C, N = s.N, L = s.L;
   if (C == 0) return;
   ColumnEncoder& enc = *encoder;
-  u32 totalDeps = 0, loadedDeps = 0;
+  ChangeMetaCall m{C, L, s.K};
+  parseChangeMeta(m);
+  const u32 loadedDeps = m.loadedDeps, totalDeps = m.laterDeps;
+  saveVals.ensure(ctx, std::max<size_t>(std::max(std::max(C, N), s.S), (size_t)loadedDeps + totalDeps) + 2);
+  saveStrOff.ensure(ctx, std::max(C, N) + 1); saveStrLen.ensure(ctx, std::max(C, N) + 1);
+  auto col = [&](int k) { changeMetaColumn(m, k, saveVals.p, saveStrOff.p, saveStrLen.p); };
+  auto add = [&](int k, size_t len) { s.changeCols.push_back({CHANGE_COLS[k].id, enc.outLen - len, len}); };
+  col(CC_ACTOR);      add(CC_ACTOR, enc.rleNum(saveVals.p, C, false));
+  col(CC_SEQ);        add(CC_SEQ, enc.deltaNum(saveVals.p, C));
+  col(CC_MAX_OP);     add(CC_MAX_OP, enc.deltaNum(saveVals.p, C));
+  col(CC_TIME);       add(CC_TIME, enc.deltaNum(saveVals.p, C));
+  col(CC_MESSAGE);    add(CC_MESSAGE, enc.rle(StrCol{arena.p, saveStrOff.p, saveStrLen.p}, C));
+  col(CC_DEPS_NUM);   add(CC_DEPS_NUM, enc.rleNum(saveVals.p, C, false));
+  col(CC_DEPS_INDEX); add(CC_DEPS_INDEX, enc.deltaNum(saveVals.p, (size_t)loadedDeps + totalDeps));
+  col(CC_EXTRA_LEN);  add(CC_EXTRA_LEN, enc.rleNum(saveVals.p, C, false));
+                      add(CC_EXTRA_RAW, enc.raw(arena.p, saveStrOff.p, saveStrLen.p, C));
+  checkErr();
+}
+
+inline void Engine::parseChangeMeta(ChangeMetaCall& m) {
+  const size_t C = m.C, L = m.L, K = m.K;
   if (K > 0) {
     chPairs.ensure(ctx, K); chOff.ensure(ctx, K); chLen.ensure(ctx, K);
     h2d(ctx, chPairs.p, changes.data() + L, K * sizeof(HostChange));
@@ -1469,8 +1490,8 @@ inline void Engine::saveChangeColumns(SaveCall& s) {
     nOps.ensure(ctx, K + 1); nPreds.ensure(ctx, K + 1); nDeps.ensure(ctx, K + 1); nActors.ensure(ctx, K + 1);
     foreach(ctx, K, ParseKernel{arena.p, chOff.p, chLen.p, K, meta.p, colOff.p, colLen.p, nOps.p, nPreds.p, nDeps.p, nActors.p, errWord.p, flagWord.p + 8});
     depBase.ensure(ctx, K + 1); scan_exclusive(ctx, scanTmp, nDeps.p, depBase.p, K);
-    totalDeps = readU32(depBase.p + K);
-    depIdx.ensure(ctx, totalDeps + 1); primary.ensure(ctx, K);
+    m.laterDeps = readU32(depBase.p + K);
+    depIdx.ensure(ctx, m.laterDeps + 1); primary.ensure(ctx, K);
     const size_t tcap = pow2_at_least(2 * C + 2);
     hashTable.ensure(ctx, tcap); dev_memset(ctx, hashTable.p, 0xff, tcap * 4);
     foreach(ctx, C, HashInsertKernel{hashes.p, hashTable.p, (u64)tcap - 1});
@@ -1484,25 +1505,27 @@ inline void Engine::saveChangeColumns(SaveCall& s) {
       foreach_warp(ctx, 1, LoadedColKernel{LC_SUM, arena.p, dn.off, dn.len, 0, 0, nullptr, nullptr, nullptr, sumD.p});
       d2h(ctx, &sum, sumD.p, 8); sync(ctx);
     }
-    loadedDeps = (u32)sum;
+    m.loadedDeps = (u32)sum;
   }
-  saveVals.ensure(ctx, std::max<size_t>(std::max(std::max(C, N), s.S), (size_t)loadedDeps + totalDeps) + 2);
-  saveStrOff.ensure(ctx, std::max(C, N) + 1); saveStrLen.ensure(ctx, std::max(C, N) + 1);
-  auto loadedVal = [&](int k, size_t count) { if (L > 0) decodeLoadedCol(k, count, saveVals.p, saveStrOff.p, saveStrLen.p); };
-  auto changeVal = [&](int which) { if (K > 0) foreach(ctx, K, SaveChangeValKernel{which, arena.p, meta.p, actorSlots.p, (u64)actorCap - 1, saveVals.p + L, saveStrOff.p + L, saveStrLen.p + L, errWord.p}); };
-  auto add = [&](int k, size_t len) { s.changeCols.push_back({CHANGE_COLS[k].id, enc.outLen - len, len}); };
-  loadedVal(CC_ACTOR, L);     changeVal(SM_ACTOR);     add(CC_ACTOR, enc.rleNum(saveVals.p, C, false));
-  loadedVal(CC_SEQ, L);       changeVal(SM_SEQ);       add(CC_SEQ, enc.deltaNum(saveVals.p, C));
-  loadedVal(CC_MAX_OP, L);    changeVal(SM_MAX_OP);    add(CC_MAX_OP, enc.deltaNum(saveVals.p, C));
-  loadedVal(CC_TIME, L);      changeVal(SM_TIME);      add(CC_TIME, enc.deltaNum(saveVals.p, C));
-  loadedVal(CC_MESSAGE, L);   if (K > 0) foreach(ctx, K, SaveMessageKernel{meta.p, saveStrOff.p + L, saveStrLen.p + L});
-                              add(CC_MESSAGE, enc.rle(StrCol{arena.p, saveStrOff.p, saveStrLen.p}, C));
-  loadedVal(CC_DEPS_NUM, L);  changeVal(SM_DEPS_NUM);  add(CC_DEPS_NUM, enc.rleNum(saveVals.p, C, false));
-  loadedVal(CC_DEPS_INDEX, loadedDeps); if (totalDeps > 0) foreach(ctx, totalDeps, SaveDepIndexKernel{depIdx.p, saveVals.p + loadedDeps});
-                              add(CC_DEPS_INDEX, enc.deltaNum(saveVals.p, (size_t)loadedDeps + totalDeps));
-  loadedVal(CC_EXTRA_LEN, L); changeVal(SM_EXTRA_LEN); add(CC_EXTRA_LEN, enc.rleNum(saveVals.p, C, false));
-                              add(CC_EXTRA_RAW, enc.raw(arena.p, saveStrOff.p, saveStrLen.p, C));
-  checkErr();
+}
+
+inline void Engine::changeMetaColumn(const ChangeMetaCall& m, int col, long long* out, u32* strOff, u32* strLen) {
+  const size_t L = m.L, K = m.K;
+  if (col == CC_DEPS_INDEX) {
+    if (L > 0) decodeLoadedCol(CC_DEPS_INDEX, m.loadedDeps, out, strOff, strLen);
+    if (m.laterDeps > 0) foreach(ctx, m.laterDeps, SaveDepIndexKernel{depIdx.p, out + m.loadedDeps});
+    return;
+  }
+  if (L > 0) decodeLoadedCol(col, L, out, strOff, strLen);
+  if (K == 0) return;
+  if (col == CC_MESSAGE) { foreach(ctx, K, SaveMessageKernel{meta.p, strOff + L, strLen + L}); return; }
+  int which = SM_ACTOR;
+  switch (col) {
+    case CC_ACTOR: which = SM_ACTOR; break; case CC_SEQ: which = SM_SEQ; break; case CC_MAX_OP: which = SM_MAX_OP; break;
+    case CC_TIME: which = SM_TIME; break; case CC_DEPS_NUM: which = SM_DEPS_NUM; break; case CC_EXTRA_LEN: which = SM_EXTRA_LEN; break;
+    default: throw Error(AMG_ERR_INTERNAL, "changeMetaColumn: no values for column " + std::to_string(col));
+  }
+  foreach(ctx, K, SaveChangeValKernel{which, arena.p, meta.p, actorSlots.p, (u64)actorCap - 1, out + L, strOff + L, strLen + L, errWord.p});
 }
 
 // document ops (columnar.js:60-82); chldActor / chldCtr are always null in this format version: empty
@@ -2240,6 +2263,118 @@ inline void Engine::gatherHashes(const std::vector<u32>& idx, std::string& out) 
   foreach(ctx, idx.size(), SyncHashGatherKernel{hashes.p, syncIdx.p, syncHashOut.p});
   d2h(ctx, &out[0], syncHashOut.p, out.size()); sync(ctx);
   syncTimer(false);   // adds to the span of the syncChangesToSend call it follows
+}
+
+
+// ------------------------------------------------------------ getHistory snapshots (snapshot.cuh; src/automerge.js:105-118)
+// out[i] = the flat whole-document patch that getPatch(loadChanges(init(), getAllChanges()[0, prefixLens[i]))) returns
+inline void Engine::historyPatches(const u64* prefixLens, size_t n, std::vector<std::string>& out) {
+  out.clear(); lastHistoryMs = 0;
+  for (size_t i = 0; i < n; i++)
+    if (prefixLens[i] > numApplied) throw Error(AMG_ERR_RANGE, "history prefix length " + std::to_string(prefixLens[i]) + " exceeds the " + std::to_string(numApplied) + " applied changes");
+  if (n == 0) return;
+  if (!loaded.haveHashGraph) computeHashGraph();   // the prefixes' heads are change hashes (as amg_decode_history)
+  HistoryPatchCall h; h.C = numApplied; h.A = st.actorIds.size(); h.N = numRows; h.S = numSucc;
+  if (h.C >= (1u << 31) || h.N + h.S >= (1u << 31)) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: document too large for history snapshots");
+  const float keepSyncMs = lastSyncMs; lastSyncMs = 0;
+  struct Restore { Engine& e; float ms; ~Restore() { e.lastSyncMs = ms; } } restore{*this, keepSyncMs};   // the timer is shared with the sync calls
+  struct SideJoin { Ctx& c; ~SideJoin() { side_join(c); } } sideJoin{ctx};
+  syncTimer(true);
+  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+  if (h.C) { snapChangeMeta(h); snapActorOrder(h); snapChangeIndexes(h); }
+  const Ord ord{actorRank.p, bits_for(std::max<size_t>(h.A, 2) - 1)};
+  for (size_t i = 0; i < n; i++) {
+    const size_t k = (size_t)prefixLens[i];
+    dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+    const size_t Nk = snapFilter(h, k);
+    PatchOut p;
+    buildPatch(PatchInputs{snapDoc.view(), Nk, true, snapSuccOff.p, snapSucc.p, snapSuccCnt.p, ord}, p);
+    side_join(ctx); sync(ctx);
+    checkErr();
+    snapHeader(h, k, p);
+    finishPatch(p);
+    out.emplace_back((const char*)p.bytes, p.bytesLen);   // patchBuf is reused by the next prefix length
+  }
+  syncTimer(false); lastHistoryMs = lastSyncMs;
+}
+
+// 1. actor number, seq, maxOp and dependency indexes of every applied change (the change metadata phase save() uses)
+inline void Engine::snapChangeMeta(HistoryPatchCall& h) {
+  const size_t C = h.C;
+  h.m = ChangeMetaCall{C, loaded.numChanges, C - loaded.numChanges};
+  parseChangeMeta(h.m);
+  h.D = (size_t)h.m.loadedDeps + h.m.laterDeps;
+  for (DBuf<long long>* b : {&h.cActor, &h.cSeq, &h.cMaxOp, &h.cDepsNum}) b->ensure(ctx, C + 1);
+  h.strOff.ensure(ctx, std::max(C, h.D) + 1); h.strLen.ensure(ctx, std::max(C, h.D) + 1); h.depsNum32.ensure(ctx, C + 1); h.depBase.ensure(ctx, C + 2);
+  h.depIdxV.ensure(ctx, h.D + 1); h.depIdx.ensure(ctx, h.D + 1);
+  changeMetaColumn(h.m, CC_ACTOR, h.cActor.p, h.strOff.p, h.strLen.p);
+  changeMetaColumn(h.m, CC_SEQ, h.cSeq.p, h.strOff.p, h.strLen.p);
+  changeMetaColumn(h.m, CC_MAX_OP, h.cMaxOp.p, h.strOff.p, h.strLen.p);
+  changeMetaColumn(h.m, CC_DEPS_NUM, h.cDepsNum.p, h.strOff.p, h.strLen.p);
+  changeMetaColumn(h.m, CC_DEPS_INDEX, h.depIdxV.p, h.strOff.p, h.strLen.p);
+  foreach(ctx, C, HistI64ToU32Kernel{h.cDepsNum.p, h.depsNum32.p});
+  scan_exclusive(ctx, scanTmp, h.depsNum32.p, h.depBase.p, C);
+  foreach(ctx, h.D, HistI64ToU32Kernel{h.depIdxV.p, h.depIdx.p});
+  checkErr();
+}
+
+// 2. each actor's changes by seq (the history kernels: key = actor << 40 | seq, radix sort, segment starts)
+inline void Engine::snapActorOrder(HistoryPatchCall& h) {
+  const size_t C = h.C, A = h.A;
+  h.chKey.ensure(ctx, C + 1); h.changeOrder.ensure(ctx, C + 1); h.actorStart.ensure(ctx, A + 2);
+  foreach(ctx, C, HistChangeKeyKernel{h.cActor.p, h.cSeq.p, h.chKey.p, h.changeOrder.p});
+  radix_sort_pairs(ctx, sortTmp, h.chKey, h.changeOrder, C, 0, 40); radix_sort_pairs(ctx, sortTmp, h.chKey, h.changeOrder, C, 40, 57);
+  foreach(ctx, A + 1, HistLowerBoundKernel{h.chKey.p, (u32)C, 40, h.actorStart.p});
+}
+
+// 3. the change of every row id and succ entry; the first dependent of every change
+inline void Engine::snapChangeIndexes(HistoryPatchCall& h) {
+  const size_t C = h.C, N = h.N, S = h.S;
+  h.rowChange.ensure(ctx, N + 1); h.succChange.ensure(ctx, S + 1); h.firstDep.ensure(ctx, C + 1);
+  foreach(ctx, N, SnapChangeOfKernel{doc.id.p, h.actorStart.p, h.changeOrder.p, h.cMaxOp.p, (u32)h.A, h.rowChange.p, errWord.p});
+  foreach(ctx, S, SnapChangeOfKernel{succ.p, h.actorStart.p, h.changeOrder.p, h.cMaxOp.p, (u32)h.A, h.succChange.p, errWord.p});
+  dev_memset(ctx, h.firstDep.p, 0xff, (C + 1) * 4);
+  foreach(ctx, h.D, SnapFirstDepKernel{h.depBase.p, h.depIdx.p, (u32)C, h.firstDep.p});
+  checkErr();
+}
+
+// 4. per prefix length: flag the kept rows and count their kept succ entries, two scans, one gather
+inline size_t Engine::snapFilter(HistoryPatchCall& h, size_t k) {
+  const size_t N = h.N;
+  if (k == 0 || N == 0) return 0;
+  for (DBuf<u32>* b : {&h.keep, &h.cnt}) b->ensure(ctx, N + 1);
+  for (DBuf<u32>* b : {&h.rowPos, &h.cntPos}) b->ensure(ctx, N + 2);
+  foreach(ctx, N, SnapKeepKernel{h.rowChange.p, succOff.p, h.succChange.p, (u32)k, h.keep.p, h.cnt.p});
+  scan_exclusive(ctx, scanTmp, h.keep.p, h.rowPos.p, N);
+  scan_exclusive(ctx, scanTmp, h.cnt.p, h.cntPos.p, N);
+  u32 Nk = 0, Sk = 0; readU32x2(h.rowPos.p + N, h.cntPos.p + N, &Nk, &Sk);
+  snapDoc.ensure(ctx, (size_t)Nk + 1); snapSuccOff.ensure(ctx, (size_t)Nk + 2); snapSuccCnt.ensure(ctx, (size_t)Nk + 2); snapSucc.ensure(ctx, (size_t)Sk + 1);
+  foreach(ctx, N, SnapGatherKernel{doc.view(), succOff.p, succ.p, h.succChange.p, (u32)k, (u32)N, h.keep.p, h.rowPos.p, h.cntPos.p,
+                                   snapDoc.view(), snapSuccOff.p, snapSucc.p, snapSuccCnt.p});
+  return Nk;
+}
+
+// 5. per prefix length: heads (changes whose first dependent is not in the prefix, sorted by hash), clock and maxOp
+inline void Engine::snapHeader(HistoryPatchCall& h, size_t k, PatchOut& out) {
+  const size_t A = h.A;
+  out.pendingChanges = 0; out.actors = st.actorIds; out.maxOp = 0; out.clock.clear(); out.deps.clear();
+  if (k == 0) return;
+  h.headFlag.ensure(ctx, k + 1); h.headPos.ensure(ctx, k + 2); h.headIdx.ensure(ctx, k + 1); h.clock.ensure(ctx, A + 2);
+  dev_memset(ctx, h.clock.p, 0, (A + 1) * 8);   // [A]: maxOp
+  foreach(ctx, k, SnapHeaderKernel{h.cActor.p, h.cSeq.p, h.cMaxOp.p, h.firstDep.p, (u32)k, (u32)A, h.headFlag.p,
+                                   reinterpret_cast<unsigned long long*>(h.clock.p), reinterpret_cast<unsigned long long*>(h.clock.p + A)});
+  scan_exclusive(ctx, scanTmp, h.headFlag.p, h.headPos.p, k);
+  foreach(ctx, k, CompactKernel{h.headFlag.p, h.headPos.p, h.headIdx.p});
+  const u32 nh = readU32(h.headPos.p + k);
+  h.headHashes.ensure(ctx, (size_t)nh * 32 + 32);
+  foreach(ctx, nh, SyncHashGatherKernel{hashes.p, h.headIdx.p, h.headHashes.p});
+  std::vector<u64> clock(A + 1); std::vector<std::array<u8, 32>> heads(nh);
+  d2h(ctx, clock.data(), h.clock.p, (A + 1) * 8);
+  if (nh) d2h(ctx, heads.data(), h.headHashes.p, (size_t)nh * 32);
+  sync(ctx);
+  std::sort(heads.begin(), heads.end());
+  out.maxOp = clock[A]; out.deps = std::move(heads);
+  for (size_t a = 0; a < A; a++) if (clock[a] > 0) out.clock.emplace_back((u32)a, clock[a]);
 }
 
 }  // namespace amg

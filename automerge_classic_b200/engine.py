@@ -92,6 +92,10 @@ class Library:
         L.amg_encode_changes.argtypes = [vp, vp, C.c_size_t, vp, vp, vp, vp]
         L.amg_last_encode_ms.restype = C.c_float
         L.amg_last_encode_ms.argtypes = [vp]
+        L.amg_get_history_patches.restype = C.c_int
+        L.amg_get_history_patches.argtypes = [vp, vp, C.c_size_t, vp, vp]
+        L.amg_last_history_ms.restype = C.c_float
+        L.amg_last_history_ms.argtypes = [vp]
 
     def check(self, rc, err):
         if rc != 0:
@@ -710,6 +714,24 @@ class GpuBackendDoc:
     def last_encode_ms(self):
         """Device span of the last encode_flat call (CUDA events), ms."""
         return float(self._lib.L.amg_last_encode_ms(self.h))
+
+    # ---- getHistory snapshots (src/automerge.js:105-118), on the device
+    def history_patches_flat(self, lengths):
+        """amg_get_history_patches: for every k in `lengths`, the FlatPatch of getPatch(loadChanges(init(), getAllChanges()[:k]))
+        (k = 0 .. number of applied changes; repeats and any order allowed), filtered from the document's op table in one
+        device call. The document is not touched."""
+        lens = np.ascontiguousarray([int(k) for k in lengths], dtype=np.uint64)
+        bl, err = C.c_void_p(), _ErrStruct()
+        self._lib.check(self._lib.L.amg_get_history_patches(self.h, lens.ctypes.data_as(C.c_void_p), C.c_size_t(len(lens)), C.byref(bl), C.byref(err)), err)
+        return [FlatPatch(raw) for raw in self._buffers(bl)]
+
+    def history_patches(self, lengths):
+        """history_patches_flat as patch dicts (what getPatch returns)."""
+        return [fp.to_patch(True) for fp in self.history_patches_flat(lengths)]
+
+    def last_history_ms(self):
+        """Device span of the last history_patches_flat call (CUDA events), ms."""
+        return float(self._lib.L.amg_last_history_ms(self.h))
 
     def dump_ops(self):
         rows, n, succ, m, err = C.c_void_p(), C.c_size_t(), C.c_void_p(), C.c_size_t(), _ErrStruct()

@@ -137,6 +137,20 @@ int amg_encode_changes(amg_backend* b, const uint8_t* table, size_t table_len, a
 /* device span of the last amg_encode_changes call in ms (CUDA events on the engine's main stream, like amg_last_decode_ms) */
 float amg_last_encode_ms(amg_backend* b);
 
+/* src/automerge.js:105-118 getHistory: the `snapshot` of history entry k - 1 is built from the first k changes of
+ * getAllChanges order (application order; for a loaded document its stored changes first): Frontend.applyPatch(init(),
+ * backend.getPatch(backend.loadChanges(backend.init(), history.slice(0, k)))). This returns that getPatch for every
+ * k = prefix_lens[i]: n self-contained flat patches in the amg_patch_bytes layout, one buffer per length in the order given
+ * (lengths may repeat and need not be sorted). Such a prefix is causally closed, so each patch is computed from the
+ * document's own op table, filtered to the ops of the prefix's changes, without re-sending any change: pendingChanges is 0,
+ * deps are the prefix's heads, clock and maxOp its own; the actor table is the document's (its clock lists only the
+ * prefix's actors). k = 0 gives the patch of getPatch(init()). Queued changes are never part of a prefix. A length greater
+ * than the number of applied changes is AMG_RANGE_ERROR. A loaded document's history is rebuilt first, as amg_get_changes
+ * does (AMG_UNSUPPORTED for a loaded document that holds columns with unknown ids). The document is not touched. */
+int amg_get_history_patches(amg_backend* b, const uint64_t* prefix_lens, size_t n, amg_buffers** out, amg_error* err);
+/* device span of the last amg_get_history_patches call in ms (CUDA events on the engine's main stream, like amg_last_decode_ms) */
+float amg_last_history_ms(amg_backend* b);
+
 /* returned buffer lists */
 size_t amg_buffers_count(const amg_buffers* l);
 const uint8_t* amg_buffers_get(const amg_buffers* l, size_t i, size_t* len);

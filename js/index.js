@@ -79,9 +79,14 @@ function getChanges(backend, haveDeps) {                           // backend.js
 function getChangesAdded(backend1, backend2) { return native.getChangesAdded(backendState(backend1), backendState(backend2)) }   // backend.js:166-168
 function getChangeByHash(backend, hash) { return native.getChangeByHash(backendState(backend), fromHex([hash])) }               // backend.js:176-178
 function getMissingDeps(backend, heads = []) { return native.getMissingDeps(backendState(backend), fromHex(heads)).map(toHex) } // backend.js:190-192
+// getHistory's snapshots (src/automerge.js:105-118): for every k, the patch getPatch(loadChanges(init(), getAllChanges(backend).slice(0, k)))
+// returns, filtered on the device from the document's op table; no change is re-sent
+function historyPatches(backend, prefixLengths) {
+  return native.historyPatches(backendState(backend), prefixLengths).map(flat => inflatePatch(flat, true))
+}
 
 const backendApi = { init, clone, free, applyChanges, applyLocalChange, save, load, loadChanges, getPatch,
-  getHeads, getAllChanges, getChanges, getChangesAdded, getChangeByHash, getMissingDeps }
+  getHeads, getAllChanges, getChanges, getChangesAdded, getChangeByHash, getMissingDeps, historyPatches }
 
 // backend/sync.js:19 hard-imports './backend': the sync functions of backend/index.js are re-created over this backend by
 // loading the reference's sync.js with its backend import redirected (it only calls getHeads / getChanges /
