@@ -265,6 +265,18 @@ napi_value HistoryPatches(napi_env env, napi_callback_info info) {
   if (amg_get_history_patches(b, lens.data(), n, &l, &err)) return throwAmg(env, err);
   return buffersToJs(env, l);
 }
+// merge(state, other) — src/automerge.js:61-67 at the backend level: applies the changes of `other` that `state` lacks,
+// copied device to device (amg_merge); returns the flat patch applyChanges returns. Documents on different devices throw an
+// Error with code 'AMG_UNSUPPORTED' and change nothing (js/index.js then applies getChangesAdded itself).
+napi_value Merge(napi_env env, napi_callback_info info) {
+  napi_value argv[2]; amg_backend *dst, *src; if (!getArgs(env, info, 2, argv) || !getBackend(env, argv[0], &dst) || !getBackend(env, argv[1], &src)) return nullptr;
+  amg_patch* patch = nullptr; amg_error err;
+  if (amg_merge(dst, src, 1, &patch, &err)) {
+    if (err.code == AMG_UNSUPPORTED) { napi_throw_error(env, "AMG_UNSUPPORTED", err.msg); return nullptr; }
+    return throwAmg(env, err);
+  }
+  return patchToJs(env, patch);
+}
 // Backend.free — backend/backend.js:16-19: releases the device memory now instead of at garbage collection
 napi_value Free(napi_env env, napi_callback_info info) {
   napi_value argv[1]; Holder* h; if (!getArgs(env, info, 1, argv) || !getHolder(env, argv[0], &h)) return nullptr;
@@ -278,7 +290,7 @@ napi_value InitModule(napi_env env, napi_value exports) {
     {"getHeads", GetHeads}, {"getChanges", GetChanges}, {"getChangesAdded", GetChangesAdded}, {"getChangeByHash", GetChangeByHash},
     {"getMissingDeps", GetMissingDeps}, {"clockOf", ClockOf}, {"hashByActor", HashByActor}, {"syncBloom", SyncBloom},
     {"syncChangesToSend", SyncChangesToSend}, {"decodeChanges", DecodeChanges}, {"decodeHistory", DecodeHistory},
-    {"encodeChanges", EncodeChanges}, {"historyPatches", HistoryPatches}};
+    {"encodeChanges", EncodeChanges}, {"historyPatches", HistoryPatches}, {"merge", Merge}};
   for (auto& f : fns) { napi_value fn; napi_create_function(env, f.name, NAPI_AUTO_LENGTH, f.fn, nullptr, &fn); napi_set_named_property(env, exports, f.name, fn); }
   return exports;
 }

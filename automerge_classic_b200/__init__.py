@@ -75,6 +75,25 @@ def getHistory(backend):
     return [HistoryEntry(history, i) for i in range(n)]
 
 
+def merge(local, remote):
+    """Automerge.merge (src/automerge.js:61-67) at the backend level: [newLocalHandle, patch], where the patch is the one
+    applyChanges(local, getChangesAdded(local, remote)) returns. The changes go from remote's device memory to local's
+    without leaving the device. The local handle is frozen, as applyChanges freezes it; remote is not changed. When the
+    document class has no device merge, or the engine declines (Unsupported, e.g. documents on different devices), the
+    changes take the host route."""
+    state, other = _backend_state(local), _backend_state(remote)
+    patch = None
+    if hasattr(state, 'merge'):
+        try:
+            patch = state.merge(other)
+        except Unsupported:
+            pass   # nothing changed: the host route below
+    if patch is None:
+        patch = state.apply_changes(other.get_changes_added(state))
+    local['frozen'] = True
+    return [{'state': state, 'heads': state.heads()}, patch]
+
+
 Backend = bind_sync(_Facade(GpuBackendDoc))
 __all__ = ['Backend', 'GpuBackendDoc', 'AmgError', 'Unsupported', 'bind_sync', 'decodeChange', 'decodeChanges', 'encodeChange', 'encodeChanges',
-           'getHistory', 'HistoryEntry']
+           'getHistory', 'HistoryEntry', 'merge']

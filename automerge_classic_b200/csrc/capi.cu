@@ -1,5 +1,5 @@
 // amgpu — extern "C" surface (include/amgpu.h) over amg::Engine, plus the host-side hash graph
-// (reference backend/new.js:1921-2028: getChanges / getChangesAdded / getChangeByHash / getMissingDeps).
+// (reference backend/new.js:1921-2028: getChanges / getChangeByHash / getMissingDeps; getChangesAdded runs on the device).
 #include <unordered_map>
 #include "../../include/amgpu.h"
 #include "engine_impl.cuh"
@@ -63,8 +63,7 @@ struct amg_backend {
     if (const HostChange* o = eng.originalOf(idx)) return std::string((const char*)eng.hostArena.data() + o->off, o->len);
     const HostChange& c = eng.changes[idx];
     std::string plain((const char*)eng.hostArena.data() + c.off, c.len);
-    if (idx < eng.loaded.historyRebuilt && plain.size() >= 256) return deflateChange(plain);   // what encodeChange returns for a rebuilt change (columnar.js:738)
-    return plain;
+    return eng.exportsDeflated(idx) ? deflateChange(plain) : plain;
   }
   // new.js:1921-1973 getChanges(haveDeps): the indexes of the changes it returns, in its order. n == 0: every applied change
   // (the host graph is not needed for that; the caller makes sure the hashes are known).
@@ -142,7 +141,7 @@ amg_backend* amg_clone(amg_backend* src, amg_error* err) {
     d.numApplied = s.numApplied; d.hashes.ensure(c, s.numApplied * 32 + 64); d2d(c, d.hashes.p, s.hashes.p, s.numApplied * 32);
     d.numRows = s.numRows; d.doc.copyFrom(c, s.doc, s.numRows);
     d.numSucc = s.numSucc; d.succOff.ensure(c, s.numRows + 2); d2d(c, d.succOff.p, s.succOff.p, (s.numRows + 1) * 4); d.succ.ensure(c, s.numSucc + 1); d2d(c, d.succ.p, s.succ.p, s.numSucc * 8);
-    d.st = s.st; d.changes = s.changes; d.deflatedOriginal = s.deflatedOriginal; d.loaded = s.loaded;
+    d.st = s.st; d.changes = s.changes; d.deflatedOriginal = s.deflatedOriginal; d.deflateOnExport = s.deflateOnExport; d.loaded = s.loaded;
     d.unknownCols = s.unknownCols; d.queue = s.queue; d.queueOriginal = s.queueOriginal;
     while (d.actorCap < 2 * (d.st.actorIds.size() + 16)) d.actorCap *= 2;
     d.actorSlots.ensure(c, d.actorCap); d.rebuildActorTable();
@@ -289,18 +288,20 @@ int amg_get_history_patches(amg_backend* b, const uint64_t* prefix_lens, size_t 
     *out = guard.release(); return 0;)
 }
 float amg_last_history_ms(amg_backend* b) { return b->eng.lastHistoryMs; }
-// new.js:1979-1997
+// new.js:1979-1997: the changes in their order from Engine::changesAddedFrom (no host hash graph is built)
 int amg_get_changes_added(amg_backend* bn, amg_backend* bo, amg_buffers** out, amg_error* err) {
   AMG_GUARD(
-    bn->ensureGraph(); bo->ensureGraph(); HostGraph& g = bn->g; auto* l = new amg_buffers();
-    std::vector<Hash> stack = bn->eng.st.heads, toReturn; std::unordered_map<Hash, bool, HashHasher> seen;
-    while (!stack.empty()) {
-      Hash h = stack.back(); stack.pop_back();
-      if (!seen.count(h) && !bo->g.indexByHash.count(h)) { seen[h] = true; toReturn.push_back(h); auto& ds = g.deps[g.indexByHash[h]]; stack.insert(stack.end(), ds.begin(), ds.end()); }
-    }
-    for (auto it = toReturn.rbegin(); it != toReturn.rend(); ++it) l->items.push_back(bn->changeBytes(g.indexByHash[*it]));
-    *out = l; return 0;)
+    std::vector<u32> idx; bo->eng.changesAddedFrom(bn->eng, idx);
+    auto* l = new amg_buffers(); std::unique_ptr<amg_buffers> guard(l);
+    for (u32 i : idx) l->items.push_back(bn->changeBytes(i));
+    *out = guard.release(); return 0;)
 }
+// src/automerge.js:61-67 merge(local, remote): applyChanges(local, getChangesAdded(local, remote)), the bytes device to device
+int amg_merge(amg_backend* dst, amg_backend* src, int want_patch, amg_patch** out, amg_error* err) {
+  AMG_GUARD(PatchOut p; dst->eng.mergeFrom(src->eng, want_patch != 0, p);
+            if (out) *out = want_patch ? serialize(p) : nullptr; return 0;)
+}
+float amg_last_merge_ms(amg_backend* b) { return b->eng.lastMergeMs; }
 int amg_get_change_by_hash(amg_backend* b, const uint8_t hash[32], amg_buffers** out, amg_error* err) {
   AMG_GUARD(b->ensureGraph(); auto* l = new amg_buffers(); auto it = b->g.indexByHash.find(toHash(hash));
             if (it != b->g.indexByHash.end()) l->items.push_back(b->changeBytes(it->second)); *out = l; return 0;)

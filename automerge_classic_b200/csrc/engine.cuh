@@ -31,6 +31,7 @@
 #include "changes.cuh"
 #include "encchg.cuh"
 #include "snapshot.cuh"
+#include "merge.cuh"
 #include "unknowncols.hpp"
 
 namespace amg {
@@ -166,6 +167,14 @@ class Engine {
     return it != deflatedOriginal.end() && it->idx == idx ? &it->range : nullptr;
   }
   std::vector<HostChange> queue, queueOriginal;   // not yet causally ready (+ original range, len 0 = not deflated)
+  std::vector<u32> deflateOnExport;   // ascending applied indexes of changes a merge applied in plain form where getChangesAdded hands them over DEFLATEd
+  // getChanges & co hand change idx out DEFLATEd, as encodeChange returns a change of 256 bytes or more (columnar.js:738):
+  // a change rebuilt by computeHashGraph, or one a merge applied in plain form. A change that arrived DEFLATEd goes out as
+  // its original bytes instead (originalOf).
+  bool exportsDeflated(u32 idx) const {
+    if (changes[idx].len < 256 || originalOf(idx)) return false;
+    return idx < loaded.historyRebuilt || std::binary_search(deflateOnExport.begin(), deflateOnExport.end(), idx);
+  }
   Trace trace{ctx};
   HBuf<u8> patchBuf;   // pinned: patch records are copied device -> host directly into their final place
   // ---- scratch (grow-only)
@@ -329,6 +338,9 @@ class Engine {
   // What one call's phases hand to each other (engine_impl.cuh). Device scratch stays in the engine: grow-only, reused.
   struct ApplyCall {
     const u8* const* bufs; const size_t* lens; size_t n; const u8* blob; const u64* offsets; bool isLocal, wantPatch;   // pointer array or packed blob
+    // merge: per new entry, 1 = goes out DEFLATEd once applied (Engine::deflateOnExport). A merge batch is causally complete
+    // over the document (every dependency is applied or in the batch), so no marked entry is left waiting in the queue.
+    const u8* exportMarks = nullptr;
     enum { SRC_PINNED, SRC_DEVICE, SRC_PAGEABLE } srcKind = SRC_PAGEABLE; bool offsetsByDma = false, copiesFirst = false;
     size_t total = 0, arenaLen0 = 0, cur = 0, Bq = 0, B = 0;   // batch: n new changes, then Bq queued ones; bytes arena[arenaLen0, cur)
     struct Piece { size_t byteEnd, changeEnd, mark; }; std::vector<Piece> pieces;
@@ -346,7 +358,8 @@ class Engine {
     void needBatch() { if (fill.joinable()) fill.join(); }
     ~ApplyCall() { needBatch(); }
   };
-  void applyChanges(const u8* const* bufs, const size_t* lens, size_t n, const u8* blob, const u64* offsets, bool isLocal, bool wantPatch, PatchOut& out);
+  void applyChanges(const u8* const* bufs, const size_t* lens, size_t n, const u8* blob, const u64* offsets, bool isLocal, bool wantPatch, PatchOut& out,
+                    const u8* exportMarks = nullptr);
   void applyChangesOnce(ApplyCall& a, PatchOut& out);   // the phases, in order:
   void stageBatch(ApplyCall& a), inflateBatch(ApplyCall& a), runGate(ApplyCall& a), internActors(ApplyCall& a), checkSequence(ApplyCall& a), finalizeOps(ApplyCall& a),
        orderOpSet(ApplyCall& a), computeHeads(ApplyCall& a), commit(ApplyCall& a);
@@ -497,6 +510,16 @@ class Engine {
   void snapHeader(HistoryPatchCall& h, size_t k, PatchOut& out);
   float lastHistoryMs = 0;   // device span of the last historyPatches call (CUDA events; 0 in the emulation build)
   DocBufs snapDoc; DBuf<u32> snapSuccOff, snapSuccCnt; DBuf<u64> snapSucc;   // the prefix document (grow-only; never the document's own)
+
+  // ---------------------------------------------------------------- merge (merge.cuh)
+  // The applied changes of `src` this document lacks, as indexes into src.changes, in the order getChangesAdded returns
+  // them (new.js:1979-1997). Runs on this engine's stream and scratch; src is only read (its history is rebuilt first when
+  // it was loaded, as getChangesAdded does). Both documents must be on the same device (AMG_ERR_UNSUPPORTED otherwise).
+  void changesAddedFrom(Engine& src, std::vector<u32>& order);
+  // Automerge.merge (src/automerge.js:61-67): those changes, gathered from src's arena into one device blob, through applyChanges
+  void mergeFrom(Engine& src, bool wantPatch, PatchOut& out);
+  float lastMergeMs = 0;   // device span of the last mergeFrom call (CUDA events; 0 in the emulation build)
+  DBuf<u32> mergeAbsent, mergeSlot, mergeList, mergeHeadIdx; DBuf<u8> mergeHeads, mergeBlob; DBuf<MergeRange> mergeRanges;
  private:
   void uploadCandidates(const u32* idx, size_t count);
   void syncTimer(bool start);

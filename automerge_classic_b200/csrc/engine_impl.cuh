@@ -71,7 +71,7 @@ inline void Engine::finishPatch(PatchOut& out) {
 inline void Engine::reset() {
   sync(ctx); loaded = LoadedDoc(); unknownCols.clear();
   arenaLen = 0; hostArena.len = 0; numApplied = 0; numRows = 0; numSucc = 0; dev_memset(ctx, succOff.p, 0, 4);
-  st = DocState(); changes.clear(); deflatedOriginal.clear();
+  st = DocState(); changes.clear(); deflatedOriginal.clear(); deflateOnExport.clear();
   queue.clear(); queueOriginal.clear(); rebuildActorTable();
 }
 
@@ -79,8 +79,9 @@ inline void Engine::reset() {
 // (new.js:1833-1840) the first attempt goes without them; if a change then stays unapplied (or looks out of sequence)
 // because it refers to history, the hash graph is computed and the call starts over. Nothing was committed by then.
 struct NeedHistory {};
-inline void Engine::applyChanges(const u8* const* bufs, const size_t* lens, size_t n, const u8* blob, const u64* offsets, bool isLocal, bool wantPatch, PatchOut& out) {
-  auto once = [&]() { ApplyCall a{bufs, lens, n, blob, offsets, isLocal, wantPatch}; applyChangesOnce(a, out); };
+inline void Engine::applyChanges(const u8* const* bufs, const size_t* lens, size_t n, const u8* blob, const u64* offsets, bool isLocal, bool wantPatch, PatchOut& out,
+                                 const u8* exportMarks) {
+  auto once = [&]() { ApplyCall a{bufs, lens, n, blob, offsets, isLocal, wantPatch, exportMarks}; applyChangesOnce(a, out); };
   try { once(); return; }
   catch (NeedHistory&) {}
   catch (Error& e) { if (loaded.haveHashGraph || e.code != AMG_ERR_RANGE) throw; }
@@ -546,8 +547,10 @@ inline void Engine::finalizeOps(ApplyCall& a) {
       // bulk changes (thousands of ops in one change): their columns are expanded in parallel by the token / record
       // decoders of doccols.cuh, column by column; whatever those decline (non-canonical streams, columns that do not hold
       // exactly the op count) and all other large changes go through DecodeColumnKernel (one thread per column)
-      if (lastNumLarge <= 8) decodeHugeChanges(raw, lastNumLarge);
-      foreach(ctx, (size_t)NCOLS * lastNumLarge, DecodeColumnKernel{arena.p, largeList.p, lastNumLarge, hot.p, nOps.p, nPreds.p, rawBase.p, rawPredBase.p, applied.p, raw, errWord.p, hugeDone.p});
+      // (hugeDone is only this batch's when decodeHugeChanges ran: otherwise it holds an earlier batch's flags)
+      const bool huge = lastNumLarge <= 8;
+      if (huge) decodeHugeChanges(raw, lastNumLarge);
+      foreach(ctx, (size_t)NCOLS * lastNumLarge, DecodeColumnKernel{arena.p, largeList.p, lastNumLarge, hot.p, nOps.p, nPreds.p, rawBase.p, rawPredBase.p, applied.p, raw, errWord.p, huge ? hugeDone.p : nullptr});
     }
   }
   const size_t M = a.M;
@@ -723,6 +726,7 @@ inline void Engine::commit(ApplyCall& a) {
       const u32 base0 = (u32)changes.size();
       if (!a.batchOriginal.empty()) for (size_t b = 0; b < B; b++) { const HostChange o = a.originalOf(b); if (o.len) deflatedOriginal.push_back({base0 + (u32)b, o}); }
       else { deflatedOriginal.reserve(deflatedOriginal.size() + a.deflIdx.size()); for (size_t k = 0; k < a.deflIdx.size(); k++) deflatedOriginal.push_back({base0 + a.deflIdx[k], a.inflOrig[k]}); }
+      if (a.exportMarks) for (size_t b = 0; b < a.n; b++) if (a.exportMarks[b]) deflateOnExport.push_back(base0 + (u32)b);
       if (changes.empty()) changes.swap(batchStore); else changes.insert(changes.end(), batchStore.begin(), batchStore.end());
     } else {
       std::vector<u32> byRank(numNew);
@@ -730,6 +734,7 @@ inline void Engine::commit(ApplyCall& a) {
       for (size_t k = 0; k < numNew; k++) {
         const u32 b = byRank[k];
         { const HostChange o = a.originalOf(b); if (o.len) deflatedOriginal.push_back({(u32)changes.size(), o}); }
+        if (a.exportMarks && b < a.n && a.exportMarks[b]) deflateOnExport.push_back((u32)changes.size());   // only the copy that was applied carries its mark
         changes.push_back(batchStore[b]);
       }
     }
@@ -2375,6 +2380,97 @@ inline void Engine::snapHeader(HistoryPatchCall& h, size_t k, PatchOut& out) {
   std::sort(heads.begin(), heads.end());
   out.maxOp = clock[A]; out.deps = std::move(heads);
   for (size_t a = 0; a < A; a++) if (clock[a] > 0) out.clock.emplace_back((u32)a, clock[a]);
+}
+
+// ------------------------------------------------------------ merge (merge.cuh; new.js:1979-1997, src/automerge.js:61-67)
+// Which changes: every applied change of src whose hash this document has not applied, one table lookup each. That is
+// exactly the set the reference's walk from src's heads visits (DESIGN.md section 3): a document applies a change only
+// after its dependencies, so every ancestor of a change this document has is here as well, and every absent change is
+// reached from src's heads through absent changes only. The order is the walk's; it runs on the host over the absent
+// changes' dependency indexes, for the reason syncChangesToSend gives (a device walk needs one launch per level).
+inline void Engine::changesAddedFrom(Engine& src, std::vector<u32>& order) {
+  order.clear();
+  if (!loaded.haveHashGraph) computeHashGraph();   // new.js:1980; the package builds both documents' graphs (DESIGN.md section 5)
+  if (!src.loaded.haveHashGraph) src.computeHashGraph();
+  if (src.ctx.device != ctx.device)
+    throw Error(AMG_ERR_UNSUPPORTED, "amgpu: the documents are on different devices (" + std::to_string(src.ctx.device) + ", " + std::to_string(ctx.device) + ")");
+  sync(src.ctx);   // src's buffers are read on this engine's stream
+  const size_t C = src.numApplied;
+  if (C == 0) return;
+  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+  // 1. presence: this document's hashes in a table, one probe per change of src, then flag -> scan -> compact
+  size_t tcap = pow2_at_least(2 * numApplied + 2);
+  hashTable.ensure(ctx, tcap); dev_memset(ctx, hashTable.p, 0xff, tcap * 4);
+  foreach(ctx, numApplied, HashInsertKernel{hashes.p, hashTable.p, (u64)tcap - 1});
+  mergeAbsent.ensure(ctx, C + 1); mergeSlot.ensure(ctx, C + 2);
+  foreach(ctx, C, MergeProbeKernel{hashes.p, hashTable.p, (u64)tcap - 1, src.hashes.p, mergeAbsent.p});
+  scan_exclusive(ctx, scanTmp, mergeAbsent.p, mergeSlot.p, C);
+  const size_t K = readU32(mergeSlot.p + C);
+  if (K == 0) return;
+  mergeList.ensure(ctx, K + 1);
+  foreach(ctx, C, CompactKernel{mergeAbsent.p, mergeSlot.p, mergeList.p});
+  std::vector<u32> absent(K); d2h(ctx, absent.data(), mergeList.p, K * 4); sync(ctx);
+  // 2. the absent changes' dependencies in header order (the order of dependenciesByHash) and src's heads, as change
+  //    indexes of src: ParseKernel over their headers in src's arena, src's hashes in the table, ResolveDepsKernelT
+  std::vector<HostChange> pairs(K); for (size_t k = 0; k < K; k++) pairs[k] = src.changes[absent[k]];
+  chPairs.ensure(ctx, K); chOff.ensure(ctx, K); chLen.ensure(ctx, K);
+  h2d(ctx, chPairs.p, pairs.data(), K * sizeof(HostChange));
+  foreach(ctx, K, SplitPairsKernel{chPairs.p, chOff.p, chLen.p});
+  meta.ensure(ctx, K); colOff.ensure(ctx, (size_t)NCOLS * K); colLen.ensure(ctx, (size_t)NCOLS * K);
+  nOps.ensure(ctx, K + 1); nPreds.ensure(ctx, K + 1); nDeps.ensure(ctx, K + 1); nActors.ensure(ctx, K + 1);
+  foreach(ctx, K, ParseKernel{src.arena.p, chOff.p, chLen.p, K, meta.p, colOff.p, colLen.p, nOps.p, nPreds.p, nDeps.p, nActors.p, errWord.p, flagWord.p + 8});
+  depBase.ensure(ctx, K + 1); scan_exclusive(ctx, scanTmp, nDeps.p, depBase.p, K);
+  const u32 D = readU32(depBase.p + K);
+  checkErr();
+  depIdx.ensure(ctx, (size_t)D + 1); primary.ensure(ctx, K);
+  tcap = pow2_at_least(2 * C + 2);
+  hashTable.ensure(ctx, tcap); dev_memset(ctx, hashTable.p, 0xff, tcap * 4);
+  foreach(ctx, C, HashInsertKernel{src.hashes.p, hashTable.p, (u64)tcap - 1});
+  // numApplied = 0: primary[b] looks up change b of src, which exists (b < K <= C); only depIdx is used here
+  foreach(ctx, K, ResolveDepsKernelT<ChangeMeta>{src.arena.p, src.hashes.p, hashTable.p, (u64)tcap - 1, meta.p, nDeps.p, 0, depBase.p, depIdx.p, primary.p});
+  const size_t H = src.st.heads.size();
+  mergeHeads.ensure(ctx, H * 32 + 32); mergeHeadIdx.ensure(ctx, H + 1);
+  std::vector<u8> headBytes(H * 32); for (size_t i = 0; i < H; i++) memcpy(headBytes.data() + 32 * i, src.st.heads[i].data(), 32);
+  h2d(ctx, mergeHeads.p, headBytes.data(), H * 32);
+  foreach(ctx, H, HashLookupKernel{src.hashes.p, hashTable.p, (u64)tcap - 1, mergeHeads.p, mergeHeadIdx.p});
+  std::vector<u32> base(K + 1), deps(D), stack(H);
+  d2h(ctx, base.data(), depBase.p, (K + 1) * 4); d2h(ctx, deps.data(), depIdx.p, (size_t)D * 4); d2h(ctx, stack.data(), mergeHeadIdx.p, H * 4); sync(ctx);
+  // 3. new.js:1983-1994: heads in order, popped from the back; the seen test at pop time; dependencies pushed in header
+  //    order; a change this document has stops the walk. Then reversed (:1996).
+  std::vector<u32> posOf(C, EMPTY32); for (size_t k = 0; k < K; k++) posOf[absent[k]] = (u32)k;
+  std::vector<u8> seen(K, 0);
+  while (!stack.empty()) {
+    const u32 c = stack.back(); stack.pop_back();
+    const u32 k = c < C ? posOf[c] : EMPTY32;
+    if (k == EMPTY32 || seen[k]) continue;
+    seen[k] = 1; order.push_back(c);
+    stack.insert(stack.end(), deps.begin() + base[k], deps.begin() + base[k + 1]);
+  }
+  std::reverse(order.begin(), order.end());
+}
+
+// The changes to send are the bytes getChangesAdded returns (amg_backend::changeBytes): a change's DEFLATEd original when
+// it has one, else its plain bytes. A change getChangesAdded would DEFLATE on the way out (exportsDeflated) goes over
+// plain and marked instead, so that this document hands it out DEFLATEd later, as if it had received it that way.
+inline void Engine::mergeFrom(Engine& src, bool wantPatch, PatchOut& out) {
+  lastMergeMs = 0;
+  const float keepSyncMs = lastSyncMs; lastSyncMs = 0;
+  struct Restore { Engine& e; float ms; ~Restore() { e.lastSyncMs = ms; } } restore{*this, keepSyncMs};   // the timer is shared with the sync calls
+  syncTimer(true);
+  std::vector<u32> idx; changesAddedFrom(src, idx);
+  const size_t K = idx.size();
+  std::vector<u64> offs(K + 1, 0); std::vector<MergeRange> ranges(K); std::vector<u8> marks(K + 1, 0);
+  for (size_t k = 0; k < K; k++) {
+    const u32 c = idx[k]; const HostChange* o = src.originalOf(c); const HostChange r = o ? *o : src.changes[c];
+    marks[k] = src.exportsDeflated(c) ? 1 : 0;
+    ranges[k] = MergeRange{offs[k], r.off, r.len}; offs[k + 1] = offs[k] + r.len;
+  }
+  if ((u64)arenaLen + offs[K] + 64 >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: change arena limited to 4 GiB per document");
+  mergeBlob.ensure(ctx, offs[K] + 64); mergeRanges.ensure(ctx, K + 1);
+  h2d(ctx, mergeRanges.p, ranges.data(), K * sizeof(MergeRange));
+  merge_gather(ctx, K, MergeGatherKernel{src.arena.p, mergeBlob.p, mergeRanges.p});
+  applyChanges(nullptr, nullptr, K, mergeBlob.p, offs.data(), false, wantPatch, out, marks.data());   // the device-blob path of amg_apply_changes_packed
+  syncTimer(false); lastMergeMs = lastSyncMs;
 }
 
 }  // namespace amg

@@ -96,6 +96,10 @@ class Library:
         L.amg_get_history_patches.argtypes = [vp, vp, C.c_size_t, vp, vp]
         L.amg_last_history_ms.restype = C.c_float
         L.amg_last_history_ms.argtypes = [vp]
+        L.amg_merge.restype = C.c_int
+        L.amg_merge.argtypes = [vp, vp, C.c_int, vp, vp]
+        L.amg_last_merge_ms.restype = C.c_float
+        L.amg_last_merge_ms.argtypes = [vp]
 
     def check(self, rc, err):
         if rc != 0:
@@ -603,6 +607,23 @@ class GpuBackendDoc:
         bl, err = C.c_void_p(), _ErrStruct()
         self._lib.check(self._lib.L.amg_get_changes_added(self.h, old.h, C.byref(bl), C.byref(err)), err)
         return self._buffers(bl)
+
+    def merge_flat(self, other, want_patch=True):
+        """amg_merge: applies the changes of `other` this document lacks, in getChangesAdded order, copied device to device
+        (src/automerge.js:61-67). Returns the FlatPatch applyChanges would (None with want_patch=False). Raises
+        Unsupported when the documents are on different devices, before anything changed."""
+        pp, err = C.c_void_p(), _ErrStruct()
+        self._lib.check(self._lib.L.amg_merge(self.h, other.h, int(want_patch), C.byref(pp), C.byref(err)), err)
+        return self._take_patch(pp) if want_patch else None
+
+    def merge(self, other, want_patch=True):
+        """merge_flat as the patch dict applyChanges returns."""
+        fp = self.merge_flat(other, want_patch)
+        return fp.to_patch(False) if want_patch else None
+
+    def last_merge_ms(self):
+        """Device span of the last merge_flat call (CUDA events), ms."""
+        return float(self._lib.L.amg_last_merge_ms(self.h))
 
     def get_change_by_hash(self, hash_):
         bl, err = C.c_void_p(), _ErrStruct()

@@ -67,8 +67,28 @@ int amg_save(amg_backend* b, amg_buffers** out, amg_error* err);
 int amg_get_heads(amg_backend* b, amg_buffers** out, amg_error* err);
 /* Backend.getAllChanges / getChanges(haveDeps) — backend.js:142-156 -> new.js:1921-1973; have_deps = n hashes x 32 bytes */
 int amg_get_changes(amg_backend* b, const uint8_t* have_deps, size_t n, amg_buffers** out, amg_error* err);
-/* Backend.getChangesAdded(old, new) — backend.js:166-168 -> new.js:1979-1997 */
+/* Backend.getChangesAdded(old, new) — backend.js:166-168 -> new.js:1979-1997. The changes of b_new that b_old lacks are
+ * found by hash lookups on the device and ordered on the host over their dependency indexes; no host hash graph is built.
+ * A loaded document's history is rebuilt first (both documents). The two documents must be on the same CUDA device
+ * (AMG_UNSUPPORTED otherwise). */
 int amg_get_changes_added(amg_backend* b_new, amg_backend* b_old, amg_buffers** out, amg_error* err);
+/* Automerge.merge(localDoc, remoteDoc) — src/automerge.js:61-67, at the backend level: applyChanges(dst, getChangesAdded(dst,
+ * src)) (backend.js:27-32, 166-168) without the changes leaving the device. The changes of src that dst lacks, in
+ * getChangesAdded's order, are copied from src's arena into one device buffer and applied to dst through the device-memory
+ * path of amg_apply_changes_packed; *out is the patch that applyChanges returns (want_patch == 0: none, *out = NULL).
+ *   - No changes to send (src == dst, src a clone of dst, src's changes a subset of dst's): dst applies an empty batch and
+ *     *out is the patch applyChanges(dst, []) returns (queued changes of dst are retried, as always).
+ *   - src's queued changes are never sent; dst's queued changes may become applicable.
+ *   - src is not changed (a loaded src has its history rebuilt first, as getChangesAdded does; so has a loaded dst).
+ *   - A change getChangesAdded would hand over DEFLATEd because the engine rebuilt it (>= 256 bytes) goes over in plain
+ *     form; dst returns it DEFLATEd from getChanges, getChangeByHash, getChangesAdded and sync, as it would after the host
+ *     route. Only amg_arena shows the plain bytes.
+ *   - dst and src on different CUDA devices: AMG_UNSUPPORTED, nothing changed (amg_get_changes_added declines them too).
+ *   - An apply error (e.g. both documents hold a different change for the same actor and seq) is the error applyChanges
+ *     reports for the same changes, and dst is unchanged. */
+int amg_merge(amg_backend* dst, amg_backend* src, int want_patch, amg_patch** out, amg_error* err);
+/* device span of the last amg_merge call in ms, lookups, copy and apply (CUDA events on dst's main stream, like amg_last_history_ms) */
+float amg_last_merge_ms(amg_backend* dst);
 /* Backend.getChangeByHash — backend.js:176-178 -> new.js:1999-2002; zero buffers when unknown */
 int amg_get_change_by_hash(amg_backend* b, const uint8_t hash[32], amg_buffers** out, amg_error* err);
 /* Backend.getMissingDeps — backend.js:190-192 -> new.js:2014-2028: hashes of 32 bytes */

@@ -85,8 +85,23 @@ function historyPatches(backend, prefixLengths) {
   return native.historyPatches(backendState(backend), prefixLengths).map(flat => inflatePatch(flat, true))
 }
 
+// Automerge.merge (src/automerge.js:61-67) at the backend level: applyChanges(backend1, getChangesAdded(backend1, backend2)),
+// with the changes copied from backend2's device memory to backend1's. backend1 is frozen, as applyChanges freezes it.
+// Documents on different devices take the same route through JavaScript.
+function merge(backend1, backend2) {
+  const state = backendState(backend1), other = backendState(backend2)
+  let flat
+  try { flat = native.merge(state, other) } catch (e) {
+    if (e.code !== 'AMG_UNSUPPORTED') throw e
+    return applyChanges(backend1, getChangesAdded(backend1, backend2))
+  }
+  const patch = inflatePatch(flat, false)
+  backend1.frozen = true
+  return [{state, heads: patch.deps}, patch]
+}
+
 const backendApi = { init, clone, free, applyChanges, applyLocalChange, save, load, loadChanges, getPatch,
-  getHeads, getAllChanges, getChanges, getChangesAdded, getChangeByHash, getMissingDeps, historyPatches }
+  getHeads, getAllChanges, getChanges, getChangesAdded, getChangeByHash, getMissingDeps, historyPatches, merge }
 
 // backend/sync.js:19 hard-imports './backend': the sync functions of backend/index.js are re-created over this backend by
 // loading the reference's sync.js with its backend import redirected (it only calls getHeads / getChanges /
