@@ -15,6 +15,17 @@ struct HashHasher { size_t operator()(const Hash& h) const { size_t v; memcpy(&v
 Hash toHash(const u8* p) { Hash h; memcpy(h.data(), p, 32); return h; }
 std::string hashHex(const Hash& h) { return hex_of(h.data(), 32); }
 
+// A change's dependency hashes, actor and seq, read from its header (columnar.js decodeChangeHeader) in the host arena
+struct ChangeHeader { std::vector<Hash> deps; std::string actor; u64 seq; };
+ChangeHeader readHeader(const u8* arena, const HostChange& c) {
+  ByteReader r(arena, c.off + 8, c.off + c.len); r.pos++; r.uleb();
+  ChangeHeader h; h.deps.resize(r.uleb());
+  for (Hash& d : h.deps) { memcpy(d.data(), arena + r.pos, 32); r.skip(32); }
+  const u64 al = r.uleb(); h.actor.assign((const char*)arena + r.pos, al); r.skip(al);
+  h.seq = r.uleb();
+  return h;
+}
+
 // Host hash graph, filled lazily from the applied changes' headers (the reference defers it too: new.js:1887-1912)
 struct HostGraph {
   size_t known = 0;
@@ -30,23 +41,18 @@ struct amg_backend {
 
   void ensureGraph() {
     Engine& e = eng;
-    if (!e.loaded.haveHashGraph) e.computeHashGraph();   // new.js:1922, 1980, 2000, 2015
+    e.computeHashGraph();   // new.js:1922, 1980, 2000, 2015
     if (g.known == e.numApplied) return;
     const size_t from = g.known, to = e.numApplied;
     e.ensureHostMirror();   // the change headers are read from the host copy of the arena (fetched now if the batch came from pinned / device memory)
     std::vector<u8> hs((to - from) * 32); d2h(e.ctx, hs.data(), e.hashes.p + from * 32, hs.size()); sync(e.ctx);
     for (size_t i = from; i < to; i++) {
       Hash h; memcpy(h.data(), hs.data() + (i - from) * 32, 32);
-      const HostChange& c = e.changes[i];
-      ByteReader r(e.hostArena.data(), c.off + 8, c.off + c.len); r.pos++; r.uleb();
-      const u64 nd = r.uleb(); std::vector<Hash> deps(nd);
-      for (u64 k = 0; k < nd; k++) { memcpy(deps[k].data(), e.hostArena.data() + r.pos, 32); r.skip(32); }
-      const u64 al = r.uleb(); std::string actor((const char*)e.hostArena.data() + r.pos, al); r.skip(al);
-      const u64 seq = r.uleb();
-      g.hash.push_back(h); g.actor.push_back(actor); g.seq.push_back(seq); g.deps.push_back(deps);
+      ChangeHeader c = readHeader(e.hostArena.data(), e.changes[i]);
       g.indexByHash[h] = (u32)i; g.dependents[h];
-      for (auto& d : deps) g.dependents[d].push_back(h);
-      auto& v = g.hashesByActor[actor]; if (v.size() < seq) v.resize(seq); v[seq - 1] = h;
+      for (auto& d : c.deps) g.dependents[d].push_back(h);
+      auto& v = g.hashesByActor[c.actor]; if (v.size() < c.seq) v.resize(c.seq); v[c.seq - 1] = h;
+      g.hash.push_back(h); g.actor.push_back(std::move(c.actor)); g.seq.push_back(c.seq); g.deps.push_back(std::move(c.deps));
     }
     g.known = to;
   }
@@ -108,34 +114,47 @@ void setErr(amg_error* err, int code, const std::string& msg) {
   if (!err) return;
   err->code = code; snprintf(err->msg, sizeof(err->msg), "%s", msg.c_str());
 }
-#define AMG_GUARD(...) \
-  try { __VA_ARGS__ } catch (amg::Error& e) { amg::drop_pending_peeks(); setErr(err, e.code, e.what()); return e.code; } \
-  catch (std::exception& e) { amg::drop_pending_peeks(); setErr(err, AMG_INTERNAL_ERROR, e.what()); return AMG_INTERNAL_ERROR; }
+// A failed call: the peeks it left pending are dropped, *err and (for an amg::Error) *failed are set, the code is returned
+int fail(amg_error* err, int code, const char* msg, size_t* failed = nullptr, size_t failedAt = 0) {
+  amg::drop_pending_peeks(); setErr(err, code, msg);
+  if (failed) *failed = failedAt;
+  return code;
+}
+// The body of an extern "C" call returning an error code; AMG_GUARD_FAILED also reports `source` (read after the throw)
+// in *failed when the call fails with an amg::Error
+#define AMG_GUARD_FAILED(failed, source, ...) \
+  try { __VA_ARGS__ } catch (amg::Error& e) { return fail(err, e.code, e.what(), failed, source); } \
+  catch (std::exception& e) { return fail(err, AMG_INTERNAL_ERROR, e.what()); }
+#define AMG_GUARD(...) AMG_GUARD_FAILED(nullptr, 0, __VA_ARGS__)
+
+// amg_init / amg_load / amg_clone: a new backend that `fill` completes, or nullptr with *err set (the backend is freed)
+template <class F> amg_backend* construct(int device, amg_error* err, F fill) {
+  try { std::unique_ptr<amg_backend> b(new amg_backend(device)); fill(*b); return b.release(); }
+  catch (amg::Error& e) { fail(err, e.code, e.what()); }
+  catch (std::exception& e) { fail(err, AMG_INTERNAL_ERROR, e.what()); }
+  return nullptr;
+}
+
+// A list for the caller, filled by `fill`; freed if fill throws
+template <class F> std::unique_ptr<amg_buffers> buffers(F fill) { std::unique_ptr<amg_buffers> l(new amg_buffers()); fill(l->items); return l; }
+typedef std::vector<std::string> Items;
 
 amg_patch* serialize(const PatchOut& p) { return new amg_patch{p.bytes, p.bytesLen}; }
 }  // namespace
 
 extern "C" {
 
-amg_backend* amg_init(int cuda_device, amg_error* err) {
-  try { return new amg_backend(cuda_device); }
-  catch (amg::Error& e) { setErr(err, e.code, e.what()); return nullptr; }
-  catch (std::exception& e) { setErr(err, AMG_INTERNAL_ERROR, e.what()); return nullptr; }
-}
+amg_backend* amg_init(int cuda_device, amg_error* err) { return construct(cuda_device, err, [](amg_backend&) {}); }
 void amg_free(amg_backend* b) { delete b; }
 amg_backend* amg_load(int cuda_device, const uint8_t* data, size_t len, amg_error* err) {
-  amg_backend* b = nullptr;
-  try { b = new amg_backend(cuda_device); b->eng.loadDocument(data, len); return b; }
-  catch (amg::Error& e) { setErr(err, e.code, e.what()); delete b; return nullptr; }
-  catch (std::exception& e) { setErr(err, AMG_INTERNAL_ERROR, e.what()); delete b; return nullptr; }
+  return construct(cuda_device, err, [&](amg_backend& b) { b.eng.loadDocument(data, len); });
 }
 int amg_reset(amg_backend* b, amg_error* err) { AMG_GUARD(b->g = HostGraph(); b->eng.reset(); return 0;) }
 int amg_reserve(amg_backend* b, size_t arena_bytes, amg_error* err) { AMG_GUARD(b->eng.hostArena.reserve(arena_bytes); b->eng.arena.ensure(b->eng.ctx, arena_bytes + 64, b->eng.arenaLen); return 0;) }
 
 amg_backend* amg_clone(amg_backend* src, amg_error* err) {
-  try {
-    auto* b = new amg_backend(src->eng.ctx.device);
-    Engine& d = b->eng; Engine& s = src->eng; Ctx& c = d.ctx;
+  return construct(src->eng.ctx.device, err, [&](amg_backend& b) {
+    Engine& d = b.eng; Engine& s = src->eng; Ctx& c = d.ctx;
     sync(s.ctx); s.ensureHostMirror();
     d.hostArena.assign(s.hostArena); d.arenaLen = s.arenaLen; d.arena.ensure(c, s.arenaLen + 64); d2d(c, d.arena.p, s.arena.p, s.arenaLen);
     d.numApplied = s.numApplied; d.hashes.ensure(c, s.numApplied * 32 + 64); d2d(c, d.hashes.p, s.hashes.p, s.numApplied * 32);
@@ -146,9 +165,7 @@ amg_backend* amg_clone(amg_backend* src, amg_error* err) {
     while (d.actorCap < 2 * (d.st.actorIds.size() + 16)) d.actorCap *= 2;
     d.actorSlots.ensure(c, d.actorCap); d.rebuildActorTable();
     sync(c);
-    return b;
-  } catch (amg::Error& e) { amg::drop_pending_peeks(); setErr(err, e.code, e.what()); return nullptr; }
-  catch (std::exception& e) { amg::drop_pending_peeks(); setErr(err, AMG_INTERNAL_ERROR, e.what()); return nullptr; }
+  });
 }
 
 int amg_apply_changes(amg_backend* b, const uint8_t* const* bufs, const size_t* lens, size_t n, int is_local, int want_patch, amg_patch** out, amg_error* err) {
@@ -178,35 +195,35 @@ void amg_buffers_free(amg_buffers* l) { delete l; }
 void amg_free_mem(void* p) { free(p); }
 
 int amg_get_heads(amg_backend* b, amg_buffers** out, amg_error* err) {
-  AMG_GUARD(auto* l = new amg_buffers(); for (auto& h : b->eng.st.heads) l->items.emplace_back((const char*)h.data(), 32); *out = l; return 0;)
+  AMG_GUARD(*out = buffers([&](Items& l) { for (auto& h : b->eng.st.heads) l.emplace_back((const char*)h.data(), 32); }).release(); return 0;)
 }
 
 // new.js:2033-2055
 int amg_save(amg_backend* b, amg_buffers** out, amg_error* err) {
-  AMG_GUARD(auto* l = new amg_buffers(); std::unique_ptr<amg_buffers> guard(l); l->items.emplace_back(); b->eng.saveDocument(l->items.back()); *out = guard.release(); return 0;)
+  AMG_GUARD(*out = buffers([&](Items& l) { l.emplace_back(); b->eng.saveDocument(l.back()); }).release(); return 0;)
 }
 
 // new.js:1921-1973
 int amg_get_changes(amg_backend* b, const uint8_t* have_deps, size_t n, amg_buffers** out, amg_error* err) {
   AMG_GUARD(
-    b->ensureGraph(); auto* l = new amg_buffers(); std::unique_ptr<amg_buffers> guard(l);
-    for (u32 i : b->changesSince(have_deps, n)) l->items.push_back(b->changeBytes(i));
-    *out = guard.release(); return 0;)
+    b->ensureGraph();
+    *out = buffers([&](Items& l) { for (u32 i : b->changesSince(have_deps, n)) l.push_back(b->changeBytes(i)); }).release(); return 0;)
 }
 // sync.js:234-238 makeBloomFilter: Bloom filter over the hashes of getChanges(last_sync), built on the device
 int amg_sync_bloom(amg_backend* b, const uint8_t* last_sync, size_t n, amg_buffers** out, amg_error* err) {
   AMG_GUARD(
-    Engine& e = b->eng; if (!e.loaded.haveHashGraph) e.computeHashGraph();   // the hashes of a loaded document (new.js:1922)
-    auto* l = new amg_buffers(); std::unique_ptr<amg_buffers> guard(l); l->items.emplace_back();
-    if (n == 0) e.syncBloom(nullptr, e.numApplied, l->items.back());   // every applied change: no host graph needed
-    else { const std::vector<u32> idx = b->changesSince(last_sync, n); e.syncBloom(idx.data(), idx.size(), l->items.back()); }
-    *out = guard.release(); return 0;)
+    Engine& e = b->eng; e.computeHashGraph();   // the hashes of a loaded document (new.js:1922)
+    *out = buffers([&](Items& l) {
+      l.emplace_back();
+      if (n == 0) e.syncBloom(nullptr, e.numApplied, l.back());   // every applied change: no host graph needed
+      else { const std::vector<u32> idx = b->changesSince(last_sync, n); e.syncBloom(idx.data(), idx.size(), l.back()); }
+    }).release(); return 0;)
 }
 // sync.js:246-306 getChangesToSend for a non-empty `have`
 int amg_sync_changes_to_send(amg_backend* b, const uint8_t* last_sync, size_t n_last, const amg_bloom* filters, size_t n_filters,
                              const uint8_t* need, size_t n_need, amg_buffers** out_changes, amg_buffers** out_hashes, amg_error* err) {
   AMG_GUARD(
-    Engine& e = b->eng; if (!e.loaded.haveHashGraph) e.computeHashGraph();
+    Engine& e = b->eng; e.computeHashGraph();
     std::vector<u32> cand; if (n_last > 0) cand = b->changesSince(last_sync, n_last);
     const u32* idx = n_last > 0 ? cand.data() : nullptr; const size_t count = n_last > 0 ? cand.size() : e.numApplied;
     std::vector<Engine::BloomSpec> fs(n_filters);
@@ -226,85 +243,72 @@ int amg_sync_changes_to_send(amg_backend* b, const uint8_t* last_sync, size_t n_
       }
     }
     for (size_t i = 0; i < count; i++) if (send[i]) outIdx.push_back(idx ? idx[i] : (u32)i);
-    auto* lc = new amg_buffers(); std::unique_ptr<amg_buffers> gc(lc); auto* lh = new amg_buffers(); std::unique_ptr<amg_buffers> gh(lh);
-    lh->items.emplace_back(); e.gatherHashes(outIdx, lh->items.back());
-    for (u32 i : outIdx) lc->items.push_back(b->changeBytes(i));
-    *out_changes = gc.release(); *out_hashes = gh.release(); return 0;)
+    auto lh = buffers([&](Items& l) { l.emplace_back(); e.gatherHashes(outIdx, l.back()); });
+    auto lc = buffers([&](Items& l) { for (u32 i : outIdx) l.push_back(b->changeBytes(i)); });
+    *out_changes = lc.release(); *out_hashes = lh.release(); return 0;)
 }
-float amg_last_sync_ms(amg_backend* b) { return b->eng.lastSyncMs; }
+float amg_last_sync_ms(amg_backend* b) { return b->eng.spans.ms[SPAN_SYNC]; }
 // columnar.js:770-776 decodeChange over n change containers, into one change table
 int amg_decode_changes(amg_backend* b, const uint8_t* blob, const uint64_t* offsets, size_t n, amg_buffers** out, size_t* failed_index, amg_error* err) {
   if (failed_index) *failed_index = 0;
-  try {
-    auto* l = new amg_buffers(); std::unique_ptr<amg_buffers> guard(l); l->items.emplace_back();
-    b->eng.decodeChanges(blob, (const u64*)offsets, n, false, l->items.back());
-    *out = guard.release(); return 0;
-  } catch (amg::Error& e) { amg::drop_pending_peeks(); if (failed_index) *failed_index = b->eng.decodeFailed; setErr(err, e.code, e.what()); return e.code; }
-  catch (std::exception& e) { amg::drop_pending_peeks(); setErr(err, AMG_INTERNAL_ERROR, e.what()); return AMG_INTERNAL_ERROR; }
+  AMG_GUARD_FAILED(failed_index, b->eng.decodeFailed,
+    *out = buffers([&](Items& l) { l.emplace_back(); b->eng.decodeChanges(blob, (const u64*)offsets, n, false, l.back()); }).release(); return 0;)
 }
 // the same for every applied change, in getAllChanges order (new.js:1925-1927), read from device memory
 int amg_decode_history(amg_backend* b, amg_buffers** out, amg_error* err) {
   AMG_GUARD(
-    auto* l = new amg_buffers(); std::unique_ptr<amg_buffers> guard(l); l->items.emplace_back();
-    if (!b->eng.loaded.haveHashGraph) b->eng.computeHashGraph();   // (new.js:1922) before the change count is taken
-    b->eng.decodeChanges(nullptr, nullptr, b->eng.changes.size(), true, l->items.back());
-    *out = guard.release(); return 0;)
+    b->eng.computeHashGraph();   // (new.js:1922) before the change count is taken
+    *out = buffers([&](Items& l) { l.emplace_back(); b->eng.decodeChanges(nullptr, nullptr, b->eng.changes.size(), true, l.back()); }).release(); return 0;)
 }
-float amg_last_decode_ms(amg_backend* b) { return b->eng.lastDecodeMs; }
+float amg_last_decode_ms(amg_backend* b) { return b->eng.spans.ms[SPAN_DECODE]; }
 // columnar.js:710-739 encodeChange over the changes of a change table: plain changes from the device, the ones of 256 bytes
 // or more DEFLATEd here (columnar.js:738), over a few host threads when there are many
 int amg_encode_changes(amg_backend* b, const uint8_t* table, size_t table_len, amg_buffers** out_changes, amg_buffers** out_hashes,
                        size_t* failed_index, amg_error* err) {
   if (failed_index) *failed_index = 0;
-  try {
+  AMG_GUARD_FAILED(failed_index, b->eng.encodeFailed,
     std::string bytes, hs; std::vector<u64> offs;
     b->eng.encodeChanges(table, table_len, bytes, offs, hs);
-    auto* lc = new amg_buffers(); std::unique_ptr<amg_buffers> gc(lc); auto* lh = new amg_buffers(); std::unique_ptr<amg_buffers> gh(lh);
-    const size_t n = offs.size() - 1; lc->items.resize(n);
-    auto fill = [&](size_t from, size_t to) {
-      for (size_t i = from; i < to; i++) {
-        const u64 len = offs[i + 1] - offs[i];
-        if (len >= 256) lc->items[i] = amg_backend::deflateChange(std::string(bytes, offs[i], len)); else lc->items[i].assign(bytes, offs[i], len);
+    auto lc = buffers([&](Items& l) {
+      const size_t n = offs.size() - 1; l.resize(n);
+      auto fill = [&](size_t from, size_t to) {
+        for (size_t i = from; i < to; i++) {
+          const u64 len = offs[i + 1] - offs[i];
+          if (len >= 256) l[i] = amg_backend::deflateChange(std::string(bytes, offs[i], len)); else l[i].assign(bytes, offs[i], len);
+        }
+      };
+      const size_t nThreads = std::min<size_t>(std::max(1u, std::thread::hardware_concurrency()), std::min<size_t>(16, n / 4096 + 1));
+      if (nThreads <= 1) fill(0, n);
+      else {
+        std::vector<std::thread> th; const size_t per = (n + nThreads - 1) / nThreads;
+        for (size_t t = 0; t < nThreads; t++) th.emplace_back(fill, std::min(n, t * per), std::min(n, (t + 1) * per));
+        for (auto& x : th) x.join();
       }
-    };
-    const size_t nThreads = std::min<size_t>(std::max(1u, std::thread::hardware_concurrency()), std::min<size_t>(16, n / 4096 + 1));
-    if (nThreads <= 1) fill(0, n);
-    else {
-      std::vector<std::thread> th; const size_t per = (n + nThreads - 1) / nThreads;
-      for (size_t t = 0; t < nThreads; t++) th.emplace_back(fill, std::min(n, t * per), std::min(n, (t + 1) * per));
-      for (auto& x : th) x.join();
-    }
-    lh->items.push_back(std::move(hs));
-    *out_changes = gc.release(); *out_hashes = gh.release(); return 0;
-  } catch (amg::Error& e) { amg::drop_pending_peeks(); if (failed_index) *failed_index = b->eng.encodeFailed; setErr(err, e.code, e.what()); return e.code; }
-  catch (std::exception& e) { amg::drop_pending_peeks(); setErr(err, AMG_INTERNAL_ERROR, e.what()); return AMG_INTERNAL_ERROR; }
+    });
+    auto lh = buffers([&](Items& l) { l.push_back(std::move(hs)); });
+    *out_changes = lc.release(); *out_hashes = lh.release(); return 0;)
 }
-float amg_last_encode_ms(amg_backend* b) { return b->eng.lastEncodeMs; }
+float amg_last_encode_ms(amg_backend* b) { return b->eng.spans.ms[SPAN_ENCODE]; }
 // src/automerge.js:105-118 getHistory's snapshots: getPatch(loadChanges(init(), getAllChanges()[0, k))) for every k
 int amg_get_history_patches(amg_backend* b, const uint64_t* prefix_lens, size_t n, amg_buffers** out, amg_error* err) {
-  AMG_GUARD(
-    auto* l = new amg_buffers(); std::unique_ptr<amg_buffers> guard(l);
-    b->eng.historyPatches((const u64*)prefix_lens, n, l->items);
-    *out = guard.release(); return 0;)
+  AMG_GUARD(*out = buffers([&](Items& l) { b->eng.historyPatches((const u64*)prefix_lens, n, l); }).release(); return 0;)
 }
-float amg_last_history_ms(amg_backend* b) { return b->eng.lastHistoryMs; }
+float amg_last_history_ms(amg_backend* b) { return b->eng.spans.ms[SPAN_HISTORY]; }
 // new.js:1979-1997: the changes in their order from Engine::changesAddedFrom (no host hash graph is built)
 int amg_get_changes_added(amg_backend* bn, amg_backend* bo, amg_buffers** out, amg_error* err) {
   AMG_GUARD(
     std::vector<u32> idx; bo->eng.changesAddedFrom(bn->eng, idx);
-    auto* l = new amg_buffers(); std::unique_ptr<amg_buffers> guard(l);
-    for (u32 i : idx) l->items.push_back(bn->changeBytes(i));
-    *out = guard.release(); return 0;)
+    *out = buffers([&](Items& l) { for (u32 i : idx) l.push_back(bn->changeBytes(i)); }).release(); return 0;)
 }
 // src/automerge.js:61-67 merge(local, remote): applyChanges(local, getChangesAdded(local, remote)), the bytes device to device
 int amg_merge(amg_backend* dst, amg_backend* src, int want_patch, amg_patch** out, amg_error* err) {
   AMG_GUARD(PatchOut p; dst->eng.mergeFrom(src->eng, want_patch != 0, p);
             if (out) *out = want_patch ? serialize(p) : nullptr; return 0;)
 }
-float amg_last_merge_ms(amg_backend* b) { return b->eng.lastMergeMs; }
+float amg_last_merge_ms(amg_backend* b) { return b->eng.spans.ms[SPAN_MERGE]; }
 int amg_get_change_by_hash(amg_backend* b, const uint8_t hash[32], amg_buffers** out, amg_error* err) {
-  AMG_GUARD(b->ensureGraph(); auto* l = new amg_buffers(); auto it = b->g.indexByHash.find(toHash(hash));
-            if (it != b->g.indexByHash.end()) l->items.push_back(b->changeBytes(it->second)); *out = l; return 0;)
+  AMG_GUARD(b->ensureGraph(); auto it = b->g.indexByHash.find(toHash(hash));
+            *out = buffers([&](Items& l) { if (it != b->g.indexByHash.end()) l.push_back(b->changeBytes(it->second)); }).release(); return 0;)
 }
 // new.js:2014-2028
 int amg_get_missing_deps(amg_backend* b, const uint8_t* heads, size_t n, amg_buffers** out, amg_error* err) {
@@ -313,20 +317,13 @@ int amg_get_missing_deps(amg_backend* b, const uint8_t* heads, size_t n, amg_buf
     for (size_t i = 0; i < n; i++) allDeps[toHash(heads + 32 * i)] = true;
     e.ensureHostMirror();
     for (auto& q : e.queue) {
-      Hash h;
-      // hash of the queued change: SHA-256 over bytes [8..) — computed on the host for the (short) queue
-      ByteReader r(e.hostArena.data(), q.off + 8, q.off + q.len); r.pos++; r.uleb();
-      const u64 nd = r.uleb(); for (u64 k = 0; k < nd; k++) { allDeps[toHash(e.hostArena.data() + r.pos)] = true; r.skip(32); }
-      u32 hh[8] = {0x6a09e667, 0xbb67ae85, 0x3c6ef372, 0xa54ff53a, 0x510e527f, 0x9b05688c, 0x1f83d9ab, 0x5be0cd19};
-      const u8* m = e.hostArena.data() + q.off + 8; const u32 mlen = q.len - 8; std::vector<u8> padded(m, m + mlen); padded.push_back(0x80);
-      while (padded.size() % 64 != 56) padded.push_back(0); for (int i = 7; i >= 0; i--) padded.push_back((u8)(((u64)mlen * 8) >> (8 * i)));
-      for (size_t o = 0; o < padded.size(); o += 64) { u32 w[16]; for (int i = 0; i < 16; i++) w[i] = (u32)padded[o + 4 * i] << 24 | (u32)padded[o + 4 * i + 1] << 16 | (u32)padded[o + 4 * i + 2] << 8 | padded[o + 4 * i + 3]; sha256_compress(hh, w, SHA_K); }
-      for (int i = 0; i < 8; i++) { h[4 * i] = hh[i] >> 24; h[4 * i + 1] = hh[i] >> 16; h[4 * i + 2] = hh[i] >> 8; h[4 * i + 3] = hh[i]; }
+      for (auto& d : readHeader(e.hostArena.data(), q).deps) allDeps[d] = true;
+      Hash h; host_sha256(e.hostArena.data() + q.off + 8, q.len - 8, h.data());   // the queued change's hash: SHA-256 over bytes [8..)
       inQueue[h] = true;
     }
-    auto* l = new amg_buffers();
-    for (auto& kv : allDeps) if (!b->g.indexByHash.count(kv.first) && !inQueue.count(kv.first)) l->items.emplace_back((const char*)kv.first.data(), 32);
-    *out = l; return 0;)
+    *out = buffers([&](Items& l) {
+      for (auto& kv : allDeps) if (!b->g.indexByHash.count(kv.first) && !inQueue.count(kv.first)) l.emplace_back((const char*)kv.first.data(), 32);
+    }).release(); return 0;)
 }
 int amg_clock_of(amg_backend* b, const uint8_t* actor, size_t actor_len, uint64_t* seq_out, amg_error* err) {
   AMG_GUARD(std::string a((const char*)actor, actor_len); *seq_out = 0; Engine& e = b->eng;

@@ -94,6 +94,22 @@ struct Trace {
   Ctx& ctx; HostClock clk; bool active = false; int nEv = 0, nHost = 12;
 };
 
+// Device span of the last call of each entry point kind (amg_last_*_ms): CUDA events on the main stream around the call's
+// uploads, kernels and read-backs; 0 in the emulation build. start(k) zeroes k's slot and opens the span, resume(k) opens
+// it without zeroing, stop() adds the span to the slot. A call that throws never reaches stop(): its slot stays 0.
+enum SpanKind { SPAN_SYNC, SPAN_DECODE, SPAN_ENCODE, SPAN_HISTORY, SPAN_MERGE, NUM_SPANS };
+struct DeviceSpans {
+  float ms[NUM_SPANS] = {0};
+  explicit DeviceSpans(Ctx& c) : ctx(c) {}
+  void start(SpanKind k) { ms[k] = 0; resume(k); }
+  void resume(SpanKind k); void stop();
+#ifndef AMG_EMU
+  ~DeviceSpans() { for (auto& e : ev) if (e) cudaEventDestroy(e); }
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+#endif
+  Ctx& ctx; SpanKind kind = SPAN_SYNC;
+};
+
 struct PatchOut {   // flat patch, written straight into the engine's pinned output buffer (layout: include/amgpu.h)
   u64 maxOp = 0, pendingChanges = 0; bool hasActorSeq = false; std::string actor; u64 seq = 0;
   std::vector<std::pair<u32, u64>> clock; std::vector<std::array<u8, 32>> deps; std::vector<std::string> actors;
@@ -177,6 +193,7 @@ class Engine {
   }
   Trace trace{ctx};
   HBuf<u8> patchBuf;   // pinned: patch records are copied device -> host directly into their final place
+  DeviceSpans spans{ctx};   // sync, decode, encode, history and merge calls
   // ---- scratch (grow-only)
   DBuf<u32> chOff, chLen, nOps, nPreds, nDeps, nActors, colOff, colLen, depBase, depIdx, primary, pass, flagWord, appRank, opBase, predBase, timeBase, amapBase, amap, authorSlot, newSlots;
   DBuf<u8> applied; DBuf<ChangeHot> hot; DBuf<ChangeMeta> meta /* save(): full headers */; DBuf<u64> errWord; DBuf<u32> hashTable;
@@ -231,7 +248,6 @@ class Engine {
     if (ctx.evMirror) cudaEventDestroy(ctx.evMirror);
     if (ctx.evFork) cudaEventDestroy(ctx.evFork);
     if (ctx.evJoin) cudaEventDestroy(ctx.evJoin);
-    for (auto& e : syncEv) if (e) cudaEventDestroy(e);
 #endif
   }
 
@@ -267,6 +283,7 @@ class Engine {
     errSnapshot = w[k]; errSnapLaunches = launchesNow;
   }
   u64 fetchErr() { if (errSnapLaunches != ctx.launches) { void* none[1] = {nullptr}; readWords({}, none); } return errSnapshot; }
+  void clearErr() { dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull; }   // the next check reads the word again
   static std::string opIdText(u64 id, const std::vector<std::string>& actors) {
     const u32 a = id_actor(id);
     return std::to_string(id_ctr(id)) + "@" + (a < actors.size() ? hex_of((const u8*)actors[a].data(), actors[a].size()) : std::string("?"));
@@ -321,6 +338,9 @@ class Engine {
   u32 readU32(const u32* dptr) { u32 v = 0; void* d[1] = {&v}; readWords({{dptr, 4}}, d); return v; }
   void readU32x2(const u32* a, const u32* b, u32* va, u32* vb) { void* d[2] = {va, vb}; readWords({{a, 4}, {b, 4}}, d); }
   void fill32(u32* p, u32 v, size_t n) { foreach(ctx, n, FillU32Kernel{p, v}); }
+  u64 hashTableOf(const u8* hs, size_t count);   // hashTable over hashes [0, count); returns its slot mask
+  u32 parseChangeHeaders(const u8* ar, const HostChange* pairs, size_t K);   // then resolveChangeDeps: dependency indexes from change headers
+  u64 resolveChangeDeps(const u8* ar, const u8* hs, size_t C, size_t K, size_t base, u32 totalDeps);
   // sort `perm` (row ids) by successive 64-bit fields produced by keyFn(field) ; stable LSD over fields
   void sortPairs(DBuf<u64>& keys, DBuf<u32>& vals, size_t n, int bits) { radix_sort_pairs(ctx, sortTmp, keys, vals, n, 0, bits); }
 
@@ -443,7 +463,7 @@ class Engine {
     DBuf<u32> listD; DBuf<u8> newHashes; std::vector<u8> isDep;
     HistOpView view() { return HistOpView{d, opId.p, opSrc.p, opPredStart.p, opPredNum.p, opOrder.p, pairRowSorted.p, (u32)N}; }
   };
-  void computeHashGraph();   // change history of a loaded document (history.cuh); the sections, in order:
+  void computeHashGraph();   // change history of a loaded document (history.cuh), once (later calls return at once); the sections, in order:
   void histChangeColumns(HistoryCall& h), histActorOrder(HistoryCall& h), histPredsAndDeletions(HistoryCall& h), histOpsToChanges(HistoryCall& h),
        histActorTables(HistoryCall& h), histEncode(HistoryCall& h), histHashes(HistoryCall& h), histCheckHeads(HistoryCall& h), histCommit(HistoryCall& h);
 
@@ -454,7 +474,6 @@ class Engine {
   void syncBloom(const u32* idx, size_t count, std::string& out);   // BloomFilter(hashes).bytes
   void syncChangesToSend(const u32* idx, size_t count, const std::vector<BloomSpec>& filters, std::vector<u8>& send);   // send[i]: Bloom-negative or depends on one
   void gatherHashes(const std::vector<u32>& idx, std::string& out);   // 32 bytes per change
-  float lastSyncMs = 0;   // device span (CUDA events on the main stream) of the last sync call's uploads, kernels and read-backs (0 in the emulation build)
   DBuf<u32> syncIdx, syncBits; DBuf<u8> syncFilterBits, syncNeg, syncHashOut; DBuf<BloomRef> syncFilters;
 
   // ---------------------------------------------------------------- decodeChange / decodeChanges (changes.cuh)
@@ -469,7 +488,8 @@ class Engine {
   void decodeChanges(const u8* blob, const u64* offsets, size_t n, bool history, std::string& out);
   void stageDecodeInput(DecodeCall& d, const u8* blob, const u64* offsets), inflateDecodeInput(DecodeCall& d), decodeTable(DecodeCall& d, std::string& out);
   [[noreturn]] void throwDecodeError(DecodeCall& d, const u64* words);
-  size_t decodeFailed = 0; float lastDecodeMs = 0;   // failing change of the last call; its device span (CUDA events; 0 in the emulation build)
+  std::pair<size_t, int> firstFailingChange(const u64* words, int numPhases, int opPhase, const u32* opBaseDev, size_t n);
+  size_t decodeFailed = 0;   // failing change of the last call
   DBuf<u8> dcArena, dcHash, dcOut; DBuf<u32> dcOff, dcLen, dcCLen, dcOps, dcPreds, dcActors, dcBytes, dcOpBase, dcPredBase, dcActorBase, dcByteBase, dcColOff, dcColLen, dcRows, dcChld;
   DBuf<ChangeMeta> dcMeta; DBuf<u64> dcErr, dcTotals; DBuf<u32> dcDefl;
 
@@ -491,7 +511,7 @@ class Engine {
        encodeColumns(EncodeCall& e), encodeHashes(EncodeCall& e);
   void copyEncodeOutput(EncodeCall& e, std::string& out, std::vector<u64>& offs, std::string& hashesOut);
   [[noreturn]] void throwEncodeError(EncodeCall& e, const u64* words);
-  size_t encodeFailed = 0; float lastEncodeMs = 0;   // failing change of the last call; its device span (CUDA events; 0 in the emulation build)
+  size_t encodeFailed = 0;   // failing change of the last call
 
   // ---------------------------------------------------------------- getHistory snapshots (snapshot.cuh)
   // The whole-document patch of the first k applied changes (getAllChanges order) for every k of a list: the op table
@@ -508,7 +528,6 @@ class Engine {
   void snapChangeMeta(HistoryPatchCall& h), snapActorOrder(HistoryPatchCall& h), snapChangeIndexes(HistoryPatchCall& h);
   size_t snapFilter(HistoryPatchCall& h, size_t k);   // per prefix length: the prefix document into snapDoc (returns its rows)
   void snapHeader(HistoryPatchCall& h, size_t k, PatchOut& out);
-  float lastHistoryMs = 0;   // device span of the last historyPatches call (CUDA events; 0 in the emulation build)
   DocBufs snapDoc; DBuf<u32> snapSuccOff, snapSuccCnt; DBuf<u64> snapSucc;   // the prefix document (grow-only; never the document's own)
 
   // ---------------------------------------------------------------- merge (merge.cuh)
@@ -518,14 +537,9 @@ class Engine {
   void changesAddedFrom(Engine& src, std::vector<u32>& order);
   // Automerge.merge (src/automerge.js:61-67): those changes, gathered from src's arena into one device blob, through applyChanges
   void mergeFrom(Engine& src, bool wantPatch, PatchOut& out);
-  float lastMergeMs = 0;   // device span of the last mergeFrom call (CUDA events; 0 in the emulation build)
   DBuf<u32> mergeAbsent, mergeSlot, mergeList, mergeHeadIdx; DBuf<u8> mergeHeads, mergeBlob; DBuf<MergeRange> mergeRanges;
  private:
   void uploadCandidates(const u32* idx, size_t count);
-  void syncTimer(bool start);
-#ifndef AMG_EMU
-  cudaEvent_t syncEv[2] = {nullptr, nullptr};
-#endif
 };
 
 }  // namespace amg

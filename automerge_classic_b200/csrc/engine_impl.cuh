@@ -199,7 +199,7 @@ inline void Engine::stageBatch(ApplyCall& a) {
     foreach(ctx, B, SplitPairsKernel{chPairs.p, chOff.p, chLen.p});
   }
   dev_memset(ctx, arena.p + a.cur, 0, 64);
-  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+  clearErr();
   hashes.ensure(ctx, (numApplied + B) * 32 + 64, numApplied * 32);
   deflList.ensure(ctx, B + 1);
   a.hashOut = hashes.p + numApplied * 32;
@@ -327,6 +327,14 @@ inline HostChange Engine::ApplyCall::originalOf(size_t b) const {
   return it != deflIdx.end() && *it == (u32)b ? inflOrig[it - deflIdx.begin()] : HostChange{0, 0};
 }
 
+// hashTable holding g for hash g of hashes [0, count) (for repeated hashes the smallest g)
+inline u64 Engine::hashTableOf(const u8* hs, size_t count) {
+  const size_t tcap = pow2_at_least(2 * count + 2);
+  hashTable.ensure(ctx, tcap); dev_memset(ctx, hashTable.p, 0xff, tcap * 4);
+  foreach(ctx, count, HashInsertKernel{hs, hashTable.p, (u64)tcap - 1});
+  return (u64)tcap - 1;
+}
+
 // ------------------------------------------------------------ 3. causal gate
 // (parse errors surface with the first host round trip of the gate: the error word travels with every small read, and a
 //  change that failed to parse has zero deps / ops so the kernels in between have nothing to walk)
@@ -335,10 +343,8 @@ inline void Engine::runGate(ApplyCall& a) {
   depBase.ensure(ctx, B + 1); scan_exclusive(ctx, scanTmp, nDeps.p, depBase.p, B);
   const size_t depBound = (a.cur - a.arenaLen0) / 32 + B + 1;   // every dependency occupies 32 bytes of its change: no need to read the exact total
   depIdx.ensure(ctx, depBound + 1); primary.ensure(ctx, B); pass.ensure(ctx, B);
-  a.G = numApplied + B; const size_t tcap = pow2_at_least(2 * a.G + 2);
-  hashTable.ensure(ctx, tcap); dev_memset(ctx, hashTable.p, 0xff, tcap * 4);
-  foreach(ctx, a.G, HashInsertKernel{hashes.p, hashTable.p, (u64)tcap - 1});
-  foreach(ctx, B, ResolveDepsKernel{arena.p, hashes.p, hashTable.p, (u64)tcap - 1, hot.p, nDeps.p, numApplied, depBase.p, depIdx.p, primary.p});
+  a.G = numApplied + B; const u64 mask = hashTableOf(hashes.p, a.G);
+  foreach(ctx, B, ResolveDepsKernel{arena.p, hashes.p, hashTable.p, mask, hot.p, nDeps.p, numApplied, depBase.p, depIdx.p, primary.p});
   fill32(pass.p, 1, B);
   dev_memset(ctx, flagWord.p + 12, 0, 4);
   foreach(ctx, B, GateDupFlagKernel{primary.p, numApplied, flagWord.p + 12});
@@ -984,7 +990,7 @@ inline void Engine::throwPatchValueError(u64 ew, size_t numProps) {
 }
 
 inline void Engine::getPatch(PatchOut& out) {
-  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+  clearErr();
   succCnt.ensure(ctx, numRows + 2);
   foreach(ctx, numRows, SuccCntFromOffKernel{succOff.p, succCnt.p});
   struct SideJoin { Ctx& c; ~SideJoin() { side_join(c); } } sideJoin{ctx};
@@ -1149,7 +1155,7 @@ inline void Engine::computeHashGraph() {
   if (L == 0) { loaded.haveHashGraph = true; return; }
   if (L >= (1u << 29) || numRows + numSucc >= (1u << 30)) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: document too large for history reconstruction");
   HistoryCall h{L, numRows, numSucc, st.actorIds.size(), doc.view()};
-  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+  clearErr();
   histChangeColumns(h); histActorOrder(h); histPredsAndDeletions(h); histOpsToChanges(h); histActorTables(h);
   histEncode(h); histHashes(h); histCheckHeads(h); histCommit(h);
 }
@@ -1389,7 +1395,7 @@ inline int Engine::debugDecodeColumn(const u8* bytes, size_t len, int kind, size
     if (!ok) { sync(ctx); return 1; }
     if (kind == 3 && n) foreach(ctx, n, U32ToI64Kernel{tmp.p, outD.p});
   } else {
-    dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+    clearErr();
     foreach_warp(ctx, 1, DebugColumnKernel{kind, colBytes.p, (u32)len, (u32)n, outD.p, tmp.p, errWord.p});
     checkErr();
   }
@@ -1409,7 +1415,7 @@ inline void Engine::decodeRaw(const u8* blob, const u64* offsets, size_t n, u8* 
   }
   DBuf<u8> ar; ar.ensure(ctx, staged.size() + 64); h2d(ctx, ar.p, staged.data(), staged.size()); dev_memset(ctx, ar.p + staged.size(), 0, 64);
   chOff.ensure(ctx, n); chLen.ensure(ctx, n); h2d(ctx, chOff.p, off.data(), n * 4); h2d(ctx, chLen.p, len.data(), n * 4);
-  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull; hashTmp.ensure(ctx, n * 32 + 64);
+  clearErr(); hashTmp.ensure(ctx, n * 32 + 64);
   foreach(ctx, n, ShaKernel{ar.p, chOff.p, chLen.p, hashTmp.p, errWord.p, nullptr, nullptr});
   applied.ensure(ctx, n); dev_memset(ctx, applied.p, 1, n);
   u32 tot[4] = {0, 0, 0, 0}; void* dst[4] = {&tot[0], &tot[1], &tot[2], &tot[3]};
@@ -1456,7 +1462,7 @@ inline void Engine::saveDocument(std::string& result) {
   if (!encoder) encoder.reset(new ColumnEncoder(ctx, scanTmp));
   encoder->outLen = 0;
   SaveCall s{numApplied, numRows, numSucc, loaded.numChanges, numApplied - loaded.numChanges};
-  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+  clearErr();
   saveVals.ensure(ctx, std::max(std::max(s.C, s.N), s.S) + 2);
   saveChangeColumns(s); saveOpColumns(s); packDocument(s, result);
 }
@@ -1488,19 +1494,8 @@ inline void Engine::saveChangeColumns(SaveCall& s) {
 inline void Engine::parseChangeMeta(ChangeMetaCall& m) {
   const size_t C = m.C, L = m.L, K = m.K;
   if (K > 0) {
-    chPairs.ensure(ctx, K); chOff.ensure(ctx, K); chLen.ensure(ctx, K);
-    h2d(ctx, chPairs.p, changes.data() + L, K * sizeof(HostChange));
-    foreach(ctx, K, SplitPairsKernel{chPairs.p, chOff.p, chLen.p});
-    meta.ensure(ctx, K); colOff.ensure(ctx, (size_t)NCOLS * K); colLen.ensure(ctx, (size_t)NCOLS * K);
-    nOps.ensure(ctx, K + 1); nPreds.ensure(ctx, K + 1); nDeps.ensure(ctx, K + 1); nActors.ensure(ctx, K + 1);
-    foreach(ctx, K, ParseKernel{arena.p, chOff.p, chLen.p, K, meta.p, colOff.p, colLen.p, nOps.p, nPreds.p, nDeps.p, nActors.p, errWord.p, flagWord.p + 8});
-    depBase.ensure(ctx, K + 1); scan_exclusive(ctx, scanTmp, nDeps.p, depBase.p, K);
-    m.laterDeps = readU32(depBase.p + K);
-    depIdx.ensure(ctx, m.laterDeps + 1); primary.ensure(ctx, K);
-    const size_t tcap = pow2_at_least(2 * C + 2);
-    hashTable.ensure(ctx, tcap); dev_memset(ctx, hashTable.p, 0xff, tcap * 4);
-    foreach(ctx, C, HashInsertKernel{hashes.p, hashTable.p, (u64)tcap - 1});
-    foreach(ctx, K, ResolveDepsKernelT<ChangeMeta>{arena.p, hashes.p, hashTable.p, (u64)tcap - 1, meta.p, nDeps.p, L, depBase.p, depIdx.p, primary.p});
+    m.laterDeps = parseChangeHeaders(arena.p, changes.data() + L, K);
+    resolveChangeDeps(arena.p, hashes.p, C, K, L, m.laterDeps);
   }
   if (L > 0) {   // number of dependency indexes the loaded changes carry
     DBuf<u64>& sumD = pairSucc; sumD.ensure(ctx, 1);
@@ -1512,6 +1507,28 @@ inline void Engine::parseChangeMeta(ChangeMetaCall& m) {
     }
     m.loadedDeps = (u32)sum;
   }
+}
+
+// Dependency indexes of K changes: parseChangeHeaders parses the headers at `pairs` in `ar` into meta / nDeps / depBase and
+// returns the number of dependency hashes; resolveChangeDeps looks them up among hashes [0, C) into depIdx and returns the
+// table's mask. `base`: ResolveDepsKernelT's numApplied (with 0 only depIdx is meaningful). Neither checks the error word; a
+// caller that checks it right after parseChangeHeaders gets it with the total, at no extra read.
+inline u32 Engine::parseChangeHeaders(const u8* ar, const HostChange* pairs, size_t K) {
+  chPairs.ensure(ctx, K); chOff.ensure(ctx, K); chLen.ensure(ctx, K);
+  h2d(ctx, chPairs.p, pairs, K * sizeof(HostChange));
+  foreach(ctx, K, SplitPairsKernel{chPairs.p, chOff.p, chLen.p});
+  meta.ensure(ctx, K); colOff.ensure(ctx, (size_t)NCOLS * K); colLen.ensure(ctx, (size_t)NCOLS * K);
+  nOps.ensure(ctx, K + 1); nPreds.ensure(ctx, K + 1); nDeps.ensure(ctx, K + 1); nActors.ensure(ctx, K + 1);
+  foreach(ctx, K, ParseKernel{ar, chOff.p, chLen.p, K, meta.p, colOff.p, colLen.p, nOps.p, nPreds.p, nDeps.p, nActors.p, errWord.p, flagWord.p + 8});
+  depBase.ensure(ctx, K + 1); scan_exclusive(ctx, scanTmp, nDeps.p, depBase.p, K);
+  return readU32(depBase.p + K);
+}
+
+inline u64 Engine::resolveChangeDeps(const u8* ar, const u8* hs, size_t C, size_t K, size_t base, u32 totalDeps) {
+  depIdx.ensure(ctx, (size_t)totalDeps + 1); primary.ensure(ctx, K);
+  const u64 mask = hashTableOf(hs, C);
+  foreach(ctx, K, ResolveDepsKernelT<ChangeMeta>{ar, hs, hashTable.p, mask, meta.p, nDeps.p, base, depBase.p, depIdx.p, primary.p});
+  return mask;
 }
 
 inline void Engine::changeMetaColumn(const ChangeMetaCall& m, int col, long long* out, u32* strOff, u32* strLen) {
@@ -1721,7 +1738,7 @@ inline void Engine::ensureLoadRows(size_t n) {
 // decoder (doccols.cuh); short, malformed or non-canonical ones the serial walkers, which also report the errors.
 inline void Engine::countRows(LoadCall& l) {
   const DocCols& dc = l.dc;
-  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull; dev_memset(ctx, flagWord.p, 0, 16);
+  clearErr(); dev_memset(ctx, flagWord.p, 0, 16);
   { const char* e = getenv("AMG_PAR_DOC_MIN"); if (e) parDocMinRows = (size_t)strtoull(e, nullptr, 10); }
   auto succInParallel = [&](size_t rows) {   // many rows: the succ total in parallel too (succNum then needs no serial decode)
     if (rows < parDocMinRows || rows >= (1u << 29)) return;
@@ -1826,17 +1843,22 @@ inline void Engine::commitLoad(LoadCall& l) {
   actorSlots.ensure(ctx, actorCap); rebuildActorTable();
 }
 
-// ---------------------------------------------------------------- sync protocol (sync.js:234-306)
-inline void Engine::syncTimer(bool start) {
+// ---------------------------------------------------------------- device spans (amg_last_*_ms)
+inline void DeviceSpans::resume(SpanKind k) {
+  kind = k;
 #ifndef AMG_EMU
-  if (!syncEv[0]) for (auto& e : syncEv) CUDA_CHECK(cudaEventCreate(&e));
-  CUDA_CHECK(cudaEventRecord(syncEv[start ? 0 : 1], ctx.stream));
-  if (!start) { float ms = 0; CUDA_CHECK(cudaEventSynchronize(syncEv[1])); CUDA_CHECK(cudaEventElapsedTime(&ms, syncEv[0], syncEv[1])); lastSyncMs += ms; }
-#else
-  (void)start;
+  if (!ev[0]) for (auto& e : ev) CUDA_CHECK(cudaEventCreate(&e));
+  CUDA_CHECK(cudaEventRecord(ev[0], ctx.stream));
+#endif
+}
+inline void DeviceSpans::stop() {
+#ifndef AMG_EMU
+  float t = 0; CUDA_CHECK(cudaEventRecord(ev[1], ctx.stream));
+  CUDA_CHECK(cudaEventSynchronize(ev[1])); CUDA_CHECK(cudaEventElapsedTime(&t, ev[0], ev[1])); ms[kind] += t;
 #endif
 }
 
+// ---------------------------------------------------------------- sync protocol (sync.js:234-306)
 inline void Engine::uploadCandidates(const u32* idx, size_t count) {
   if (!idx) return;
   syncIdx.ensure(ctx, count + 1); h2d(ctx, syncIdx.p, idx, count * 4);
@@ -1844,10 +1866,9 @@ inline void Engine::uploadCandidates(const u32* idx, size_t count) {
 
 // makeBloomFilter (sync.js:234-238): BloomFilter(hashes).bytes = LEB128 numEntries, 10, 7, then ceil(10 * count / 8) bytes
 inline void Engine::syncBloom(const u32* idx, size_t count, std::string& out) {
-  out.clear(); lastSyncMs = 0;
+  out.clear(); spans.start(SPAN_SYNC);
   if (count == 0) return;   // BloomFilter([]).bytes is empty
   const size_t bitsBytes = (BLOOM_BITS_PER_ENTRY * count + 7) / 8, words = (bitsBytes + 3) / 4;
-  syncTimer(true);
   uploadCandidates(idx, count);
   syncBits.ensure(ctx, words); dev_memset(ctx, syncBits.p, 0, words * 4);
   foreach(ctx, count, BloomAddKernel{hashes.p, idx ? syncIdx.p : nullptr, 8 * (u64)bitsBytes, syncBits.p});
@@ -1855,16 +1876,15 @@ inline void Engine::syncBloom(const u32* idx, size_t count, std::string& out) {
   const size_t at = out.size(); out.resize(at + words * 4);
   d2h(ctx, &out[at], syncBits.p, words * 4); sync(ctx);
   out.resize(at + bitsBytes);
-  syncTimer(false);
+  spans.stop();
 }
 
 // getChangesToSend (sync.js:246-306) for a non-empty `have`: which candidates go out because of the peer's filters.
 inline void Engine::syncChangesToSend(const u32* idx, size_t count, const std::vector<BloomSpec>& filters, std::vector<u8>& send) {
-  send.assign(count, 0); lastSyncMs = 0;
+  send.assign(count, 0); spans.start(SPAN_SYNC);
   if (count == 0) return;
   for (auto& f : filters)
     if (f.numProbes > BLOOM_MAX_PROBES) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: a Bloom filter with " + std::to_string(f.numProbes) + " probes (the device path takes at most " + std::to_string(BLOOM_MAX_PROBES) + ")");
-  syncTimer(true);
   uploadCandidates(idx, count);
   const u32* idxD = idx ? syncIdx.p : nullptr;
   // sync.js:273-276: a candidate is negative when no filter contains it
@@ -1880,30 +1900,18 @@ inline void Engine::syncChangesToSend(const u32* idx, size_t count, const std::v
   foreach(ctx, count, BloomProbeKernel{hashes.p, idxD, syncFilterBits.p, syncFilters.p, (u32)refs.size(), syncNeg.p});
   d2h(ctx, send.data(), syncNeg.p, count); sync(ctx);
   size_t numNeg = 0; for (u8 v : send) numNeg += v;
-  if (numNeg == 0 || numNeg == count) { syncTimer(false); return; }   // a peer that has everything, or a new one: no closure needed
+  if (numNeg == 0 || numNeg == count) { spans.stop(); return; }   // a peer that has everything, or a new one: no closure needed
   // sync.js:277-289: everything that depends on a Bloom-negative candidate goes too. The candidates' dependency indexes are
-  // resolved like save() does (ParseKernel over their headers, scan, HashInsertKernel, ResolveDepsKernelT<ChangeMeta>).
+  // resolved like save() does (parseChangeHeaders, resolveChangeDeps).
   const size_t K = count, C = numApplied;
   std::vector<HostChange> pairs(K); for (size_t i = 0; i < K; i++) pairs[i] = changes[idx ? idx[i] : i];
-  chPairs.ensure(ctx, K); chOff.ensure(ctx, K); chLen.ensure(ctx, K);
-  h2d(ctx, chPairs.p, pairs.data(), K * sizeof(HostChange));
-  foreach(ctx, K, SplitPairsKernel{chPairs.p, chOff.p, chLen.p});
-  meta.ensure(ctx, K); colOff.ensure(ctx, (size_t)NCOLS * K); colLen.ensure(ctx, (size_t)NCOLS * K);
-  nOps.ensure(ctx, K + 1); nPreds.ensure(ctx, K + 1); nDeps.ensure(ctx, K + 1); nActors.ensure(ctx, K + 1);
-  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
-  foreach(ctx, K, ParseKernel{arena.p, chOff.p, chLen.p, K, meta.p, colOff.p, colLen.p, nOps.p, nPreds.p, nDeps.p, nActors.p, errWord.p, flagWord.p + 8});
-  depBase.ensure(ctx, K + 1); scan_exclusive(ctx, scanTmp, nDeps.p, depBase.p, K);
-  const u32 totalDeps = readU32(depBase.p + K);
+  clearErr();
+  const u32 totalDeps = parseChangeHeaders(arena.p, pairs.data(), K);
   checkErr();
-  depIdx.ensure(ctx, totalDeps + 1); primary.ensure(ctx, K);
-  const size_t tcap = pow2_at_least(2 * C + 2);
-  hashTable.ensure(ctx, tcap); dev_memset(ctx, hashTable.p, 0xff, tcap * 4);
-  foreach(ctx, C, HashInsertKernel{hashes.p, hashTable.p, (u64)tcap - 1});
-  // numApplied = 0: primary[b] looks up change b, which exists (b < K <= C); only depIdx is used here
-  foreach(ctx, K, ResolveDepsKernelT<ChangeMeta>{arena.p, hashes.p, hashTable.p, (u64)tcap - 1, meta.p, nDeps.p, 0, depBase.p, depIdx.p, primary.p});
+  resolveChangeDeps(arena.p, hashes.p, C, K, 0, totalDeps);
   std::vector<u32> base(K + 1), deps(totalDeps);
   d2h(ctx, base.data(), depBase.p, (K + 1) * 4); d2h(ctx, deps.data(), depIdx.p, (size_t)totalDeps * 4); sync(ctx);
-  syncTimer(false);
+  spans.stop();
   // One forward pass in application order: a change is applied only after its dependencies (a loaded document stores its
   // changes in topological order), so a candidate's candidate dependencies are decided before it is. This stays on the host
   // on purpose: it is O(candidates + deps), while a device frontier walk needs one launch per dependency level, which on a
@@ -1920,15 +1928,13 @@ inline void Engine::syncChangesToSend(const u32* idx, size_t count, const std::v
 
 // ------------------------------------------------------------ decodeChange / decodeChanges (changes.cuh)
 inline void Engine::decodeChanges(const u8* blob, const u64* offsets, size_t n, bool history, std::string& out) {
-  DecodeCall d; d.n = n; d.history = history; decodeFailed = 0; lastDecodeMs = 0;
-  const float keepSyncMs = lastSyncMs; lastSyncMs = 0;
-  struct Restore { Engine& e; float ms; ~Restore() { e.lastSyncMs = ms; } } restore{*this, keepSyncMs};   // the timer is shared with the sync calls
-  syncTimer(true);
+  DecodeCall d; d.n = n; d.history = history; decodeFailed = 0;
+  spans.start(SPAN_DECODE);
   dcErr.ensure(ctx, DP_NUM); dev_memset(ctx, dcErr.p, 0, DP_NUM * 8);
-  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+  clearErr();
   dcOff.ensure(ctx, n + 1); dcLen.ensure(ctx, n + 1); dcHash.ensure(ctx, n * 32 + 64);
   if (history) {   // every applied change (getAllChanges order), inflated copies in place; their hashes are the engine's
-    if (!loaded.haveHashGraph) computeHashGraph();
+    computeHashGraph();
     if (n) {
       chPairs.ensure(ctx, n); h2d(ctx, chPairs.p, changes.data(), n * sizeof(HostChange));
       foreach(ctx, n, SplitPairsKernel{chPairs.p, dcOff.p, dcLen.p});
@@ -1941,7 +1947,7 @@ inline void Engine::decodeChanges(const u8* blob, const u64* offsets, size_t n, 
     d.ar = dcArena.p;
   }
   decodeTable(d, out);
-  syncTimer(false); lastDecodeMs = lastSyncMs;
+  spans.stop();
 }
 
 // the caller's bytes into scratch (never into the document's arena): device memory is copied device to device, host
@@ -2035,17 +2041,24 @@ inline void Engine::decodeTable(DecodeCall& d, std::string& out) {
   d2h(ctx, &out[0], dcOut.p, d.size); sync(ctx);
 }
 
-// The change the sequential reference fails on first: the smallest failing change over all phases (op errors are keyed by
-// op: mapped to their change), and for it the error of its earliest phase.
-inline void Engine::throwDecodeError(DecodeCall& d, const u64* w) {
-  const size_t n = d.n; std::vector<u32> opBase(n + 1); d2h(ctx, opBase.data(), dcOpBase.p, (n + 1) * 4); sync(ctx);
+// The change the sequential reference fails on first: the smallest failing change over the phases' error words (those of
+// phase opPhase are keyed by op and mapped to their change through the n + 1 op offsets at opBaseDev), and its earliest
+// failing phase
+inline std::pair<size_t, int> Engine::firstFailingChange(const u64* w, int numPhases, int opPhase, const u32* opBaseDev, size_t n) {
+  std::vector<u32> opBase(n + 1); d2h(ctx, opBase.data(), opBaseDev, (n + 1) * 4); sync(ctx);
   size_t best = SIZE_MAX; int phase = -1;
-  for (int k = 0; k < DP_NUM; k++) {
+  for (int k = 0; k < numPhases; k++) {
     if (!w[k]) continue;
     size_t c = (size_t)(w[k] >> 8);
-    if (k == DP_OPS) c = (size_t)(std::upper_bound(opBase.begin(), opBase.end(), (u32)c) - opBase.begin()) - 1;
+    if (k == opPhase) c = (size_t)(std::upper_bound(opBase.begin(), opBase.end(), (u32)c) - opBase.begin()) - 1;
     if (c < best) { best = c; phase = k; }
   }
+  return {best, phase};
+}
+
+// The first failing change (firstFailingChange), and for it the error of its earliest phase
+inline void Engine::throwDecodeError(DecodeCall& d, const u64* w) {
+  const auto [best, phase] = firstFailingChange(w, DP_NUM, DP_OPS, dcOpBase.p, d.n);
   decodeFailed = best; const u32 code = (u32)(w[phase] & 0xff);
   auto actorIndex = [](u32 a) { return "No actor index " + std::to_string(a); };
   if (code == DE_CHUNK_TYPE_N) {
@@ -2077,15 +2090,13 @@ inline void Engine::throwDecodeError(DecodeCall& d, const u64* w) {
 
 // ------------------------------------------------------------ encodeChange over a change table (encchg.cuh)
 inline void Engine::encodeChanges(const u8* table, size_t len, std::string& out, std::vector<u64>& offs, std::string& hashesOut) {
-  EncodeCall e; e.len = len; encodeFailed = 0; lastEncodeMs = 0;
-  const float keepSyncMs = lastSyncMs; lastSyncMs = 0;
-  struct Restore { Engine& e; float ms; ~Restore() { e.lastSyncMs = ms; } } restore{*this, keepSyncMs};   // the timer is shared with the sync calls
-  syncTimer(true);
-  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+  EncodeCall e; e.len = len; encodeFailed = 0;
+  spans.start(SPAN_ENCODE);
+  clearErr();
   stageEncodeInput(e, table);
   if (e.n) { validateTable(e); encodeActorTables(e); encodePrep(e); encodeColumns(e); encodeHashes(e); }
   copyEncodeOutput(e, out, offs, hashesOut);
-  syncTimer(false); lastEncodeMs = lastSyncMs;
+  spans.stop();
 }
 
 // 1. the table into scratch as decodeChanges stages its input (pinned, pageable or device memory); the header's sections
@@ -2206,17 +2217,9 @@ inline void Engine::copyEncodeOutput(EncodeCall& e, std::string& out, std::vecto
   d2h(ctx, offs.data(), e.outOff.p, (n + 1) * 8); d2h(ctx, &hashesOut[0], e.hashes.p, n * 32); sync(ctx);
 }
 
-// The smallest failing change over both phases (op errors are keyed by op: mapped to their change), and for it the error
-// of its earliest phase
+// The first failing change (firstFailingChange), and for it the error of its earliest phase
 inline void Engine::throwEncodeError(EncodeCall& e, const u64* w) {
-  const size_t n = e.n; std::vector<u32> opBase(n + 1); d2h(ctx, opBase.data(), e.opBase.p, (n + 1) * 4); sync(ctx);
-  size_t best = SIZE_MAX; int phase = -1;
-  for (int k = 0; k < EP_NUM; k++) {
-    if (!w[k]) continue;
-    size_t c = (size_t)(w[k] >> 8);
-    if (k == EP_OPS) c = (size_t)(std::upper_bound(opBase.begin(), opBase.end(), (u32)c) - opBase.begin()) - 1;
-    if (c < best) { best = c; phase = k; }
-  }
+  const auto [best, phase] = firstFailingChange(w, EP_NUM, EP_OPS, e.opBase.p, e.n);
   encodeFailed = best; const u32 code = (u32)(w[phase] & 0xff);
   const std::string at = "change table: change " + std::to_string(best) + ": ";
   switch (code) {
@@ -2239,8 +2242,8 @@ inline void Engine::throwEncodeError(EncodeCall& e, const u64* w) {
     default: break;
   }
   if (phase == EP_OPS) {   // the messages that name a value of the op
-    const size_t j = (size_t)(w[phase] >> 8); ChangeRec r; d2h(ctx, &r, e.T.ch + best, sizeof(r)); sync(ctx);
-    OpRec o; d2h(ctx, &o, e.T.ops + r.firstOp + (j - opBase[best]), sizeof(o)); sync(ctx);
+    const size_t j = (size_t)(w[phase] >> 8); ChangeRec r; u32 opBase = 0; d2h(ctx, &r, e.T.ch + best, sizeof(r)); d2h(ctx, &opBase, e.opBase.p + best, 4); sync(ctx);
+    OpRec o; d2h(ctx, &o, e.T.ops + r.firstOp + (j - opBase), sizeof(o)); sync(ctx);
     auto actorIndex = [](u32 a) { return "No actor index " + std::to_string(a); };
     switch (code) {
       case EE_KEY_ACTOR: throw Error(AMG_ERR_RANGE, actorIndex(o.keyActor));
@@ -2262,35 +2265,33 @@ inline void Engine::throwEncodeError(EncodeCall& e, const u64* w) {
 inline void Engine::gatherHashes(const std::vector<u32>& idx, std::string& out) {
   out.assign(idx.size() * 32, '\0');
   if (idx.empty()) return;
-  syncTimer(true);
+  spans.resume(SPAN_SYNC);
   syncIdx.ensure(ctx, idx.size() + 1); h2d(ctx, syncIdx.p, idx.data(), idx.size() * 4);
   syncHashOut.ensure(ctx, idx.size() * 32);
   foreach(ctx, idx.size(), SyncHashGatherKernel{hashes.p, syncIdx.p, syncHashOut.p});
   d2h(ctx, &out[0], syncHashOut.p, out.size()); sync(ctx);
-  syncTimer(false);   // adds to the span of the syncChangesToSend call it follows
+  spans.stop();   // adds to the span of the syncChangesToSend call it follows
 }
 
 
 // ------------------------------------------------------------ getHistory snapshots (snapshot.cuh; src/automerge.js:105-118)
 // out[i] = the flat whole-document patch that getPatch(loadChanges(init(), getAllChanges()[0, prefixLens[i]))) returns
 inline void Engine::historyPatches(const u64* prefixLens, size_t n, std::vector<std::string>& out) {
-  out.clear(); lastHistoryMs = 0;
+  out.clear(); spans.ms[SPAN_HISTORY] = 0;   // also when the call fails before its span starts
   for (size_t i = 0; i < n; i++)
     if (prefixLens[i] > numApplied) throw Error(AMG_ERR_RANGE, "history prefix length " + std::to_string(prefixLens[i]) + " exceeds the " + std::to_string(numApplied) + " applied changes");
   if (n == 0) return;
-  if (!loaded.haveHashGraph) computeHashGraph();   // the prefixes' heads are change hashes (as amg_decode_history)
+  computeHashGraph();   // the prefixes' heads are change hashes (as amg_decode_history)
   HistoryPatchCall h; h.C = numApplied; h.A = st.actorIds.size(); h.N = numRows; h.S = numSucc;
   if (h.C >= (1u << 31) || h.N + h.S >= (1u << 31)) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: document too large for history snapshots");
-  const float keepSyncMs = lastSyncMs; lastSyncMs = 0;
-  struct Restore { Engine& e; float ms; ~Restore() { e.lastSyncMs = ms; } } restore{*this, keepSyncMs};   // the timer is shared with the sync calls
   struct SideJoin { Ctx& c; ~SideJoin() { side_join(c); } } sideJoin{ctx};
-  syncTimer(true);
-  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+  spans.start(SPAN_HISTORY);
+  clearErr();
   if (h.C) { snapChangeMeta(h); snapActorOrder(h); snapChangeIndexes(h); }
   const Ord ord{actorRank.p, bits_for(std::max<size_t>(h.A, 2) - 1)};
   for (size_t i = 0; i < n; i++) {
     const size_t k = (size_t)prefixLens[i];
-    dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+    clearErr();
     const size_t Nk = snapFilter(h, k);
     PatchOut p;
     buildPatch(PatchInputs{snapDoc.view(), Nk, true, snapSuccOff.p, snapSucc.p, snapSuccCnt.p, ord}, p);
@@ -2300,7 +2301,7 @@ inline void Engine::historyPatches(const u64* prefixLens, size_t n, std::vector<
     finishPatch(p);
     out.emplace_back((const char*)p.bytes, p.bytesLen);   // patchBuf is reused by the next prefix length
   }
-  syncTimer(false); lastHistoryMs = lastSyncMs;
+  spans.stop();
 }
 
 // 1. actor number, seq, maxOp and dependency indexes of every applied change (the change metadata phase save() uses)
@@ -2390,20 +2391,18 @@ inline void Engine::snapHeader(HistoryPatchCall& h, size_t k, PatchOut& out) {
 // changes' dependency indexes, for the reason syncChangesToSend gives (a device walk needs one launch per level).
 inline void Engine::changesAddedFrom(Engine& src, std::vector<u32>& order) {
   order.clear();
-  if (!loaded.haveHashGraph) computeHashGraph();   // new.js:1980; the package builds both documents' graphs (DESIGN.md section 5)
-  if (!src.loaded.haveHashGraph) src.computeHashGraph();
+  computeHashGraph();   // new.js:1980; the package builds both documents' graphs (DESIGN.md section 5)
+  src.computeHashGraph();
   if (src.ctx.device != ctx.device)
     throw Error(AMG_ERR_UNSUPPORTED, "amgpu: the documents are on different devices (" + std::to_string(src.ctx.device) + ", " + std::to_string(ctx.device) + ")");
   sync(src.ctx);   // src's buffers are read on this engine's stream
   const size_t C = src.numApplied;
   if (C == 0) return;
-  dev_memset(ctx, errWord.p, 0, 16); errSnapLaunches = ~0ull;
+  clearErr();
   // 1. presence: this document's hashes in a table, one probe per change of src, then flag -> scan -> compact
-  size_t tcap = pow2_at_least(2 * numApplied + 2);
-  hashTable.ensure(ctx, tcap); dev_memset(ctx, hashTable.p, 0xff, tcap * 4);
-  foreach(ctx, numApplied, HashInsertKernel{hashes.p, hashTable.p, (u64)tcap - 1});
+  const u64 ownMask = hashTableOf(hashes.p, numApplied);
   mergeAbsent.ensure(ctx, C + 1); mergeSlot.ensure(ctx, C + 2);
-  foreach(ctx, C, MergeProbeKernel{hashes.p, hashTable.p, (u64)tcap - 1, src.hashes.p, mergeAbsent.p});
+  foreach(ctx, C, MergeProbeKernel{hashes.p, hashTable.p, ownMask, src.hashes.p, mergeAbsent.p});
   scan_exclusive(ctx, scanTmp, mergeAbsent.p, mergeSlot.p, C);
   const size_t K = readU32(mergeSlot.p + C);
   if (K == 0) return;
@@ -2411,28 +2410,16 @@ inline void Engine::changesAddedFrom(Engine& src, std::vector<u32>& order) {
   foreach(ctx, C, CompactKernel{mergeAbsent.p, mergeSlot.p, mergeList.p});
   std::vector<u32> absent(K); d2h(ctx, absent.data(), mergeList.p, K * 4); sync(ctx);
   // 2. the absent changes' dependencies in header order (the order of dependenciesByHash) and src's heads, as change
-  //    indexes of src: ParseKernel over their headers in src's arena, src's hashes in the table, ResolveDepsKernelT
+  //    indexes of src: their headers in src's arena, resolved against src's hashes (parseChangeHeaders, resolveChangeDeps)
   std::vector<HostChange> pairs(K); for (size_t k = 0; k < K; k++) pairs[k] = src.changes[absent[k]];
-  chPairs.ensure(ctx, K); chOff.ensure(ctx, K); chLen.ensure(ctx, K);
-  h2d(ctx, chPairs.p, pairs.data(), K * sizeof(HostChange));
-  foreach(ctx, K, SplitPairsKernel{chPairs.p, chOff.p, chLen.p});
-  meta.ensure(ctx, K); colOff.ensure(ctx, (size_t)NCOLS * K); colLen.ensure(ctx, (size_t)NCOLS * K);
-  nOps.ensure(ctx, K + 1); nPreds.ensure(ctx, K + 1); nDeps.ensure(ctx, K + 1); nActors.ensure(ctx, K + 1);
-  foreach(ctx, K, ParseKernel{src.arena.p, chOff.p, chLen.p, K, meta.p, colOff.p, colLen.p, nOps.p, nPreds.p, nDeps.p, nActors.p, errWord.p, flagWord.p + 8});
-  depBase.ensure(ctx, K + 1); scan_exclusive(ctx, scanTmp, nDeps.p, depBase.p, K);
-  const u32 D = readU32(depBase.p + K);
+  const u32 D = parseChangeHeaders(src.arena.p, pairs.data(), K);
   checkErr();
-  depIdx.ensure(ctx, (size_t)D + 1); primary.ensure(ctx, K);
-  tcap = pow2_at_least(2 * C + 2);
-  hashTable.ensure(ctx, tcap); dev_memset(ctx, hashTable.p, 0xff, tcap * 4);
-  foreach(ctx, C, HashInsertKernel{src.hashes.p, hashTable.p, (u64)tcap - 1});
-  // numApplied = 0: primary[b] looks up change b of src, which exists (b < K <= C); only depIdx is used here
-  foreach(ctx, K, ResolveDepsKernelT<ChangeMeta>{src.arena.p, src.hashes.p, hashTable.p, (u64)tcap - 1, meta.p, nDeps.p, 0, depBase.p, depIdx.p, primary.p});
+  const u64 srcMask = resolveChangeDeps(src.arena.p, src.hashes.p, C, K, 0, D);
   const size_t H = src.st.heads.size();
   mergeHeads.ensure(ctx, H * 32 + 32); mergeHeadIdx.ensure(ctx, H + 1);
   std::vector<u8> headBytes(H * 32); for (size_t i = 0; i < H; i++) memcpy(headBytes.data() + 32 * i, src.st.heads[i].data(), 32);
   h2d(ctx, mergeHeads.p, headBytes.data(), H * 32);
-  foreach(ctx, H, HashLookupKernel{src.hashes.p, hashTable.p, (u64)tcap - 1, mergeHeads.p, mergeHeadIdx.p});
+  foreach(ctx, H, HashLookupKernel{src.hashes.p, hashTable.p, srcMask, mergeHeads.p, mergeHeadIdx.p});
   std::vector<u32> base(K + 1), deps(D), stack(H);
   d2h(ctx, base.data(), depBase.p, (K + 1) * 4); d2h(ctx, deps.data(), depIdx.p, (size_t)D * 4); d2h(ctx, stack.data(), mergeHeadIdx.p, H * 4); sync(ctx);
   // 3. new.js:1983-1994: heads in order, popped from the back; the seen test at pop time; dependencies pushed in header
@@ -2453,10 +2440,7 @@ inline void Engine::changesAddedFrom(Engine& src, std::vector<u32>& order) {
 // it has one, else its plain bytes. A change getChangesAdded would DEFLATE on the way out (exportsDeflated) goes over
 // plain and marked instead, so that this document hands it out DEFLATEd later, as if it had received it that way.
 inline void Engine::mergeFrom(Engine& src, bool wantPatch, PatchOut& out) {
-  lastMergeMs = 0;
-  const float keepSyncMs = lastSyncMs; lastSyncMs = 0;
-  struct Restore { Engine& e; float ms; ~Restore() { e.lastSyncMs = ms; } } restore{*this, keepSyncMs};   // the timer is shared with the sync calls
-  syncTimer(true);
+  spans.start(SPAN_MERGE);
   std::vector<u32> idx; changesAddedFrom(src, idx);
   const size_t K = idx.size();
   std::vector<u64> offs(K + 1, 0); std::vector<MergeRange> ranges(K); std::vector<u8> marks(K + 1, 0);
@@ -2470,7 +2454,7 @@ inline void Engine::mergeFrom(Engine& src, bool wantPatch, PatchOut& out) {
   h2d(ctx, mergeRanges.p, ranges.data(), K * sizeof(MergeRange));
   merge_gather(ctx, K, MergeGatherKernel{src.arena.p, mergeBlob.p, mergeRanges.p});
   applyChanges(nullptr, nullptr, K, mergeBlob.p, offs.data(), false, wantPatch, out, marks.data());   // the device-blob path of amg_apply_changes_packed
-  syncTimer(false); lastMergeMs = lastSyncMs;
+  spans.stop();
 }
 
 }  // namespace amg

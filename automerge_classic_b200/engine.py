@@ -80,31 +80,42 @@ class Library:
             getattr(L, name).restype = C.c_int
         L.amg_sync_bloom.argtypes = [vp, vp, C.c_size_t, vp, vp]
         L.amg_sync_changes_to_send.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, vp, C.c_size_t, vp, vp, vp]
-        L.amg_last_sync_ms.restype = C.c_float
-        L.amg_last_sync_ms.argtypes = [vp]
         L.amg_decode_changes.restype = C.c_int
         L.amg_decode_changes.argtypes = [vp, vp, vp, C.c_size_t, vp, vp, vp]
         L.amg_decode_history.restype = C.c_int
         L.amg_decode_history.argtypes = [vp, vp, vp]
-        L.amg_last_decode_ms.restype = C.c_float
-        L.amg_last_decode_ms.argtypes = [vp]
         L.amg_encode_changes.restype = C.c_int
         L.amg_encode_changes.argtypes = [vp, vp, C.c_size_t, vp, vp, vp, vp]
-        L.amg_last_encode_ms.restype = C.c_float
-        L.amg_last_encode_ms.argtypes = [vp]
         L.amg_get_history_patches.restype = C.c_int
         L.amg_get_history_patches.argtypes = [vp, vp, C.c_size_t, vp, vp]
-        L.amg_last_history_ms.restype = C.c_float
-        L.amg_last_history_ms.argtypes = [vp]
         L.amg_merge.restype = C.c_int
         L.amg_merge.argtypes = [vp, vp, C.c_int, vp, vp]
-        L.amg_last_merge_ms.restype = C.c_float
-        L.amg_last_merge_ms.argtypes = [vp]
+        for name in ('amg_last_sync_ms', 'amg_last_decode_ms', 'amg_last_encode_ms', 'amg_last_history_ms', 'amg_last_merge_ms'):
+            getattr(L, name).restype = C.c_float
+            getattr(L, name).argtypes = [vp]
 
     def check(self, rc, err):
         if rc != 0:
             msg = err.msg.decode('utf-8', 'replace')
             raise (Unsupported if rc == 4 else AmgError)(rc, msg)
+
+    def check_indexed(self, rc, err, failed):
+        """check() for a call over a batch of changes: the error carries `.failed_index`, the change it names"""
+        try:
+            self.check(rc, err)
+        except AmgError as e:
+            e.failed_index = failed.value
+            raise
+
+
+def _as_buffer(blob):
+    """bytes / bytearray (copied), a numpy array, or a ctypes pointer / address (e.g. pinned host or device memory) as a
+    pointer argument"""
+    if isinstance(blob, (bytes, bytearray)):
+        return (C.c_uint8 * max(len(blob), 1)).from_buffer_copy(bytes(blob) if len(blob) else b'\0')   # (an empty list of changes is legal)
+    if isinstance(blob, np.ndarray):
+        return blob.ctypes.data_as(C.c_void_p)
+    return blob
 
 
 _default = None
@@ -529,13 +540,7 @@ class GpuBackendDoc:
 
     def apply_packed_flat(self, blob, offs, n, is_local=False, want_patch=True):
         pp, err = C.c_void_p(), _ErrStruct()
-        if isinstance(blob, (bytes, bytearray)):
-            buf = (C.c_uint8 * max(len(blob), 1)).from_buffer_copy(bytes(blob) if len(blob) else b'\0')   # (an empty list of changes is legal)
-        elif isinstance(blob, np.ndarray):
-            buf = blob.ctypes.data_as(C.c_void_p)
-        else:
-            buf = blob   # a ctypes pointer / address (e.g. pinned host memory)
-        rc = self._lib.L.amg_apply_changes_packed(self.h, buf, offs.ctypes.data_as(C.c_void_p), C.c_size_t(n), int(is_local), int(want_patch),
+        rc = self._lib.L.amg_apply_changes_packed(self.h, _as_buffer(blob), offs.ctypes.data_as(C.c_void_p), C.c_size_t(n), int(is_local), int(want_patch),
                                                   C.byref(pp), C.byref(err))
         self._lib.check(rc, err)
         return self._take_patch(pp) if want_patch else None
@@ -672,20 +677,10 @@ class GpuBackendDoc:
     def decode_packed_flat(self, blob, offs, n):
         """amg_decode_changes over change i = blob[offs[i]:offs[i+1]] (bytes, a numpy array, or a pointer to pinned or device
         memory). Raises AmgError with `.failed_index` = the change the reference fails on first."""
-        if isinstance(blob, (bytes, bytearray)):
-            buf = (C.c_uint8 * max(len(blob), 1)).from_buffer_copy(bytes(blob) if len(blob) else b'\0')
-        elif isinstance(blob, np.ndarray):
-            buf = blob.ctypes.data_as(C.c_void_p)
-        else:
-            buf = blob
         offs = np.ascontiguousarray(offs, dtype=np.uint64)
         bl, failed, err = C.c_void_p(), C.c_size_t(), _ErrStruct()
-        rc = self._lib.L.amg_decode_changes(self.h, buf, offs.ctypes.data_as(C.c_void_p), C.c_size_t(n), C.byref(bl), C.byref(failed), C.byref(err))
-        try:
-            self._lib.check(rc, err)
-        except AmgError as e:
-            e.failed_index = failed.value
-            raise
+        rc = self._lib.L.amg_decode_changes(self.h, _as_buffer(blob), offs.ctypes.data_as(C.c_void_p), C.c_size_t(n), C.byref(bl), C.byref(failed), C.byref(err))
+        self._lib.check_indexed(rc, err, failed)
         return FlatChanges(self._buffers(bl)[0])
 
     def decode_changes_flat(self, changes):
@@ -724,11 +719,7 @@ class GpuBackendDoc:
             n, buf = int(length), C.c_void_p(int(table))
         bc, bh, failed, err = C.c_void_p(), C.c_void_p(), C.c_size_t(), _ErrStruct()
         rc = self._lib.L.amg_encode_changes(self.h, buf, C.c_size_t(n), C.byref(bc), C.byref(bh), C.byref(failed), C.byref(err))
-        try:
-            self._lib.check(rc, err)
-        except AmgError as e:
-            e.failed_index = failed.value
-            raise
+        self._lib.check_indexed(rc, err, failed)
         hx = self._buffers(bh)[0].hex()
         return self._buffers(bc), [hx[i:i + 64] for i in range(0, len(hx), 64)]
 

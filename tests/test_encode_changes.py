@@ -1,9 +1,7 @@
 """encodeChange on the device (GpuBackendDoc.encode_flat over a change table, csrc/encchg.cuh) against the host mirror
 columnar.encode_change: the same bytes and hashes, the same failing change. CPU run on the serial emulation build, GPU run on
 libamgpu.so."""
-import os
 import random
-import subprocess
 
 import numpy as np
 import pytest
@@ -11,28 +9,8 @@ import pytest
 import parity_checks
 import test_codec_vectors as V
 import test_decode_changes as TD
+from doc_fixtures import emu_doc, gpu_doc  # noqa: F401
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-@pytest.fixture(scope='module')
-def emu_doc():
-    subprocess.check_call([os.path.join(HERE, '_emu', 'build.sh')])
-    from automerge_classic_b200 import build
-    build.build_tracegen()
-    from automerge_classic_b200.engine import doc_class_for
-    return doc_class_for(os.path.join(HERE, '_emu', 'libamgpu_emu.so'))
-
-
-@pytest.fixture(scope='module')
-def gpu_doc():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip('no CUDA device')
-    from automerge_classic_b200 import build
-    build.build_all()
-    from automerge_classic_b200.engine import GpuBackendDoc
-    return GpuBackendDoc
 
 
 def _mirror(changes):

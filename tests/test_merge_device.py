@@ -2,37 +2,15 @@
 applied straight from the other document's arena, equal the host route applyChanges(local, getChangesAdded(local, remote))
 byte for byte, and the oracle running the reference's recipe (src/automerge.js:61-67). CPU run on the serial emulation
 build, GPU run on libamgpu.so."""
-import os
 import random
-import subprocess
 
 import pytest
 
 import replay
 from test_decode_changes import _deflate
+from doc_fixtures import emu_doc, gpu_doc  # noqa: F401
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 TRACES = [('C1', 0, 0), ('C2', 300, 0), ('C2b', 700, 0), ('C3', 600, 5), ('C4', 1500, 4), ('C6', 300, 3), ('C7', 300, 3), ('C8', 300, 3)]
-
-
-@pytest.fixture(scope='module')
-def emu_doc():
-    subprocess.check_call([os.path.join(HERE, '_emu', 'build.sh')])
-    from automerge_classic_b200 import build
-    build.build_tracegen()
-    from automerge_classic_b200.engine import doc_class_for
-    return doc_class_for(os.path.join(HERE, '_emu', 'libamgpu_emu.so'))
-
-
-@pytest.fixture(scope='module')
-def gpu_doc():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip('no CUDA device')
-    from automerge_classic_b200 import build
-    build.build_all()
-    from automerge_classic_b200.engine import GpuBackendDoc
-    return GpuBackendDoc
 
 
 # ---- documents from recipes, built the same way for the engine and the oracle

@@ -1,36 +1,14 @@
 """The sync protocol's per-change work in the engine (GpuBackendDoc.sync_bloom / sync_changes_to_send, csrc/sync.cuh) against
 the host implementation in automerge_classic_b200/sync.py: the same Bloom filter bytes, the same changes in the same order.
 CPU run on the serial emulation build, GPU run on libamgpu.so."""
-import os
 import random
-import subprocess
 
 import pytest
 
 import parity_checks
+from doc_fixtures import emu_doc, gpu_doc  # noqa: F401
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 CONFIGS = [('C3', 400, 4), ('C4', 3000, 5), ('C6', 200, 3), ('C8', 300, 4)]
-
-
-@pytest.fixture(scope='module')
-def emu_doc():
-    subprocess.check_call([os.path.join(HERE, '_emu', 'build.sh')])
-    from automerge_classic_b200 import build
-    build.build_tracegen()
-    from automerge_classic_b200.engine import doc_class_for
-    return doc_class_for(os.path.join(HERE, '_emu', 'libamgpu_emu.so'))
-
-
-@pytest.fixture(scope='module')
-def gpu_doc():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip('no CUDA device')
-    from automerge_classic_b200 import build
-    build.build_all()
-    from automerge_classic_b200.engine import GpuBackendDoc
-    return GpuBackendDoc
 
 
 def _hash(change):
