@@ -277,6 +277,20 @@ napi_value Merge(napi_env env, napi_callback_info info) {
   }
   return patchToJs(env, patch);
 }
+// applyLocalChangeTable(state, table) — backend/backend.js:54-91 applyLocalChange with the change request given as a change
+// table (layout: amgpu.h) holding one change: encoded with the author's previous change hash added to its deps and applied
+// on the device (amg_apply_local_change). Returns [patch, change]: the flat patch without the new change's hash in its deps,
+// and the binary change as encodeChange returns it.
+napi_value ApplyLocalChangeTable(napi_env env, napi_callback_info info) {
+  napi_value argv[2]; amg_backend* b; if (!getArgs(env, info, 2, argv) || !getBackend(env, argv[0], &b)) return nullptr;
+  const uint8_t* p; size_t len; if (!getBytes(env, argv[1], &p, &len)) return nullptr;
+  amg_patch* patch = nullptr; amg_buffers* change = nullptr; amg_error err;
+  if (amg_apply_local_change(b, p, len, 1, &patch, &change, &err)) return throwAmg(env, err);
+  napi_value out, ch; napi_create_array_with_length(env, 2, &out);
+  napi_get_element(env, buffersToJs(env, change), 0, &ch);
+  napi_set_element(env, out, 0, patchToJs(env, patch)); napi_set_element(env, out, 1, ch);
+  return out;
+}
 // Backend.free — backend/backend.js:16-19: releases the device memory now instead of at garbage collection
 napi_value Free(napi_env env, napi_callback_info info) {
   napi_value argv[1]; Holder* h; if (!getArgs(env, info, 1, argv) || !getHolder(env, argv[0], &h)) return nullptr;
@@ -290,7 +304,8 @@ napi_value InitModule(napi_env env, napi_value exports) {
     {"getHeads", GetHeads}, {"getChanges", GetChanges}, {"getChangesAdded", GetChangesAdded}, {"getChangeByHash", GetChangeByHash},
     {"getMissingDeps", GetMissingDeps}, {"clockOf", ClockOf}, {"hashByActor", HashByActor}, {"syncBloom", SyncBloom},
     {"syncChangesToSend", SyncChangesToSend}, {"decodeChanges", DecodeChanges}, {"decodeHistory", DecodeHistory},
-    {"encodeChanges", EncodeChanges}, {"historyPatches", HistoryPatches}, {"merge", Merge}};
+    {"encodeChanges", EncodeChanges}, {"historyPatches", HistoryPatches}, {"merge", Merge},
+    {"applyLocalChangeTable", ApplyLocalChangeTable}};
   for (auto& f : fns) { napi_value fn; napi_create_function(env, f.name, NAPI_AUTO_LENGTH, f.fn, nullptr, &fn); napi_set_named_property(env, exports, f.name, fn); }
   return exports;
 }

@@ -12,6 +12,7 @@ Handles are `{'state': doc, 'heads': [...], 'frozen': bool}` dicts exactly like 
 `{state, heads, frozen}` objects (backend/backend.js:9, 27-32; backend/util.js:1-10).
 """
 from .columnar import encode_change
+from .engine import AmgError, Unsupported
 
 
 class RangeError(Exception):
@@ -65,11 +66,33 @@ class Backend:
             return h
         raise RangeError('Unknown change: actorId = %s, seq = %d' % (actor_id, index + 1))
 
-    # backend.js:54-91
+    # backend.js:54-91. A document class with apply_local_change encodes and applies the change on the device; the checks
+    # that come before the encoder in the reference run here first, from the clock, so that their errors win. The host
+    # route below remains for other document classes and for a request the engine declines (Unsupported).
     def applyLocalChange(self, backend, change):
         state = backend_state(backend)
-        if change['seq'] <= state.clock().get(change['actor'], 0):
+        local = getattr(state, 'apply_local_change', None)
+        clock = state.clock_of(change['actor']) if local else state.clock().get(change['actor'], 0)
+        if change['seq'] <= clock:
             raise RangeError('Change request has already been applied')
+        if local:
+            if change['seq'] - 1 > clock:
+                raise RangeError('Unknown change: actorId = %s, seq = %d' % (change['actor'], change['seq'] - 1))
+            try:
+                patch, binary_change = local(change)
+            except Unsupported:
+                pass   # nothing changed: the host route
+            except AmgError as e:
+                # The seq checks above ran already, so "Unknown change" here means the change was applied to the queue
+                # (its deps are not all applied) and has no hash yet. The reference raises this after its apply too
+                # (backend.js:84-85), with the handle frozen.
+                if not str(e).startswith('Unknown change: '):
+                    raise
+                backend['frozen'] = True
+                raise RangeError(str(e)) from None
+            else:
+                backend['frozen'] = True
+                return [{'state': state, 'heads': state.heads()}, patch, binary_change]
         change = dict(change)
         if change['seq'] > 1:
             last_hash = self._hash_by_actor(state, change['actor'], change['seq'] - 2)

@@ -160,6 +160,7 @@ amg_backend* amg_clone(amg_backend* src, amg_error* err) {
     d.numApplied = s.numApplied; d.hashes.ensure(c, s.numApplied * 32 + 64); d2d(c, d.hashes.p, s.hashes.p, s.numApplied * 32);
     d.numRows = s.numRows; d.doc.copyFrom(c, s.doc, s.numRows);
     d.numSucc = s.numSucc; d.succOff.ensure(c, s.numRows + 2); d2d(c, d.succOff.p, s.succOff.p, (s.numRows + 1) * 4); d.succ.ensure(c, s.numSucc + 1); d2d(c, d.succ.p, s.succ.p, s.numSucc * 8);
+    d.lastChange.ensure(c, s.st.actorIds.size() + 1); d2d(c, d.lastChange.p, s.lastChange.p, s.st.actorIds.size() * 4);
     d.st = s.st; d.changes = s.changes; d.deflatedOriginal = s.deflatedOriginal; d.deflateOnExport = s.deflateOnExport; d.loaded = s.loaded;
     d.unknownCols = s.unknownCols; d.queue = s.queue; d.queueOriginal = s.queueOriginal;
     while (d.actorCap < 2 * (d.st.actorIds.size() + 16)) d.actorCap *= 2;
@@ -306,6 +307,15 @@ int amg_merge(amg_backend* dst, amg_backend* src, int want_patch, amg_patch** ou
             if (out) *out = want_patch ? serialize(p) : nullptr; return 0;)
 }
 float amg_last_merge_ms(amg_backend* b) { return b->eng.spans.ms[SPAN_MERGE]; }
+// backend/backend.js:54-91 applyLocalChange: encoded and applied on the device; the returned change DEFLATEd here when
+// 256 bytes or more (columnar.js:738), as amg_encode_changes returns it
+int amg_apply_local_change(amg_backend* b, const uint8_t* table, size_t table_len, int want_patch, amg_patch** out, amg_buffers** out_change, amg_error* err) {
+  AMG_GUARD(PatchOut p; std::string plain; b->eng.applyLocalChange(table, table_len, want_patch != 0, p, plain);
+            auto lc = buffers([&](Items& l) { l.push_back(plain.size() >= 256 ? amg_backend::deflateChange(plain) : plain); });
+            if (out) *out = want_patch ? serialize(p) : nullptr;
+            *out_change = lc.release(); return 0;)
+}
+float amg_last_local_ms(amg_backend* b) { return b->eng.spans.ms[SPAN_LOCAL]; }
 int amg_get_change_by_hash(amg_backend* b, const uint8_t hash[32], amg_buffers** out, amg_error* err) {
   AMG_GUARD(b->ensureGraph(); auto it = b->g.indexByHash.find(toHash(hash));
             *out = buffers([&](Items& l) { if (it != b->g.indexByHash.end()) l.push_back(b->changeBytes(it->second)); }).release(); return 0;)

@@ -43,8 +43,26 @@ static const u64 ENC_OP_BOUND = 9 * 20 + 10 + 10, ENC_PRED_BOUND = 40, ENC_CHANG
 // the staged table (sections checked by the host: inside the table, 8-byte aligned)
 struct EncTable {
   const u8* t; u64 len; u64 nOps, nPreds, nActors; const ChangeRec* ch; const OpRec* ops; const u32* preds; const ActorRef* actors;
+  // applyLocalChange: the author's previous change, hashes + 32 * *prevIdx, is one more dependency of every change of the
+  // call; the deps are then the sorted union without repeats (backend.js:76-79). prevIdx == nullptr: no extra dependency.
+  const u8* prevHashes = nullptr; const u32* prevIdx = nullptr;
   HD bool inside(u64 off, u64 n) const { return off <= len && n <= len - off; }
+  HD const u8* dep(const ChangeRec& r, u32 i) const { return t + r.depsOff + 32ULL * i; }
+  HD const u8* extraDep() const { return prevIdx ? prevHashes + 32ULL * *prevIdx : nullptr; }
 };
+HD bool enc_same_hash(const u8* a, const u8* b) { for (int k = 0; k < 32; k++) if (a[k] != b[k]) return false; return true; }
+// the number of dependencies the header lists (the deps section is in range)
+HD u32 enc_num_deps(const EncTable& T, const ChangeRec& r) {
+  const u8* x = T.extraDep();
+  if (!x) return r.nDeps;
+  u32 n = 1;
+  for (u32 i = 0; i < r.nDeps; i++) {
+    bool seen = enc_same_hash(T.dep(r, i), x);
+    for (u32 j = 0; j < i && !seen; j++) seen = enc_same_hash(T.dep(r, i), T.dep(r, j));
+    if (!seen) n++;
+  }
+  return n;
+}
 HD bool enc_set_or_inc(u32 action) { return action == 1 || action == 5; }   // encodeValue writes a value for these only (columnar.js:260)
 HD bool enc_map_key(const OpRec& o) { return o.keyStrLen != NULL32 && o.keyStrLen > 0; }
 HD bool enc_elem_key(const OpRec& o) { return !enc_map_key(o) && o.keyCtr != NULL32 && o.keyCtr > 0; }
@@ -72,7 +90,7 @@ struct EncChangeKernel {
     if (r.hasExtra && !T.inside(r.extraOff, r.extraLen)) { fail(c, EE_CHG_EXTRA); return; }
     if (r.seq > ENC_MAX_SAFE || r.startOp > ENC_MAX_SAFE || r.time > (long long)ENC_MAX_SAFE || r.time < -(long long)ENC_MAX_SAFE) { fail(c, EE_NUM_RANGE); return; }
     u64 preds = 0;
-    bound += 10 + (u64)r.msgLen + 32ULL * r.nDeps + (r.hasExtra ? (u64)r.extraLen : 0);
+    bound += 10 + (u64)r.msgLen + 32ULL * ((u64)r.nDeps + (T.prevIdx ? 1 : 0)) + (r.hasExtra ? (u64)r.extraLen : 0);
     for (u64 i = 0; i < r.nOps; i++) {   // (fields the op checks have not seen yet only make the bound larger)
       const OpRec& o = T.ops[r.firstOp + i];
       preds += o.predNum;
@@ -271,7 +289,7 @@ struct EncChangeHeadKernel {
     const ChangeRec& r = T.ch[c]; u32 len[HC_NUM]; u32 dataLen = 0;
     for (int col = 0; col < HC_NUM; col++) { len[col] = colLen[(size_t)col * n + c]; dataLen += len[col]; }
     const u32 a0 = actorBase[c];
-    const ChangeHead h{r.nDeps, T.t + entOff[a0], entLen[a0], r.seq, r.startOp, r.time, T.t + r.msgOff, r.msgLen};
+    const ChangeHead h{enc_num_deps(T, r), T.t + entOff[a0], entLen[a0], r.seq, r.startOp, r.time, T.t + r.msgOff, r.msgLen};
     const EncOthers others{other + otherStart[c], otherStart[c + 1] - otherStart[c], rep, entOff, entLen, T.t};
     const u32 extra = r.hasExtra ? r.extraLen : 0;
     ByteSink w{pass ? out + outOff[c] : nullptr, 0};
@@ -295,12 +313,15 @@ struct EncColWriteKernel {
 struct EncHashKernel {
   EncTable T; const u64* outOff; const u32* outLen; const u64* depsAt; const u64* bodyAt; u8* out; u8* hashes;
   HD void operator()(size_t c) const {
-    const ChangeRec& r = T.ch[c]; u8* dst = out + depsAt[c];
-    for (u32 i = 0; i < r.nDeps; i++) {   // insertion sort by hash bytes (columnar.js:717; deps are few)
-      const u8* h = T.t + r.depsOff + 32 * (u64)i; u32 pos = i;
+    const ChangeRec& r = T.ch[c]; u8* dst = out + depsAt[c]; const u8* x = T.extraDep(); u32 n = 0;
+    auto put = [&](const u8* h) {   // insertion sort by hash bytes (columnar.js:717; deps are few); with x, repeats are dropped
+      if (x) for (u32 k = 0; k < n; k++) if (enc_same_hash(dst + 32 * k, h)) return;
+      u32 pos = n++;
       while (pos > 0) { const u8* prev = dst + 32 * (pos - 1); int cmp = 0; for (int b = 0; b < 32 && !cmp; b++) cmp = (int)prev[b] - (int)h[b]; if (cmp <= 0) break; for (int b = 0; b < 32; b++) dst[32 * pos + b] = prev[b]; pos--; }
       for (int b = 0; b < 32; b++) dst[32 * pos + b] = h[b];
-    }
+    };
+    for (u32 i = 0; i < r.nDeps; i++) put(T.dep(r, i));
+    if (x) put(x);
     u8 digest[32]; hist_sha256(out + bodyAt[c], (u32)(outOff[c] + outLen[c] - bodyAt[c]), digest);
     for (int b = 0; b < 32; b++) hashes[c * 32 + b] = digest[b];
     for (int b = 0; b < 4; b++) out[outOff[c] + 4 + b] = digest[b];

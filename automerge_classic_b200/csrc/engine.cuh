@@ -97,7 +97,7 @@ struct Trace {
 // Device span of the last call of each entry point kind (amg_last_*_ms): CUDA events on the main stream around the call's
 // uploads, kernels and read-backs; 0 in the emulation build. start(k) zeroes k's slot and opens the span, resume(k) opens
 // it without zeroing, stop() adds the span to the slot. A call that throws never reaches stop(): its slot stays 0.
-enum SpanKind { SPAN_SYNC, SPAN_DECODE, SPAN_ENCODE, SPAN_HISTORY, SPAN_MERGE, NUM_SPANS };
+enum SpanKind { SPAN_SYNC, SPAN_DECODE, SPAN_ENCODE, SPAN_HISTORY, SPAN_MERGE, SPAN_LOCAL, NUM_SPANS };
 struct DeviceSpans {
   float ms[NUM_SPANS] = {0};
   explicit DeviceSpans(Ctx& c) : ctx(c) {}
@@ -173,6 +173,9 @@ class Engine {
   DocBufs doc; size_t numRows = 0; DBuf<u32> succOff; DBuf<u64> succ; size_t numSucc = 0;
   DBuf<ActorSlot> actorSlots; size_t actorCap = 0;
   DBuf<u32> actorRank;
+  // application index of each actor's last applied change (by document actor number; set by commit, load and clone).
+  // commit() swaps in lastChangeNext, which the sequence check of the call filled.
+  DBuf<u32> lastChange, lastChangeNext;
   // ---- persistent host state
   DocState st;
   std::vector<HostChange> changes;     // applied, in application order
@@ -193,7 +196,7 @@ class Engine {
   }
   Trace trace{ctx};
   HBuf<u8> patchBuf;   // pinned: patch records are copied device -> host directly into their final place
-  DeviceSpans spans{ctx};   // sync, decode, encode, history and merge calls
+  DeviceSpans spans{ctx};   // sync, decode, encode, history, merge and local-change calls
   // ---- scratch (grow-only)
   DBuf<u32> chOff, chLen, nOps, nPreds, nDeps, nActors, colOff, colLen, depBase, depIdx, primary, pass, flagWord, appRank, opBase, predBase, timeBase, amapBase, amap, authorSlot, newSlots;
   DBuf<u8> applied; DBuf<ChangeHot> hot; DBuf<ChangeMeta> meta /* save(): full headers */; DBuf<u64> errWord; DBuf<u32> hashTable;
@@ -428,7 +431,7 @@ class Engine {
     std::vector<std::pair<ColInfo*, const u8*>> deflated;   // columns still DEFLATEd, and where their bytes are
     std::vector<std::string> actors; std::vector<std::array<u8, 32>> heads; std::vector<u32> headIdx;
     std::vector<std::pair<u32, u32>> reps; DocCols dc{}; size_t arenaLen = 0;   // staged in the arena
-    std::vector<u64> clock; LoadedDoc doc;   // doc: what the engine keeps once the load has succeeded
+    std::vector<u64> clock; std::vector<u32> lastChange; LoadedDoc doc;   // doc: what the engine keeps once the load has succeeded
     size_t N = 0, S = 0; u32 serialMask = ALL_DOC_COLS; bool counted = false; RawRows raw{}; u64 maxOp = 0;   // rows, succ entries
     LoadCall(const u8* b, size_t n) : buf(b), len(n), r(b, 8, (u32)n) {}
   };
@@ -538,6 +541,14 @@ class Engine {
   // Automerge.merge (src/automerge.js:61-67): those changes, gathered from src's arena into one device blob, through applyChanges
   void mergeFrom(Engine& src, bool wantPatch, PatchOut& out);
   DBuf<u32> mergeAbsent, mergeSlot, mergeList, mergeHeadIdx; DBuf<u8> mergeHeads, mergeBlob; DBuf<MergeRange> mergeRanges;
+
+  // ---------------------------------------------------------------- applyLocalChange (backend.js:54-91)
+  // One change request (a change table holding one change) encoded on the device with the author's previous change hash as
+  // one more dependency, and applied from device memory (isLocal). out: the patch without the new change's hash in its
+  // deps; binary: the plain change (the caller DEFLATEs one of 256 bytes or more). A change of 256 bytes or more is marked
+  // to go out DEFLATEd (deflateOnExport). Errors leave the document unchanged, except "Unknown change" when the change
+  // waits in the queue after the apply, which the reference also raises after the apply.
+  void applyLocalChange(const u8* table, size_t len, bool wantPatch, PatchOut& out, std::string& binary);
  private:
   void uploadCandidates(const u32* idx, size_t count);
 };

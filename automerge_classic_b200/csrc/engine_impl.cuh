@@ -478,7 +478,8 @@ inline void Engine::checkSequence(ApplyCall& a) {
   DBuf<u64>& clockDev = pairKey;   // scratch reuse before the succ phase
   clockDev.ensure(ctx, A + 1); h2d(ctx, clockDev.p, a.now.clock.data(), A * 8);
   dev_memset(ctx, seqSlot.p, 0xff, (a.numNew + 1) * 4); dev_memset(ctx, flagWord.p, 0, 4);
-  foreach(ctx, B, SeqScatterKernel{hot.p, applied.p, changeActor.p, appRank.p, actorBaseD.p, actorCnt.p, clockDev.p, seqSlot.p, flagWord.p});
+  lastChangeNext.ensure(ctx, A + 1); d2d(ctx, lastChangeNext.p, lastChange.p, st.actorIds.size() * 4);   // commit() swaps it in
+  foreach(ctx, B, SeqScatterKernel{hot.p, applied.p, changeActor.p, appRank.p, actorBaseD.p, actorCnt.p, clockDev.p, seqSlot.p, flagWord.p, lastChangeNext.p, (u32)numApplied});
   foreach(ctx, B, SeqMonoKernel{hot.p, applied.p, changeActor.p, actorBaseD.p, actorCnt.p, clockDev.p, seqSlot.p, flagWord.p});
   std::vector<u32> actorCntH(A); d2h(ctx, actorCntH.data(), actorCnt.p, A * 4);
   if (readU32(flagWord.p)) throwSequenceError(a);
@@ -745,7 +746,7 @@ inline void Engine::commit(ApplyCall& a) {
       }
     }
     trace.mark("commit:changes-recorded");
-    doc.swap(sorted); numRows = a.N;
+    doc.swap(sorted); numRows = a.N; lastChange.swap(lastChangeNext);
     succOff.swap(newSuccOff); succ.swap(newSucc); numSucc = a.numPairs;
     fill32(doc.time.p, 0, a.N);
     for (auto& kv : a.unknownRows) unknownCols.byOp[kv.first] = std::move(kv.second);
@@ -1697,18 +1698,19 @@ inline void Engine::stageColumns(LoadCall& l) {
 // of every head.
 inline void Engine::loadClock(LoadCall& l) {
   const std::vector<std::string>& actors = l.actors;
-  l.clock.assign(actors.size(), 0);
+  l.clock.assign(actors.size(), 0); l.lastChange.assign(actors.size(), EMPTY32);
   bool onDevice = false; const HostChange ac = l.doc.cols[CC_ACTOR], sc = l.doc.cols[CC_SEQ]; u32 total = 0;
   if (ac.len >= parDocMinRows / 8 + 16 && sc.len > 0 && parCols.rleRecords(arena.p + ac.off, ac.len, &total) && total >= parDocMinRows) {
     const size_t n = total; DBuf<long long> aV, sV; aV.ensure(ctx, n + 1); sV.ensure(ctx, n + 1);
     if (parCols.toI64(arena.p + ac.off, ac.len, false, n, aV.p) && parCols.deltaToI64(arena.p + sc.off, sc.len, n, sV.p)) {
       sortKeys.ensure(ctx, n + 1); sortVals.ensure(ctx, n + 1); DBuf<u64> clkD; clkD.ensure(ctx, actors.size() + 1); dev_memset(ctx, clkD.p, 0, (actors.size() + 1) * 8);
+      DBuf<u32> lastD; lastD.ensure(ctx, actors.size() + 1); dev_memset(ctx, lastD.p, 0xff, (actors.size() + 1) * 4);
       dev_memset(ctx, flagWord.p, 0, 16);
       foreach(ctx, n, ClockKeyKernel{aV.p, (u32)actors.size(), sortKeys.p, sortVals.p, flagWord.p});
       sortPairs(sortKeys, sortVals, n, bits_for(actors.size() > 1 ? actors.size() - 1 : 1));
-      foreach(ctx, n, ClockCheckKernel{sortKeys.p, sortVals.p, sV.p, (u32)n, clkD.p, flagWord.p});
-      u32 bad = 0; d2h(ctx, &bad, flagWord.p, 4); if (!actors.empty()) d2h(ctx, l.clock.data(), clkD.p, actors.size() * 8); sync(ctx);
-      if (!bad) { onDevice = true; l.doc.numChanges = n; } else std::fill(l.clock.begin(), l.clock.end(), 0);
+      foreach(ctx, n, ClockCheckKernel{sortKeys.p, sortVals.p, sV.p, (u32)n, clkD.p, flagWord.p, lastD.p});
+      u32 bad = 0; d2h(ctx, &bad, flagWord.p, 4); if (!actors.empty()) { d2h(ctx, l.clock.data(), clkD.p, actors.size() * 8); d2h(ctx, l.lastChange.data(), lastD.p, actors.size() * 4); } sync(ctx);
+      if (!bad) { onDevice = true; l.doc.numChanges = n; } else { std::fill(l.clock.begin(), l.clock.end(), 0); std::fill(l.lastChange.begin(), l.lastChange.end(), EMPTY32); }
     }
   }
   if (!onDevice) {
@@ -1720,7 +1722,7 @@ inline void Engine::loadClock(LoadCall& l) {
       if (sn) seqAcc += d;
       const u64 seq = sn ? (u64)seqAcc : 0;
       if (seq != 1 && seq != l.clock[a] + 1) throw Error(AMG_ERR_RANGE, "Expected seq " + std::to_string(l.clock[a] + 1) + ", got " + std::to_string(seq) + " for actor " + hex_of((const u8*)actors[a].data(), actors[a].size()));
-      l.clock[a] = seq; l.doc.numChanges++;
+      l.clock[a] = seq; l.lastChange[a] = (u32)l.doc.numChanges++;
     }
   }
   trace.print("load", "clock", l.t0);
@@ -1837,6 +1839,7 @@ inline void Engine::commitLoad(LoadCall& l) {
   std::vector<size_t> o(hs.size()); for (size_t i = 0; i < o.size(); i++) o[i] = i; std::sort(o.begin(), o.end(), [&](size_t a, size_t b) { return hs[a] < hs[b]; });
   st = DocState{l.actors, l.reps, l.clock, l.maxOp, {}, {}}; for (size_t i : o) { st.heads.push_back(hs[i]); st.headIdx.push_back(l.headIdx[i]); }
   changes.assign(numChanges, HostChange{0, 0});
+  lastChange.ensure(ctx, st.actorIds.size() + 1); h2d(ctx, lastChange.p, l.lastChange.data(), st.actorIds.size() * 4);
   l.doc.bytes.assign((const char*)l.buf, l.len); l.doc.haveHashGraph = false; loaded = std::move(l.doc);
   trace.print("load", "host state", l.t0);
   while (actorCap < 2 * (st.actorIds.size() + 16)) actorCap *= 2;
@@ -2454,6 +2457,50 @@ inline void Engine::mergeFrom(Engine& src, bool wantPatch, PatchOut& out) {
   h2d(ctx, mergeRanges.p, ranges.data(), K * sizeof(MergeRange));
   merge_gather(ctx, K, MergeGatherKernel{src.arena.p, mergeBlob.p, mergeRanges.p});
   applyChanges(nullptr, nullptr, K, mergeBlob.p, offs.data(), false, wantPatch, out, marks.data());   // the device-blob path of amg_apply_changes_packed
+  spans.stop();
+}
+
+// ------------------------------------------------------------ applyLocalChange (backend.js:54-91)
+// The checks and the previous hash come from the engine's clock, lastChange and hashes: no host hash graph. The change
+// bytes go from the encoder's output to the apply's arena without leaving the device.
+inline void Engine::applyLocalChange(const u8* table, size_t len, bool wantPatch, PatchOut& out, std::string& binary) {
+  spans.start(SPAN_LOCAL);
+  EncodeCall e; e.len = len; encodeFailed = 0;
+  clearErr();
+  stageEncodeInput(e, table);
+  if (e.n != 1) throw Error(AMG_ERR_RANGE, "change table: applyLocalChange takes one change request, not " + std::to_string(e.n));
+  // 1. the author (actor entry 0) and seq. A record without a readable author skips the checks: validateTable reports it.
+  ChangeRec r; d2h(ctx, &r, e.T.ch, sizeof(r)); sync(ctx);
+  std::string author; bool haveAuthor = false;
+  if (r.nActors > 0 && r.actorFirst < e.T.nActors) {
+    ActorRef ar; d2h(ctx, &ar, e.T.actors + r.actorFirst, sizeof(ar)); sync(ctx);
+    if (e.T.inside(ar.off, ar.len)) { author.resize(ar.len); d2h(ctx, &author[0], e.T.t + ar.off, ar.len); sync(ctx); haveAuthor = true; }
+  }
+  auto actorNum = [&]() { return (size_t)(std::find(st.actorIds.begin(), st.actorIds.end(), author) - st.actorIds.begin()); };
+  auto unknownChange = [&](u64 seq) { return Error(AMG_ERR_RANGE, "Unknown change: actorId = " + hex_of((const u8*)author.data(), author.size()) + ", seq = " + std::to_string(seq)); };
+  if (haveAuthor) {
+    const size_t a = actorNum(); const u64 clock = a < st.actorIds.size() ? st.clock[a] : 0;
+    if (r.seq <= clock) throw Error(AMG_ERR_RANGE, "Change request has already been applied");
+    if (r.seq > 1) {   // 2. the author's change seq - 1 is its last applied change
+      if (r.seq - 1 > clock) throw unknownChange(r.seq - 1);
+      if (!loaded.haveHashGraph) {   // a loaded document knows the hashes of its heads only (new.js:1721-1725)
+        const u32 idx = readU32(lastChange.p + a);
+        if (idx < loaded.numChanges && std::find(st.headIdx.begin(), st.headIdx.end(), idx) == st.headIdx.end()) computeHashGraph();
+      }
+      e.T.prevHashes = hashes.p; e.T.prevIdx = lastChange.p + a;
+    }
+  }
+  // 3. encoded, the previous hash added to the deps by EncHashKernel
+  validateTable(e); encodeActorTables(e); encodePrep(e); encodeColumns(e); encodeHashes(e);
+  // 4. applied from device memory; a change that encodeChange returns DEFLATEd goes out DEFLATEd, as after the host route
+  const u64 offs[2] = {0, e.total}; const u8 mark[1] = {(u8)(e.total >= 256 ? 1 : 0)};
+  applyChanges(nullptr, nullptr, 1, e.out.p, offs, true, wantPatch, out, mark);
+  binary.resize(e.total); std::array<u8, 32> hash;
+  d2h(ctx, &binary[0], e.out.p, e.total); d2h(ctx, hash.data(), e.hashes.p, 32); sync(ctx);
+  { const size_t a = actorNum(); if (a == st.actorIds.size() || st.clock[a] < r.seq) throw unknownChange(r.seq); }   // it waits in the queue (backend.js:84)
+  // 5. the patch without the new change's own hash (backend.js:86-88)
+  out.deps.erase(std::remove(out.deps.begin(), out.deps.end(), hash), out.deps.end());
+  finishPatch(out);
   spans.stop();
 }
 

@@ -59,14 +59,17 @@ struct GatherNewActorsKernel {   // slot number, slot record and (up to `stride`
 struct SetActorNumKernel { ActorSlot* slots; const u32* slotIds; const u32* nums; HD void operator()(size_t i) const { slots[slotIds[i]].actorNum = nums[i]; } };
 struct ChangeActorKernel { const u32* amapBase; const u32* amap; const u8* applied; u32* changeActor; u32* actorCnt; HD void operator()(size_t b) const { if (!applied[b]) { changeActor[b] = EMPTY32; return; } const u32 a = amap[amapBase[b]]; changeActor[b] = a; warp_agg_inc(actorCnt, a); } };
 // seq == clock + 1 in application order (new.js:1559, 1571-1579): the seqs of an actor's applied changes must be
-// exactly clock+1 .. clock+count, in increasing application order
+// exactly clock+1 .. clock+count, in increasing application order. The change with seq clock+count becomes the actor's
+// last applied change: lastChange[a] = its application index (applyLocalChange reads its hash from there).
 struct SeqScatterKernel {
   const ChangeHot* meta; const u8* applied; const u32* changeActor; const u32* appRank; const u32* actorBase; const u32* actorCnt; const u64* clock; u32* seqSlot; u32* bad;
+  u32* lastChange; u32 numApplied;
   HD void operator()(size_t b) const {
     if (!applied[b]) return;
     const u32 a = changeActor[b]; const u64 seq = meta[b].seq, c0 = clock[a];
     if (seq <= c0 || seq - c0 - 1 >= actorCnt[a]) { *bad = 1; return; }
     if (atomic_cas(&seqSlot[actorBase[a] + (u32)(seq - c0 - 1)], EMPTY32, appRank[b]) != EMPTY32) *bad = 1;
+    if (seq - c0 == actorCnt[a]) lastChange[a] = numApplied + appRank[b];
   }
 };
 struct SeqMonoKernel {
@@ -160,14 +163,14 @@ struct DocKeyStrExpandKernel {
 // clock of a long loaded document (new.js:1645-1675 readDocumentChanges): changes sorted by actor (stable), every change
 // compared with the same actor's previous one
 struct ClockKeyKernel { const long long* actor; u32 numActors; u64* key; u32* val; u32* bad; HD void operator()(size_t i) const { const long long a = actor[i]; if (a == NULLV || a < 0 || (u64)a >= numActors) { *bad = 1; key[i] = 0; } else key[i] = (u64)a; val[i] = (u32)i; } };
-struct ClockCheckKernel {
-  const u64* key; const u32* val; const long long* seq; u32 n; u64* clock; u32* bad;
+struct ClockCheckKernel {   // (lastChange: the index of each actor's last change)
+  const u64* key; const u32* val; const long long* seq; u32 n; u64* clock; u32* bad; u32* lastChange;
   HD void operator()(size_t j) const {
     const u32 i = val[j]; const long long s = seq[i] == NULLV ? 0 : seq[i];
     const bool havePrev = j > 0 && key[j - 1] == key[j];
     const long long ps = havePrev ? (seq[val[j - 1]] == NULLV ? 0 : seq[val[j - 1]]) : 0;
     if (!(s == 1 || (havePrev && s == ps + 1)) || s < 0) *bad = 1;
-    if (j + 1 == n || key[j + 1] != key[j]) clock[key[j]] = (u64)s;
+    if (j + 1 == n || key[j + 1] != key[j]) { clock[key[j]] = (u64)s; lastChange[key[j]] = i; }
   }
 };
 struct DocAbsentKernel {   // fill_absent_column for a long document, one thread per row (col as in DocColumnKernel, rows from doc_col_rows)

@@ -90,7 +90,10 @@ class Library:
         L.amg_get_history_patches.argtypes = [vp, vp, C.c_size_t, vp, vp]
         L.amg_merge.restype = C.c_int
         L.amg_merge.argtypes = [vp, vp, C.c_int, vp, vp]
-        for name in ('amg_last_sync_ms', 'amg_last_decode_ms', 'amg_last_encode_ms', 'amg_last_history_ms', 'amg_last_merge_ms'):
+        L.amg_apply_local_change.restype = C.c_int
+        L.amg_apply_local_change.argtypes = [vp, vp, C.c_size_t, C.c_int, vp, vp, vp]
+        L.amg_clock_of.argtypes = [vp, vp, C.c_size_t, vp, vp]
+        for name in ('amg_last_sync_ms', 'amg_last_decode_ms', 'amg_last_encode_ms', 'amg_last_history_ms', 'amg_last_merge_ms', 'amg_last_local_ms'):
             getattr(L, name).restype = C.c_float
             getattr(L, name).argtypes = [vp]
 
@@ -596,6 +599,13 @@ class GpuBackendDoc:
         self._lib.check(fn(self.h, C.byref(bl), C.byref(err)), err)
         return self._buffers(bl)[0]
 
+    def clock_of(self, actor):
+        """clock[actor] (0 for an actor the document has not seen), without building the whole clock"""
+        a = bytes.fromhex(actor)
+        seq, err = C.c_uint64(), _ErrStruct()
+        self._lib.check(self._lib.L.amg_clock_of(self.h, a, C.c_size_t(len(a)), C.byref(seq), C.byref(err)), err)
+        return seq.value
+
     def hash_by_actor(self, actor, index):
         a = bytes.fromhex(actor)
         out, found, err = (C.c_uint8 * 32)(), C.c_int(), _ErrStruct()
@@ -629,6 +639,27 @@ class GpuBackendDoc:
     def last_merge_ms(self):
         """Device span of the last merge_flat call (CUDA events), ms."""
         return float(self._lib.L.amg_last_merge_ms(self.h))
+
+    # ---- applyLocalChange (backend.js:54-91), on the device
+    def apply_local_change_flat(self, change, want_patch=True):
+        """amg_apply_local_change: the change request (a change dict, as encode_change takes it) encoded with the author's
+        previous change hash added to its deps, and applied. Returns (FlatPatch without the new change's hash in its deps,
+        or None with want_patch=False; the binary change as encodeChange returns it). Raises Unsupported before anything
+        changed for a request the change table cannot hold (a counter of 2^32 or more)."""
+        table = FlatChanges.from_changes([change]).raw
+        pp, bl, err = C.c_void_p(), C.c_void_p(), _ErrStruct()
+        self._lib.check(self._lib.L.amg_apply_local_change(self.h, C.cast(C.c_char_p(table), C.c_void_p), C.c_size_t(len(table)), int(want_patch),
+                                                           C.byref(pp), C.byref(bl), C.byref(err)), err)
+        return (self._take_patch(pp) if want_patch else None), self._buffers(bl)[0]
+
+    def apply_local_change(self, change):
+        """apply_local_change_flat with the patch as the dict applyChanges returns."""
+        fp, binary = self.apply_local_change_flat(change)
+        return fp.to_patch(False), binary
+
+    def last_local_ms(self):
+        """Device span of the last apply_local_change_flat call (CUDA events), ms."""
+        return float(self._lib.L.amg_last_local_ms(self.h))
 
     def get_change_by_hash(self, hash_):
         bl, err = C.c_void_p(), _ErrStruct()

@@ -93,6 +93,25 @@ float amg_last_merge_ms(amg_backend* dst);
 int amg_get_change_by_hash(amg_backend* b, const uint8_t hash[32], amg_buffers** out, amg_error* err);
 /* Backend.getMissingDeps — backend.js:190-192 -> new.js:2014-2028: hashes of 32 bytes */
 int amg_get_missing_deps(amg_backend* b, const uint8_t* heads, size_t n, amg_buffers** out, amg_error* err);
+/* backend/backend.js:54-91 applyLocalChange. `table`: a change table (amg_decode_changes layout) holding one change request;
+ * pinned, pageable or device memory. *out: the patch applyChanges(isLocal) returns, without the new change's hash in its deps
+ * (want_patch == 0: none). *out_change: one buffer, the binary change as encodeChange returns it.
+ *   - The author is actor entry 0 of the change. seq <= clock[author]: AMG_RANGE_ERROR "Change request has already been
+ *     applied"; seq - 1 > clock[author]: AMG_RANGE_ERROR "Unknown change: actorId = <hex>, seq = <seq - 1>".
+ *   - For seq > 1 the hash of the author's change seq - 1 is added to the deps; the deps are then sorted and without
+ *     repeats (backend.js:76-79). It is read from the engine's hashes on the device; no host hash graph is built. A loaded
+ *     document has its history rebuilt first unless that change is one of the loaded heads.
+ *   - The change is encoded and applied on the device; its bytes go to the host only after the apply. Encoder errors
+ *     are those of amg_encode_changes, apply errors those of amg_apply_changes. A table that does not hold exactly one
+ *     change is AMG_RANGE_ERROR.
+ *   - On every error above the document is unchanged. The exception is a change whose deps are not all applied: it waits
+ *     in the queue, and the call then fails with "Unknown change: ..., seq = <seq>", as the reference does after its apply.
+ *   - A change of 256 bytes or more is returned DEFLATEd, and getChanges, getChangeByHash, getChangesAdded and sync hand it
+ *     out DEFLATEd, byte for byte as after applying the DEFLATEd form. Only amg_arena shows the plain bytes. */
+int amg_apply_local_change(amg_backend* b, const uint8_t* table, size_t table_len, int want_patch,
+                           amg_patch** out, amg_buffers** out_change, amg_error* err);
+/* device span of the last amg_apply_local_change call in ms: staging, encode, apply and the read-back of the change */
+float amg_last_local_ms(amg_backend* b);
 /* state needed by the host-side applyLocalChange (backend.js:54-91): clock[actor] and hashesByActor[actor][index] */
 int amg_clock_of(amg_backend* b, const uint8_t* actor, size_t actor_len, uint64_t* seq_out, amg_error* err);
 int amg_hash_by_actor(amg_backend* b, const uint8_t* actor, size_t actor_len, uint64_t index, uint8_t hash_out[32], int* found, amg_error* err);
