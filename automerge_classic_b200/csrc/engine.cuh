@@ -200,7 +200,8 @@ class Engine {
   // ---- scratch (grow-only)
   DBuf<u32> chOff, chLen, nOps, nPreds, nDeps, nActors, colOff, colLen, depBase, depIdx, primary, pass, flagWord, appRank, opBase, predBase, timeBase, amapBase, amap, authorSlot, newSlots;
   DBuf<u8> applied; DBuf<ChangeHot> hot; DBuf<ChangeMeta> meta /* save(): full headers */; DBuf<u64> errWord; DBuf<u32> hashTable;
-  DBuf<u32> inflCap, inflCapOff, inflOvf; DBuf<u8> inflScratch;
+  DBuf<u32> inflCap, inflCapOff, inflOvf; DBuf<u8> inflScratch; DBuf<u64> inflTotal;
+  u64 inflateSpeculate(InflateArgs& ia);   // first inflate pass + inflOff; returns the 64-bit total of the inflated sizes
   DBuf<u32> rawBase, rawPredBase, decErr, decDirect; DBuf<u64> decCursor; size_t lastDeflCount = 0, lastDeflStart = 0;
   u32* decTotalsPtr() { return reinterpret_cast<u32*>(decCursor.p + 2); }
   DBuf<u32> patchByteLen, patchByteOff; DBuf<u8> patchBytesD;   // key / value bytes shipped inside the patch   // fused decode (decode.cuh k_decode_tiles)
@@ -366,6 +367,7 @@ class Engine {
     const u8* exportMarks = nullptr;
     enum { SRC_PINNED, SRC_DEVICE, SRC_PAGEABLE } srcKind = SRC_PAGEABLE; bool offsetsByDma = false, copiesFirst = false;
     size_t total = 0, arenaLen0 = 0, cur = 0, Bq = 0, B = 0;   // batch: n new changes, then Bq queued ones; bytes arena[arenaLen0, cur)
+    size_t queueBytes = 0;   // bytes of the Bq queued entries: they lie before arenaLen0, outside [arenaLen0, cur)
     struct Piece { size_t byteEnd, changeEnd, mark; }; std::vector<Piece> pieces;
     HostChange* pairs = nullptr; u8* hashOut = nullptr; DecodeTilesArgs dargs{};   // pairs: pinned (offset, length) table of the batch
     // DEFLATEd changes: originals of queue entries (batchOriginal, dense) and of the ones inflated now (inflOrig, parallel to deflIdx)

@@ -97,6 +97,7 @@ inline void Engine::applyChangesOnce(ApplyCall& a, PatchOut& out) {
   trace.begin("upload+hash+decode");
   struct EndTrace { Trace& t; ~EndTrace() { t.end(); } } endTrace{trace};
   a.arenaLen0 = a.cur = arenaLen; a.Bq = queue.size(); a.B = a.n + a.Bq;
+  for (const HostChange& q : queue) a.queueBytes += q.len;
   if (a.blob && a.n > 0) a.total = a.offsets[a.n] - a.offsets[0]; else for (size_t i = 0; i < a.n; i++) a.total += a.lens[i];
   if ((u64)a.arenaLen0 + a.total + 64 >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: change arena limited to 4 GiB per document");
   struct Rollback { Engine* e; size_t len; bool armed = true; ~Rollback() { if (armed) { if (e->hostArena.size() > len) e->hostArena.resize(len); e->rebuildActorTable(); } } } rb{this, hostArena.size()};
@@ -282,9 +283,7 @@ inline void Engine::inflateBatch(ApplyCall& a) {
     foreach(ctx, nd, InflateCapKernel{deflList.p, chLen.p, factor, inflCap.p});
     scan_exclusive(ctx, scanTmp, inflCap.p, inflCapOff.p, nd);
     InflateArgs ia{arena.p, chOff.p, chLen.p, deflList.p, nd, inflLen.p, nullptr, 0u, origOff, origLen, inflScratch.p, inflCapOff.p, inflOvf.p, errWord.p};
-    inflate_changes(ctx, INFL_SPECULATE, ia);
-    scan_exclusive(ctx, scanTmp, inflLen.p, inflOff.p, nd);
-    const size_t extra = readU32(inflOff.p + nd);
+    const u64 extra = inflateSpeculate(ia);
     if (errSnapshot) throwKernelError(errSnapshot);   // (the error word travels with every small read)
     if ((u64)a.cur + extra + 64 >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: change arena limited to 4 GiB per document");
     const size_t extraStart = a.cur; a.cur += extra;
@@ -303,6 +302,16 @@ inline void Engine::inflateBatch(ApplyCall& a) {
   lastDeflCount = a.inflNd; lastDeflStart = a.inflExtraStart;
   trace.mark("decode:finish-enqueued");
   side_join(ctx);
+}
+// The first inflate pass (sizes into ia.outLen), the places of the inflated changes behind the batch (inflOff, 32-bit scan)
+// and their total. One stream may inflate to almost 2^31 bytes, so the scan wraps for two of them: the total is summed in
+// 64 bits by the pass itself, and the callers refuse one past the arena limit before anything is placed.
+inline u64 Engine::inflateSpeculate(InflateArgs& ia) {
+  inflTotal.ensure(ctx, 1); dev_memset(ctx, inflTotal.p, 0, 8); ia.total = inflTotal.p;
+  inflate_changes(ctx, INFL_SPECULATE, ia);
+  scan_exclusive(ctx, scanTmp, ia.outLen, inflOff.p, ia.nd);
+  u64 total = 0; void* dst[1] = {&total}; readWords({{inflTotal.p, 8}}, dst);
+  return total;
 }
 // Host side of the device inflate: which batch entries moved where. Not on the critical path: runs when the information
 // is first needed (queue hand-over, commit).
@@ -341,7 +350,9 @@ inline u64 Engine::hashTableOf(const u8* hs, size_t count) {
 inline void Engine::runGate(ApplyCall& a) {
   const size_t B = a.B;
   depBase.ensure(ctx, B + 1); scan_exclusive(ctx, scanTmp, nDeps.p, depBase.p, B);
-  const size_t depBound = (a.cur - a.arenaLen0) / 32 + B + 1;   // every dependency occupies 32 bytes of its change: no need to read the exact total
+  // every dependency occupies 32 bytes of its change, and every entry's bytes are this call's or a queued entry's: a bound
+  // instead of a read of the exact total
+  const size_t depBound = (a.cur - a.arenaLen0 + a.queueBytes) / 32 + B + 1;
   depIdx.ensure(ctx, depBound + 1); primary.ensure(ctx, B); pass.ensure(ctx, B);
   a.G = numApplied + B; const u64 mask = hashTableOf(hashes.p, a.G);
   foreach(ctx, B, ResolveDepsKernel{arena.p, hashes.p, hashTable.p, mask, hot.p, nDeps.p, numApplied, depBase.p, depIdx.p, primary.p});
@@ -415,12 +426,17 @@ inline void Engine::runGate(ApplyCall& a) {
 // ------------------------------------------------------------ 4. actors
 inline void Engine::internActors(ApplyCall& a) {
   const size_t B = a.B; a.now = st; std::vector<std::string>& actors = a.now.actorIds;
-  authorSlot.ensure(ctx, B); newSlots.ensure(ctx, B + 1); u32 fresh = 0;
+  authorSlot.ensure(ctx, B); newSlots.ensure(ctx, B + 1); u32 fresh = 0, amapTotal = 0;
+  // the actor map's place for every applied change (author + other-actor table); its exact size comes with the read below
+  // (a change has fewer table entries than bytes, so the 32-bit scan cannot wrap below the 4 GiB arena limit)
+  amapBase.ensure(ctx, B + 1); rowSlot.ensure(ctx, B + 1);
+  foreach(ctx, B, MaskedCountKernel{nActors.p, applied.p, rowSlot.p});
+  scan_exclusive(ctx, scanTmp, rowSlot.p, amapBase.p, B);
   while (true) {   // grow the table until the distinct authors fit at load factor <= 1/2
     dev_memset(ctx, flagWord.p, 0, 8);
     foreach(ctx, B, ActorInternKernel{arena.p, hot.p, applied.p, appRank.p, actorSlots.p, (u64)actorCap - 1, authorSlot.p, flagWord.p + 1});
     foreach(ctx, B, NewActorKernel{hot.p, applied.p, authorSlot.p, actorSlots.p, newSlots.p, flagWord.p});
-    u32 full = 0; readU32x2(flagWord.p, flagWord.p + 1, &fresh, &full);
+    u32 full = 0; { void* dst[3] = {&fresh, &full, &amapTotal}; readWords({{flagWord.p, 4}, {flagWord.p + 1, 4}, {amapBase.p + B, 4}}, dst); }
     if (!full && (actors.size() + fresh) * 2 <= actorCap) break;
     actorCap *= 4; actorSlots.ensure(ctx, actorCap); rebuildActorTable();
   }
@@ -459,10 +475,7 @@ inline void Engine::internActors(ApplyCall& a) {
   }
   a.ord = Ord{actorRank.p, bits_for(A > 1 ? A - 1 : 1)};
   trace.mark("actors:numbered");
-  amapBase.ensure(ctx, B + 1); rowSlot.ensure(ctx, B + 1);
-  foreach(ctx, B, MaskedCountKernel{nActors.p, applied.p, rowSlot.p});
-  scan_exclusive(ctx, scanTmp, rowSlot.p, amapBase.p, B);
-  amap.ensure(ctx, B + (a.cur - a.arenaLen0) / 2 + 2);   // author + one entry per other-actor table entry (>= 2 bytes each): bound instead of a round trip
+  amap.ensure(ctx, (size_t)amapTotal + 1);   // exact: an other-actor table entry can be a single byte (an empty id)
   foreach(ctx, B, ActorMapKernel{arena.p, hot.p, nActors.p, applied.p, appRank.p, actorSlots.p, (u64)actorCap - 1, amapBase.p, amap.p, errWord.p});
   trace.mark("actors:mapped");
 }
@@ -491,14 +504,14 @@ inline void Engine::throwActorError(u64 ew, const std::vector<std::string>& acto
   if ((ew & 0xff) != KE_UNKNOWN_ACTOR) throwKernelError(ew);
   const size_t b = (size_t)(ew >> 8); ChangeHot m0; u32 na0 = 1; d2h(ctx, &m0, hot.p + b, sizeof(ChangeHot)); d2h(ctx, &na0, nActors.p + b, 4); sync(ctx);
   std::vector<u8> bytes(m0.len); d2h(ctx, bytes.data(), arena.p + m0.off, m0.len); sync(ctx);
-  ByteReader r(bytes.data(), m0.otherOff - m0.off, m0.len); std::string culprit;
+  ByteReader r(bytes.data(), m0.otherOff - m0.off, m0.len); std::string culprit; bool found = false;   // (an empty id can be the culprit)
   for (u32 k = 0; k < na0 && !r.err; k++) {
     u32 off, len; if (k == 0) { off = m0.actorOff - m0.off; len = m0.actorLen; } else { len = (u32)r.uleb(); off = r.pos; r.skip(len); }
     if (r.err) break;
     const std::string id((const char*)bytes.data() + off, len);
-    if (std::find(actors.begin(), actors.end(), id) == actors.end()) { culprit = id; break; }
+    if (std::find(actors.begin(), actors.end(), id) == actors.end()) { culprit = id; found = true; break; }
   }
-  if (!culprit.empty()) throw Error(AMG_ERR_RANGE, "actorId " + hex_of((const u8*)culprit.data(), culprit.size()) + " is not known to document");
+  if (found) throw Error(AMG_ERR_RANGE, "actorId " + hex_of((const u8*)culprit.data(), culprit.size()) + " is not known to document");
   throwKernelError(ew);
 }
 // the sequence check failed: replay it in application order on the host to produce the reference's message
@@ -1988,9 +2001,7 @@ inline void Engine::inflateDecodeInput(DecodeCall& d) {
   foreach(ctx, nd, InflateCapKernel{dcDefl.p, dcLen.p, factor, inflCap.p});
   scan_exclusive(ctx, scanTmp, inflCap.p, inflCapOff.p, nd);
   InflateArgs ia{dcArena.p, dcOff.p, dcLen.p, dcDefl.p, nd, inflLen.p, nullptr, 0u, patchTriples.p, patchTriples.p + nd, inflScratch.p, inflCapOff.p, inflOvf.p, dcErr.p + DP_INFLATE};
-  inflate_changes(ctx, INFL_SPECULATE, ia);
-  scan_exclusive(ctx, scanTmp, inflLen.p, inflOff.p, nd);
-  const size_t extra = readU32(inflOff.p + nd), start = d.tot[3];
+  const u64 extra = inflateSpeculate(ia); const size_t start = d.tot[3];
   if ((u64)start + extra + 64 >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: change arena limited to 4 GiB per call");
   dcArena.ensure(ctx, start + extra + 64, start);
   ia.arena = dcArena.p; ia.outOff = inflOff.p; ia.extraStart = (u32)start;

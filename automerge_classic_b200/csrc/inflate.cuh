@@ -200,6 +200,7 @@ enum { INFL_SPECULATE = 0, INFL_PLACE = 1 };
 struct InflateArgs {
   u8* arena; u32* chOff; u32* chLen; const u32* list; size_t nd; u32* outLen; const u32* outOff; u32 extraStart; u32* origOff; u32* origLen;
   u8* scratch; const u32* capOff; u32* ovf; u64* errWord;
+  u64* total = nullptr;   // INFL_SPECULATE adds every outLen here: each is below 2^31 + 16, so their 32-bit scan wraps for two
 };
 HD void inflate_one(InflWarpTables& T, size_t k, int pass, const InflateArgs& a, int lane, int nlanes) {
   const u32 c = a.list[k]; const u32 off = pass == INFL_SPECULATE ? a.chOff[c] : a.origOff[k], len = pass == INFL_SPECULATE ? a.chLen[c] : a.origLen[k];
@@ -213,7 +214,10 @@ HD void inflate_one(InflWarpTables& T, size_t k, int pass, const InflateArgs& a,
     const u32 e = inflate_tabled(T, a.arena, streamBegin, streamBegin + clen, dst, cap, &out, lane, nlanes, &over);
     if (lane == 0) {
       if (e) { raise(a.errWord, e, c); a.outLen[k] = 0; }
-      else { a.outLen[k] = 9 + uleb_len(out) + out; a.origOff[k] = off; a.origLen[k] = len; a.ovf[k] = over; }
+      else {
+        a.outLen[k] = 9 + uleb_len(out) + out; a.origOff[k] = off; a.origLen[k] = len; a.ovf[k] = over;
+        if (a.total) atomic_add(reinterpret_cast<unsigned long long*>(a.total), (unsigned long long)a.outLen[k]);
+      }
     }
     INFL_SYNC();
     return;
