@@ -831,8 +831,11 @@ inline void Engine::buildPatch(const PatchInputs& in, PatchOut& out) {
     dev_memset(ctx, objTouchedAt.p, 0xff, (N + 1) * 4); dev_memset(ctx, linkDone.p, 0xff, (N + 1) * 4); dev_memset(ctx, flagWord.p, 0, 16);
     foreach(ctx, N, TouchKernel{d, groupOf.p, in.firstNewSucc, groupTouched.p, objTouchedAt.p, in.objPos, flagWord.p + 2});
     u32 linkChanged = 1, anyLink32 = 0;
-    for (int iter = 0; iter < 1000 && linkChanged; iter++) {   // three sweeps per host round trip (object nesting is shallow)
-      LinkKernel lk{d, groupOf.p, groupHasChild.p, groupFirst.p, in.objPos, groupLinked.p, objTouchedAt.p, flagWord.p + 2, linkDone.p, flagWord.p, listLinkTime.p, flagWord.p + 3};
+    // Three sweeps per host round trip, until a sweep changes nothing. A touch climbs at least one level of nesting per
+    // sweep (a parent's make row lies below its child's rows, so a serial sweep climbs exactly one), so a fixed number of
+    // rounds would leave the outer levels of deeply nested objects unlinked. It ends: objTouchedAt only decreases.
+    while (linkChanged) {
+      LinkKernel lk{d, groupOf.p, groupHasChild.p, groupFirst.p, groupTouched.p, in.objPos, groupLinked.p, objTouchedAt.p, flagWord.p + 2, linkDone.p, flagWord.p, listLinkTime.p, flagWord.p + 3};
       foreach(ctx, N, lk); foreach(ctx, N, lk);
       dev_memset(ctx, flagWord.p, 0, 4);
       foreach(ctx, N, lk);

@@ -99,8 +99,11 @@ struct TouchKernel {   // new rows and the targets of new succ entries touch the
 // setupPatches (new.js:1461-1528): a touched object links itself into its parent (the group of its make row), recursively.
 // Objects are visited in the order they were first touched; the time travels up with the link so that link edits on a
 // list parent can be ordered the same way. A list element that already carries edits of this call needs no link edit.
+// When the key / element was itself touched by this call, the parent's patch already holds the child (patchExists,
+// new.js:1472-1474, 1509-1510) and the climb stops there: the parent's ancestors are linked at the parent's own time
+// (or a later child's), not at this child's.
 struct LinkKernel {
-  DocRows d; const u32* groupOf; const u32* groupHasChild; const u32* groupFirst; const u32* objPos; u32* groupLinked; u32* objTouchedAt; u32* rootTouched; u32* linkDone; u32* changed;
+  DocRows d; const u32* groupOf; const u32* groupHasChild; const u32* groupFirst; const u32* groupTouched; const u32* objPos; u32* groupLinked; u32* objTouchedAt; u32* rootTouched; u32* linkDone; u32* changed;
   u32* listLinkTime /* per position of an element's insert row; 0xffffffff = none */; u32* anyListLink;
   HD void operator()(size_t p) const {
     const u32 t = objTouchedAt[p];
@@ -116,6 +119,7 @@ struct LinkKernel {
       const u32 e = groupFirst[g];
       atomic_min(&listLinkTime[e], t); *anyListLink = 1;   // whether an edit is really needed is known once the pops are replayed (elemHasLive)
     } else groupLinked[g] = 1;
+    if (groupTouched[g]) return;
     if (objPos[p] == ROW_NONE) *rootTouched = 1; else atomic_min(&objTouchedAt[objPos[p]], t);
   }
 };

@@ -1218,7 +1218,8 @@ def check_corrupt_documents(Doc, seed=1, per_doc=60):
 # ---------------------------------------------------------------------------------------------
 # The two places where the engine deliberately does not follow the reference's 600-op block structure (DESIGN.md section 5)
 def _list_rows(doc):
-    """(idCtr, idActorHex, keyCtr, keyActorHex or None, insert, succNum) of every list row, in document order."""
+    """(idCtr, idActorHex, keyCtr, keyActorHex or None, insert, succNum, (objCtr, objActorHex)) of every list row, in
+    document order."""
     dumped = doc.dump_ops()
     if len(dumped) == 3:       # oracle: objCtr,objActor,keyCtr,keyActor,idCtr,idActor,insert,...,succNum[9]
         rows, _, actors = dumped
@@ -1226,7 +1227,8 @@ def _list_rows(doc):
         for r in rows.astype(np.int64):
             if r[2] == -1 and r[3] == -1:
                 continue       # map row
-            out.append((int(r[4]), actors[int(r[5])], int(r[2]), actors[int(r[3])] if r[3] >= 0 else None, bool(r[6]), int(r[9])))
+            out.append((int(r[4]), actors[int(r[5])], int(r[2]), actors[int(r[3])] if r[3] >= 0 else None, bool(r[6]), int(r[9]),
+                        (int(r[0]), actors[int(r[1])])))
         return out
     rows, _ = dumped           # engine: objCtr,objActor,idCtr,idActor,keyCtr,keyActor,flags,succNum
     actors = doc._state().actors
@@ -1235,19 +1237,21 @@ def _list_rows(doc):
     for r in rows:
         if r[4] == none:
             continue
-        out.append((int(r[2]), actors[int(r[3])], int(r[4]), actors[int(r[5])] if r[5] != none else None, bool(int(r[6]) & 1), int(r[7])))
+        out.append((int(r[2]), actors[int(r[3])], int(r[4]), actors[int(r[5])] if r[5] != none else None, bool(int(r[6]) & 1), int(r[7]),
+                    (int(r[0]), actors[int(r[1])])))
     return out
 
 
 def _rga_violations(rows):
     """Elements of lower id standing between an element and the element it was inserted after: the skip rule of
-    new.js:143-162 never leaves such a pair (single list object assumed)."""
-    pos = {(r[0], r[1]): i for i, r in enumerate(rows) if r[4]}
+    new.js:143-162 never leaves such a pair. Any number of list objects: an element and its reference element lie in the
+    same object, and the rows of one object are contiguous in document order."""
+    pos = {(r[6], r[0], r[1]): i for i, r in enumerate(rows) if r[4]}
     bad = 0
     for i, r in enumerate(rows):
         if not r[4] or r[3] is None:
             continue
-        p = pos.get((r[2], r[3]))
+        p = pos.get((r[6], r[2], r[3]))
         if p is None:
             continue
         for q in rows[p + 1:i]:
