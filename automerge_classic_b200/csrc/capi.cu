@@ -1,6 +1,5 @@
-// amgpu — extern "C" surface (include/amgpu.h) over amg::Engine, plus the host-side hash graph
-// (reference backend/new.js:1921-2028: getChanges / getChangeByHash / getMissingDeps; getChangesAdded runs on the device).
-#include <unordered_map>
+// amgpu — extern "C" surface (include/amgpu.h) over amg::Engine. The hash-graph queries (reference backend/new.js:1921-2028)
+// are answered by the engine from its device hashes; only the change bytes they return come from the host arena copy.
 #include "../../include/amgpu.h"
 #include "engine_impl.cuh"
 
@@ -9,53 +8,10 @@ using namespace amg;
 struct amg_patch { const u8* p; size_t len; };   // view into the engine's pinned patch buffer
 struct amg_buffers { std::vector<std::string> items; };
 
-namespace {
-typedef std::array<u8, 32> Hash;
-struct HashHasher { size_t operator()(const Hash& h) const { size_t v; memcpy(&v, h.data(), sizeof(v)); return v; } };
-Hash toHash(const u8* p) { Hash h; memcpy(h.data(), p, 32); return h; }
-std::string hashHex(const Hash& h) { return hex_of(h.data(), 32); }
-
-// A change's dependency hashes, actor and seq, read from its header (columnar.js decodeChangeHeader) in the host arena
-struct ChangeHeader { std::vector<Hash> deps; std::string actor; u64 seq; };
-ChangeHeader readHeader(const u8* arena, const HostChange& c) {
-  ByteReader r(arena, c.off + 8, c.off + c.len); r.pos++; r.uleb();
-  ChangeHeader h; h.deps.resize(r.uleb());
-  for (Hash& d : h.deps) { memcpy(d.data(), arena + r.pos, 32); r.skip(32); }
-  const u64 al = r.uleb(); h.actor.assign((const char*)arena + r.pos, al); r.skip(al);
-  h.seq = r.uleb();
-  return h;
-}
-
-// Host hash graph, filled lazily from the applied changes' headers (the reference defers it too: new.js:1887-1912)
-struct HostGraph {
-  size_t known = 0;
-  std::vector<Hash> hash; std::vector<std::string> actor; std::vector<u64> seq; std::vector<std::vector<Hash>> deps;
-  std::unordered_map<Hash, u32, HashHasher> indexByHash; std::unordered_map<Hash, std::vector<Hash>, HashHasher> dependents;
-  std::map<std::string, std::vector<Hash>> hashesByActor;
-};
-}  // namespace
-
 struct amg_backend {
-  Engine eng; HostGraph g;
+  Engine eng;
   explicit amg_backend(int dev) : eng(dev) {}
 
-  void ensureGraph() {
-    Engine& e = eng;
-    e.computeHashGraph();   // new.js:1922, 1980, 2000, 2015
-    if (g.known == e.numApplied) return;
-    const size_t from = g.known, to = e.numApplied;
-    e.ensureHostMirror();   // the change headers are read from the host copy of the arena (fetched now if the batch came from pinned / device memory)
-    std::vector<u8> hs((to - from) * 32); d2h(e.ctx, hs.data(), e.hashes.p + from * 32, hs.size()); sync(e.ctx);
-    for (size_t i = from; i < to; i++) {
-      Hash h; memcpy(h.data(), hs.data() + (i - from) * 32, 32);
-      ChangeHeader c = readHeader(e.hostArena.data(), e.changes[i]);
-      g.indexByHash[h] = (u32)i; g.dependents[h];
-      for (auto& d : c.deps) g.dependents[d].push_back(h);
-      auto& v = g.hashesByActor[c.actor]; if (v.size() < c.seq) v.resize(c.seq); v[c.seq - 1] = h;
-      g.hash.push_back(h); g.actor.push_back(std::move(c.actor)); g.seq.push_back(c.seq); g.deps.push_back(std::move(c.deps));
-    }
-    g.known = to;
-  }
   // columnar.js:798-811 deflateChange: magic + checksum of the plain form, chunk type 2, raw DEFLATE of the body
   static std::string deflateChange(const std::string& plain) {
     ByteReader r((const u8*)plain.data(), 9, (u32)plain.size()); const u64 bodyLen = r.uleb();
@@ -71,43 +27,7 @@ struct amg_backend {
     std::string plain((const char*)eng.hostArena.data() + c.off, c.len);
     return eng.exportsDeflated(idx) ? deflateChange(plain) : plain;
   }
-  // new.js:1921-1973 getChanges(haveDeps): the indexes of the changes it returns, in its order. n == 0: every applied change
-  // (the host graph is not needed for that; the caller makes sure the hashes are known).
-  std::vector<u32> changesSince(const u8* have_deps, size_t n);
 };
-
-std::vector<u32> amg_backend::changesSince(const u8* have_deps, size_t n) {
-  std::vector<u32> out;
-  if (n == 0) { out.resize(eng.changes.size()); for (size_t i = 0; i < out.size(); i++) out[i] = (u32)i; return out; }
-  ensureGraph();
-  std::vector<Hash> stack, toReturn; std::unordered_map<Hash, bool, HashHasher> seen;
-  for (size_t i = 0; i < n; i++) {
-    Hash h = toHash(have_deps + 32 * i); seen[h] = true;
-    auto it = g.dependents.find(h); if (it == g.dependents.end() || !g.indexByHash.count(h)) throw amg::Error(AMG_RANGE_ERROR, "hash not found: " + hashHex(h));
-    stack.insert(stack.end(), it->second.begin(), it->second.end());
-  }
-  // Reference quirk reproduced on purpose (new.js:1938-1955): the traversal stops at a change with an unseen dependency, but
-  // the test below only looks at the stack and the heads - when that change was the last one on the stack and the heads
-  // have all been seen, the fast path still answers, without the changes that are concurrent to `haveDeps`.
-  while (!stack.empty()) {
-    Hash h = stack.back(); stack.pop_back(); seen[h] = true; toReturn.push_back(h);
-    bool all = true; for (auto& d : g.deps[g.indexByHash[h]]) if (!seen.count(d)) all = false;
-    if (!all) break;
-    auto& ds = g.dependents[h]; stack.insert(stack.end(), ds.begin(), ds.end());
-  }
-  bool headsSeen = true; for (auto& h : eng.st.heads) if (!seen.count(h)) headsSeen = false;
-  if (stack.empty() && headsSeen) { for (auto& h : toReturn) out.push_back(g.indexByHash[h]); return out; }
-  stack.clear(); for (size_t i = 0; i < n; i++) stack.push_back(toHash(have_deps + 32 * i)); seen.clear();
-  while (!stack.empty()) {
-    Hash h = stack.back(); stack.pop_back();
-    if (!seen.count(h)) {
-      auto it = g.indexByHash.find(h); if (it == g.indexByHash.end()) throw amg::Error(AMG_RANGE_ERROR, "hash not found: " + hashHex(h));
-      auto& ds = g.deps[it->second]; stack.insert(stack.end(), ds.begin(), ds.end()); seen[h] = true;
-    }
-  }
-  for (size_t i = 0; i < eng.changes.size(); i++) if (!seen.count(g.hash[i])) out.push_back((u32)i);
-  return out;
-}
 
 namespace {
 void setErr(amg_error* err, int code, const std::string& msg) {
@@ -149,7 +69,7 @@ void amg_free(amg_backend* b) { delete b; }
 amg_backend* amg_load(int cuda_device, const uint8_t* data, size_t len, amg_error* err) {
   return construct(cuda_device, err, [&](amg_backend& b) { b.eng.loadDocument(data, len); });
 }
-int amg_reset(amg_backend* b, amg_error* err) { AMG_GUARD(b->g = HostGraph(); b->eng.reset(); return 0;) }
+int amg_reset(amg_backend* b, amg_error* err) { AMG_GUARD(b->eng.reset(); return 0;) }
 int amg_reserve(amg_backend* b, size_t arena_bytes, amg_error* err) { AMG_GUARD(b->eng.hostArena.reserve(arena_bytes); b->eng.arena.ensure(b->eng.ctx, arena_bytes + 64, b->eng.arenaLen); return 0;) }
 
 amg_backend* amg_clone(amg_backend* src, amg_error* err) {
@@ -207,8 +127,8 @@ int amg_save(amg_backend* b, amg_buffers** out, amg_error* err) {
 // new.js:1921-1973
 int amg_get_changes(amg_backend* b, const uint8_t* have_deps, size_t n, amg_buffers** out, amg_error* err) {
   AMG_GUARD(
-    b->ensureGraph();
-    *out = buffers([&](Items& l) { for (u32 i : b->changesSince(have_deps, n)) l.push_back(b->changeBytes(i)); }).release(); return 0;)
+    std::vector<u32> idx; b->eng.changesSince(have_deps, n, idx);
+    *out = buffers([&](Items& l) { for (u32 i : idx) l.push_back(b->changeBytes(i)); }).release(); return 0;)
 }
 // sync.js:234-238 makeBloomFilter: Bloom filter over the hashes of getChanges(last_sync), built on the device
 int amg_sync_bloom(amg_backend* b, const uint8_t* last_sync, size_t n, amg_buffers** out, amg_error* err) {
@@ -216,8 +136,8 @@ int amg_sync_bloom(amg_backend* b, const uint8_t* last_sync, size_t n, amg_buffe
     Engine& e = b->eng; e.computeHashGraph();   // the hashes of a loaded document (new.js:1922)
     *out = buffers([&](Items& l) {
       l.emplace_back();
-      if (n == 0) e.syncBloom(nullptr, e.numApplied, l.back());   // every applied change: no host graph needed
-      else { const std::vector<u32> idx = b->changesSince(last_sync, n); e.syncBloom(idx.data(), idx.size(), l.back()); }
+      if (n == 0) e.syncBloom(nullptr, e.numApplied, l.back());   // every applied change: no graph walk needed
+      else { std::vector<u32> idx; e.changesSince(last_sync, n, idx); e.syncBloom(idx.data(), idx.size(), l.back()); }
     }).release(); return 0;)
 }
 // sync.js:246-306 getChangesToSend for a non-empty `have`
@@ -225,7 +145,7 @@ int amg_sync_changes_to_send(amg_backend* b, const uint8_t* last_sync, size_t n_
                              const uint8_t* need, size_t n_need, amg_buffers** out_changes, amg_buffers** out_hashes, amg_error* err) {
   AMG_GUARD(
     Engine& e = b->eng; e.computeHashGraph();
-    std::vector<u32> cand; if (n_last > 0) cand = b->changesSince(last_sync, n_last);
+    std::vector<u32> cand; if (n_last > 0) e.changesSince(last_sync, n_last, cand);
     const u32* idx = n_last > 0 ? cand.data() : nullptr; const size_t count = n_last > 0 ? cand.size() : e.numApplied;
     std::vector<Engine::BloomSpec> fs(n_filters);
     for (size_t i = 0; i < n_filters; i++) fs[i] = Engine::BloomSpec{filters[i].num_entries, filters[i].num_probes, filters[i].bits, filters[i].bits_len};
@@ -234,13 +154,12 @@ int amg_sync_changes_to_send(amg_backend* b, const uint8_t* last_sync, size_t n_
     // order, the candidates that were marked or are needed
     std::vector<u32> outIdx;
     if (n_need > 0) {
-      b->ensureGraph();
+      std::vector<u32> needIdx; e.spans.resume(SPAN_SYNC); e.lookupHashes(need, n_need, needIdx); e.spans.stop();
       std::vector<u32> posOf(e.numApplied, EMPTY32);   // change index -> candidate position
       for (size_t i = 0; i < count; i++) posOf[idx ? idx[i] : i] = (u32)i;
-      for (size_t k = 0; k < n_need; k++) {
-        auto it = b->g.indexByHash.find(toHash(need + 32 * k));
-        if (it == b->g.indexByHash.end()) continue;
-        if (posOf[it->second] != EMPTY32) send[posOf[it->second]] = 1; else outIdx.push_back(it->second);
+      for (u32 c : needIdx) {
+        if (c == DEP_MISSING) continue;
+        if (posOf[c] != EMPTY32) send[posOf[c]] = 1; else outIdx.push_back(c);
       }
     }
     for (size_t i = 0; i < count; i++) if (send[i]) outIdx.push_back(idx ? idx[i] : (u32)i);
@@ -316,32 +235,24 @@ int amg_apply_local_change(amg_backend* b, const uint8_t* table, size_t table_le
             *out_change = lc.release(); return 0;)
 }
 float amg_last_local_ms(amg_backend* b) { return b->eng.spans.ms[SPAN_LOCAL]; }
+// new.js:1999-2002
 int amg_get_change_by_hash(amg_backend* b, const uint8_t hash[32], amg_buffers** out, amg_error* err) {
-  AMG_GUARD(b->ensureGraph(); auto it = b->g.indexByHash.find(toHash(hash));
-            *out = buffers([&](Items& l) { if (it != b->g.indexByHash.end()) l.push_back(b->changeBytes(it->second)); }).release(); return 0;)
+  AMG_GUARD(u32 idx = 0; const bool found = b->eng.changeIndexOf(hash, idx);
+            *out = buffers([&](Items& l) { if (found) l.push_back(b->changeBytes(idx)); }).release(); return 0;)
 }
 // new.js:2014-2028
 int amg_get_missing_deps(amg_backend* b, const uint8_t* heads, size_t n, amg_buffers** out, amg_error* err) {
   AMG_GUARD(
-    b->ensureGraph(); std::map<Hash, bool> allDeps, inQueue; Engine& e = b->eng;
-    for (size_t i = 0; i < n; i++) allDeps[toHash(heads + 32 * i)] = true;
-    e.ensureHostMirror();
-    for (auto& q : e.queue) {
-      for (auto& d : readHeader(e.hostArena.data(), q).deps) allDeps[d] = true;
-      Hash h; host_sha256(e.hostArena.data() + q.off + 8, q.len - 8, h.data());   // the queued change's hash: SHA-256 over bytes [8..)
-      inQueue[h] = true;
-    }
-    *out = buffers([&](Items& l) {
-      for (auto& kv : allDeps) if (!b->g.indexByHash.count(kv.first) && !inQueue.count(kv.first)) l.emplace_back((const char*)kv.first.data(), 32);
-    }).release(); return 0;)
+    std::vector<std::array<u8, 32>> missing; b->eng.missingDeps(heads, n, missing);
+    *out = buffers([&](Items& l) { for (auto& h : missing) l.emplace_back((const char*)h.data(), 32); }).release(); return 0;)
 }
+float amg_last_graph_ms(amg_backend* b) { return b->eng.spans.ms[SPAN_GRAPH]; }
 int amg_clock_of(amg_backend* b, const uint8_t* actor, size_t actor_len, uint64_t* seq_out, amg_error* err) {
   AMG_GUARD(std::string a((const char*)actor, actor_len); *seq_out = 0; Engine& e = b->eng;
             for (size_t i = 0; i < e.st.actorIds.size(); i++) if (e.st.actorIds[i] == a) *seq_out = e.st.clock[i]; return 0;)
 }
 int amg_hash_by_actor(amg_backend* b, const uint8_t* actor, size_t actor_len, uint64_t index, uint8_t hash_out[32], int* found, amg_error* err) {
-  AMG_GUARD(b->ensureGraph(); *found = 0; auto it = b->g.hashesByActor.find(std::string((const char*)actor, actor_len));
-            if (it != b->g.hashesByActor.end() && index < it->second.size()) { memcpy(hash_out, it->second[index].data(), 32); *found = 1; } return 0;)
+  AMG_GUARD(*found = b->eng.hashByActor(std::string((const char*)actor, actor_len), index, hash_out) ? 1 : 0; return 0;)
 }
 
 int amg_last_timings(amg_backend* b, float* ms_out, int n) { for (int i = 0; i < n && i < 24; i++) ms_out[i] = b->eng.trace.ms[i]; return 0; }

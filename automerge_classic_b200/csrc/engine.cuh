@@ -32,6 +32,7 @@
 #include "encchg.cuh"
 #include "snapshot.cuh"
 #include "merge.cuh"
+#include "graph.cuh"
 #include "unknowncols.hpp"
 
 namespace amg {
@@ -97,7 +98,7 @@ struct Trace {
 // Device span of the last call of each entry point kind (amg_last_*_ms): CUDA events on the main stream around the call's
 // uploads, kernels and read-backs; 0 in the emulation build. start(k) zeroes k's slot and opens the span, resume(k) opens
 // it without zeroing, stop() adds the span to the slot. A call that throws never reaches stop(): its slot stays 0.
-enum SpanKind { SPAN_SYNC, SPAN_DECODE, SPAN_ENCODE, SPAN_HISTORY, SPAN_MERGE, SPAN_LOCAL, NUM_SPANS };
+enum SpanKind { SPAN_SYNC, SPAN_DECODE, SPAN_ENCODE, SPAN_HISTORY, SPAN_MERGE, SPAN_LOCAL, SPAN_GRAPH, NUM_SPANS };
 struct DeviceSpans {
   float ms[NUM_SPANS] = {0};
   explicit DeviceSpans(Ctx& c) : ctx(c) {}
@@ -196,7 +197,7 @@ class Engine {
   }
   Trace trace{ctx};
   HBuf<u8> patchBuf;   // pinned: patch records are copied device -> host directly into their final place
-  DeviceSpans spans{ctx};   // sync, decode, encode, history, merge and local-change calls
+  DeviceSpans spans{ctx};   // sync, decode, encode, history, merge, local-change and graph-query calls
   // ---- scratch (grow-only)
   DBuf<u32> chOff, chLen, nOps, nPreds, nDeps, nActors, colOff, colLen, depBase, depIdx, primary, pass, flagWord, appRank, opBase, predBase, timeBase, amapBase, amap, authorSlot, newSlots;
   DBuf<u8> applied; DBuf<ChangeHot> hot; DBuf<ChangeMeta> meta /* save(): full headers */; DBuf<u64> errWord; DBuf<u32> hashTable;
@@ -374,7 +375,7 @@ class Engine {
     std::vector<HostChange> batchOriginal, inflOrig; std::vector<u32> deflIdx; size_t inflNd = 0, inflExtraStart = 0, inflExtra = 0; bool inflPending = false;
     void finishInflate(Engine& e); HostChange originalOf(size_t b) const;
     u32 decTot[4] = {0, 0, 0, 0};   // decode totals: ops, preds, overflow, flags (1: large changes, 2: unknown columns)
-    size_t G = 0, numNew = 0; bool inOrder = true;   // gate: G = applied before + batch
+    size_t G = 0, numNew = 0; bool inOrder = true; u32 D = 0;   // gate: G = applied before + batch; D dependency entries
     std::vector<u8> appliedH; std::vector<u32> primaryH, appRankH; std::vector<HostChange> newQueue, newQueueOriginal;   // host copies: only when an entry waits or the order differs
     DocState now;   // the document's host state as this call leaves it
     size_t M = 0, P = 0, N = 0, numPairs = 0; OpRows ops{}; IdTable idt{nullptr, nullptr, 0}; Ord ord{}; DocRows w{};   // w: rows before the sort
@@ -551,7 +552,50 @@ class Engine {
   // to go out DEFLATEd (deflateOnExport). Errors leave the document unchanged, except "Unknown change" when the change
   // waits in the queue after the apply, which the reference also raises after the apply.
   void applyLocalChange(const u8* table, size_t len, bool wantPatch, PatchOut& out, std::string& binary);
+
+  // ---------------------------------------------------------------- hash-graph queries (graph.cuh; new.js:1921-2028)
+  // The dependency graph of the applied changes over change indexes, in application order, and their hashes. extendGraph()
+  // adds the changes applied since the last query. For a change applied by applyChanges, its dependency indexes and author
+  // come from the gate's own resolution: commit copies the batch's tables device to device (keepGraphInputs, no kernel),
+  // and the query reads them back. Any other change (a loaded document's, or one applied before a reset of these inputs)
+  // has its header parsed in the device arena and its dependency hashes resolved against `hashes` (parseChangeHeaders,
+  // resolveChangeDeps, SaveChangeValKernel for the author). The lists below are appended on the host. The hashes come back
+  // with them, so that getChanges resolves haveDeps and the heads on the host: a query over a current graph launches
+  // nothing. reset() drops the graph; a clone builds its own.
+  struct ChangeGraph {
+    size_t known = 0;                                 // changes [0, known) are in the graph
+    std::vector<u32> depBase{0}, deps;                // change i's dependencies in header order: deps[depBase[i], depBase[i + 1])
+    std::vector<u32> depOwner, nextDependent;         // per entry k of deps: the change it belongs to; the next entry naming the same dependency
+    std::vector<u32> firstDependent, lastDependent;   // per change: the first / last entry of deps that names it (EMPTY32: none)
+    std::vector<std::vector<u32>> byActor;            // byActor[actor number][seq - 1] = change index (an actor's changes apply in seq order)
+    std::vector<std::array<u8, 32>> hash;             // per change
+    std::vector<u32> slots;                           // open addressing over the first 8 hash bytes: change index or EMPTY32
+    template <class F> void eachDependent(u32 c, F f) const { for (u32 k = firstDependent[c]; k != EMPTY32; k = nextDependent[k]) f(depOwner[k]); }   // in application order
+    void add(u32 c, const u32* dep, size_t nDep, u32 actor, const u8* h);   // change c = known, its dependencies, author, hash
+    u32 find(const u8* h) const;                      // the change with hash h, or DEP_MISSING
+  } graph;
+  // What commit keeps of each batch for the graph: per batch entry applied flag, application rank, author's actor number,
+  // dependency offsets; the dependency indexes (gate numbering: < first: applied before, else first + batch entry).
+  struct GraphInputs {
+    struct Batch { size_t first, B, D, numNew, offB, offBase, offD; };
+    std::vector<Batch> batches; size_t usedB = 0, usedBase = 0, usedD = 0;
+    DBuf<u8> applied; DBuf<u32> rank, actor, depBase, depIdx;
+    void clear() { batches.clear(); usedB = usedBase = usedD = 0; }
+  } graphInputs;
+  void keepGraphInputs(ApplyCall& a);
+  void extendGraph();
+  void graphFromHeaders(size_t from, size_t to);
+  void graphFromBatch(const GraphInputs::Batch& b);
+  // Each query computes the hash graph of a loaded document first (new.js:1922, 2000, 2015) and times its device work in
+  // spans[SPAN_GRAPH]. changesSince: getChanges(haveDeps) as change indexes in the order the reference returns them.
+  void changesSince(const u8* haveDeps, size_t n, std::vector<u32>& out);
+  bool changeIndexOf(const u8* hash, u32& idx);   // getChangeByHash: false for a hash that is not an applied change's
+  void missingDeps(const u8* heads, size_t n, std::vector<std::array<u8, 32>>& out);   // getMissingDeps: sorted, without repeats
+  bool hashByActor(const std::string& actor, u64 index, u8* out);   // the hash of actor's change seq = index + 1
+  void lookupHashes(const u8* hs, size_t n, std::vector<u32>& idx);   // idx[i]: the applied change with hash hs[i], or DEP_MISSING
+  DBuf<u8> graphQueries; DBuf<u32> graphIdx; DBuf<long long> graphVals;
  private:
+  void lookupQueries(size_t n, size_t count, std::vector<u32>& idx);   // graphQueries[0, n) among hashes [0, count)
   void uploadCandidates(const u32* idx, size_t count);
 };
 

@@ -72,7 +72,7 @@ inline void Engine::reset() {
   sync(ctx); loaded = LoadedDoc(); unknownCols.clear();
   arenaLen = 0; hostArena.len = 0; numApplied = 0; numRows = 0; numSucc = 0; dev_memset(ctx, succOff.p, 0, 4);
   st = DocState(); changes.clear(); deflatedOriginal.clear(); deflateOnExport.clear();
-  queue.clear(); queueOriginal.clear(); rebuildActorTable();
+  queue.clear(); queueOriginal.clear(); graph = ChangeGraph(); graphInputs.clear(); rebuildActorTable();
 }
 
 // After Backend.load the hashes of the loaded changes are unknown until computeHashGraph has run. Like the reference
@@ -366,8 +366,8 @@ inline void Engine::runGate(ApplyCall& a) {
     dev_memset(ctx, flagWord.p, 0, 4);
     foreach(ctx, B, RelaxKernel{depBase.p, depIdx.p, nDeps.p, primary.p, numApplied, pass.p, flagWord.p, (u32)B + 1});
     u32 again = 0, copies = 0;
-    { void* dst[6] = {&again, &copies, &decTot[0], &decTot[1], &decTot[2], &decTot[3]};
-      readWords({{flagWord.p, 4}, {flagWord.p + 12, 4}, {decTotalsPtr(), 4}, {decTotalsPtr() + 1, 4}, {decTotalsPtr() + 2, 4}, {decTotalsPtr() + 3, 4}}, dst); }
+    { void* dst[7] = {&again, &copies, &decTot[0], &decTot[1], &decTot[2], &decTot[3], &a.D};   // a.D: the batch's dependency count (change graph)
+      readWords({{flagWord.p, 4}, {flagWord.p + 12, 4}, {decTotalsPtr(), 4}, {decTotalsPtr() + 1, 4}, {decTotalsPtr() + 2, 4}, {decTotalsPtr() + 3, 4}, {depBase.p + B, 4}}, dst); }
     checkErr();   // free: the error word came with the read
     if (iter == 0 && decodeOverflowed(decTot)) {   // the raw row tables were too small for this batch: grown, decoded again (same results otherwise)
       runDecodeTiles(arena.p, B, a.cur - a.arenaLen0, deflList.p, a.inflNd, a.inflExtraStart);   // the whole batch is resident by now (inflated changes re-pointed)
@@ -764,6 +764,7 @@ inline void Engine::commit(ApplyCall& a) {
     fill32(doc.time.p, 0, a.N);
     for (auto& kv : a.unknownRows) unknownCols.byOp[kv.first] = std::move(kv.second);
     unknownCols.colIds.insert(a.unknownIds.begin(), a.unknownIds.end());
+    keepGraphInputs(a);
     loaded.bytes.clear(); numApplied += numNew; st = std::move(a.now);
     trace.mark("commit:state-swapped");
     rebuildActorTable();   // slots of actors registered in this call become permanent (first = 0)
@@ -2516,6 +2517,209 @@ inline void Engine::applyLocalChange(const u8* table, size_t len, bool wantPatch
   out.deps.erase(std::remove(out.deps.begin(), out.deps.end(), hash), out.deps.end());
   finishPatch(out);
   spans.stop();
+}
+
+// ------------------------------------------------------------ hash-graph queries (graph.cuh; new.js:1921-2028)
+// The dependents lists are appended on the host: the graph grows batch by batch, and the walks that read it run on the
+// host anyway, so the integers come back once. A device scatter into one CSR would rebuild it whole for every batch.
+inline void Engine::ChangeGraph::add(u32 c, const u32* dep, size_t nDep, u32 actor, const u8* h) {
+  for (size_t j = 0; j < nDep; j++) {
+    const u32 d = dep[j];   // an applied change's dependencies were applied before it
+    if (d >= c) throw Error(AMG_ERR_INTERNAL, "amgpu: change " + std::to_string(c) + " depends on a change that is not applied before it");
+    const u32 k = (u32)deps.size();
+    deps.push_back(d); depOwner.push_back(c); nextDependent.push_back(EMPTY32);
+    if (firstDependent[d] == EMPTY32) firstDependent[d] = k; else nextDependent[lastDependent[d]] = k;
+    lastDependent[d] = k;
+  }
+  depBase.push_back((u32)deps.size()); firstDependent.push_back(EMPTY32); lastDependent.push_back(EMPTY32);
+  if (byActor.size() <= actor) byActor.resize((size_t)actor + 1);
+  byActor[actor].push_back(c);
+  hash.emplace_back(); memcpy(hash.back().data(), h, 32);
+  auto insert = [&](u32 i) { u64 key; memcpy(&key, hash[i].data(), 8); u64 s = mix64(key) & (slots.size() - 1); while (slots[s] != EMPTY32) s = (s + 1) & (slots.size() - 1); slots[s] = i; };
+  if (2 * hash.size() > slots.size()) {   // keep the table at most half full
+    slots.assign(pow2_at_least(std::max<size_t>(64, 4 * hash.size())), EMPTY32);
+    for (u32 i = 0; i < (u32)hash.size(); i++) insert(i);
+  } else insert(c);
+  known = (size_t)c + 1;
+}
+inline u32 Engine::ChangeGraph::find(const u8* h) const {
+  if (slots.empty()) return DEP_MISSING;
+  u64 key; memcpy(&key, h, 8);
+  for (u64 s = mix64(key) & (slots.size() - 1); slots[s] != EMPTY32; s = (s + 1) & (slots.size() - 1))
+    if (memcmp(hash[slots[s]].data(), h, 32) == 0) return slots[s];
+  return DEP_MISSING;
+}
+
+// commit: the batch's gate tables, copied device to device behind the ones kept before (read back by the next query)
+inline void Engine::keepGraphInputs(ApplyCall& a) {
+  GraphInputs& k = graphInputs; const size_t B = a.B, D = a.D;
+  GraphInputs::Batch b{numApplied, B, D, a.numNew, k.usedB, k.usedBase, k.usedD};
+  k.applied.ensure(ctx, b.offB + B + 1, b.offB); k.rank.ensure(ctx, b.offB + B + 1, b.offB); k.actor.ensure(ctx, b.offB + B + 1, b.offB);
+  k.depBase.ensure(ctx, b.offBase + B + 2, b.offBase); k.depIdx.ensure(ctx, b.offD + D + 1, b.offD);
+  d2d(ctx, k.applied.p + b.offB, applied.p, B); d2d(ctx, k.rank.p + b.offB, appRank.p, B * 4); d2d(ctx, k.actor.p + b.offB, changeActor.p, B * 4);
+  d2d(ctx, k.depBase.p + b.offBase, depBase.p, (B + 1) * 4); d2d(ctx, k.depIdx.p + b.offD, depIdx.p, D * 4);
+  k.usedB += B; k.usedBase += B + 1; k.usedD += D; k.batches.push_back(b);
+}
+
+inline void Engine::graphFromBatch(const GraphInputs::Batch& b) {
+  GraphInputs& k = graphInputs; const size_t B = b.B;
+  std::vector<u8> ap(B + 1); std::vector<u32> rank(B + 1), actor(B + 1), base(B + 2), dep(b.D + 1); std::vector<std::array<u8, 32>> hs(b.numNew);
+  d2h(ctx, ap.data(), k.applied.p + b.offB, B); d2h(ctx, rank.data(), k.rank.p + b.offB, B * 4); d2h(ctx, actor.data(), k.actor.p + b.offB, B * 4);
+  d2h(ctx, base.data(), k.depBase.p + b.offBase, (B + 1) * 4); d2h(ctx, dep.data(), k.depIdx.p + b.offD, b.D * 4);
+  d2h(ctx, hs.data(), hashes.p + b.first * 32, b.numNew * 32); sync(ctx);
+  std::vector<u32> byRank(b.numNew, EMPTY32);
+  for (size_t e = 0; e < B; e++) if (ap[e]) byRank[rank[e]] = (u32)e;
+  std::vector<u32> ds;
+  for (size_t r = 0; r < b.numNew; r++) {
+    const u32 e = byRank[r];
+    if (e == EMPTY32) throw Error(AMG_ERR_INTERNAL, "amgpu: change graph: an application rank without its change");
+    ds.clear();
+    for (u32 j = base[e]; j < base[e + 1]; j++) {   // gate numbering -> application index
+      const u32 d = dep[j];
+      ds.push_back(d == DEP_MISSING || d < b.first ? d : (d - (u32)b.first < B && ap[d - b.first] ? (u32)b.first + rank[d - b.first] : DEP_MISSING));
+    }
+    graph.add((u32)(b.first + r), ds.data(), ds.size(), actor[e], hs[r].data());
+  }
+}
+
+inline void Engine::graphFromHeaders(size_t from, size_t to) {
+  const size_t K = to - from;
+  clearErr();
+  const u32 D = parseChangeHeaders(arena.p, changes.data() + from, K);
+  checkErr();
+  resolveChangeDeps(arena.p, hashes.p, to, K, from, D);
+  graphVals.ensure(ctx, K + 1);
+  foreach(ctx, K, SaveChangeValKernel{SM_ACTOR, arena.p, meta.p, actorSlots.p, (u64)actorCap - 1, graphVals.p, nullptr, nullptr, errWord.p});
+  std::vector<u32> base(K + 1), deps((size_t)D + 1); std::vector<long long> actor(K); std::vector<std::array<u8, 32>> hs(K);
+  d2h(ctx, base.data(), depBase.p, (K + 1) * 4); d2h(ctx, deps.data(), depIdx.p, (size_t)D * 4); d2h(ctx, actor.data(), graphVals.p, K * 8);
+  d2h(ctx, hs.data(), hashes.p + from * 32, K * 32); sync(ctx);
+  checkErr();
+  for (size_t b = 0; b < K; b++) graph.add((u32)(from + b), deps.data() + base[b], base[b + 1] - base[b], (u32)actor[b], hs[b].data());
+}
+
+// Brings the graph up to [0, numApplied): kept batches where they continue it, header parses for the rest
+inline void Engine::extendGraph() {
+  GraphInputs& k = graphInputs;
+  size_t next = 0;
+  while (graph.known < numApplied) {
+    while (next < k.batches.size() && k.batches[next].first < graph.known) next++;   // already in the graph
+    if (next < k.batches.size() && k.batches[next].first == graph.known) { graphFromBatch(k.batches[next++]); continue; }
+    graphFromHeaders(graph.known, next < k.batches.size() ? k.batches[next].first : numApplied);
+  }
+  k.clear();
+}
+
+inline void Engine::lookupQueries(size_t n, size_t count, std::vector<u32>& idx) {
+  idx.assign(n, DEP_MISSING);
+  if (n == 0 || count == 0) return;
+  graphIdx.ensure(ctx, n + 1);
+  const u64 mask = hashTableOf(hashes.p, count);
+  foreach(ctx, n, HashLookupKernel{hashes.p, hashTable.p, mask, graphQueries.p, graphIdx.p});
+  d2h(ctx, idx.data(), graphIdx.p, n * 4); sync(ctx);
+}
+
+inline void Engine::lookupHashes(const u8* hs, size_t n, std::vector<u32>& idx) {
+  graphQueries.ensure(ctx, n * 32 + 32);
+  if (n) h2d(ctx, graphQueries.p, hs, n * 32);
+  lookupQueries(n, numApplied, idx);
+}
+
+// new.js:1921-1973. haveDeps and the heads are looked up in the graph's hashes; an unknown hash raises before any traversal. The
+// fast path walks forward from haveDeps through the dependents (no seen test at pop: a change reached from two seen parents
+// is returned twice, as in the reference); when it gives up, the slow path returns every change that is not an ancestor of
+// haveDeps, in application order.
+inline void Engine::changesSince(const u8* haveDeps, size_t n, std::vector<u32>& out) {
+  out.clear();
+  computeHashGraph();
+  spans.start(SPAN_GRAPH);
+  if (n == 0) { out.resize(changes.size()); for (size_t i = 0; i < out.size(); i++) out[i] = (u32)i; spans.stop(); return; }
+  extendGraph();
+  spans.stop();
+  const size_t H = st.heads.size();
+  std::vector<u32> idx(n + H);   // haveDeps, then the heads
+  for (size_t i = 0; i < n; i++) idx[i] = graph.find(haveDeps + 32 * i);
+  for (size_t h = 0; h < H; h++) idx[n + h] = graph.find(st.heads[h].data());
+  for (size_t i = 0; i < n; i++) if (idx[i] == DEP_MISSING) throw Error(AMG_ERR_RANGE, "hash not found: " + hex_of(haveDeps + 32 * i, 32));
+  const ChangeGraph& g = graph;
+  std::vector<u8> seen(numApplied, 0); std::vector<u32> stack;
+  auto push = [&](u32 c) { stack.push_back(c); };
+  for (size_t i = 0; i < n; i++) { seen[idx[i]] = 1; g.eachDependent(idx[i], push); }
+  // Reference quirk reproduced on purpose (new.js:1938-1955): the traversal stops at a change with an unseen dependency, but
+  // the test below only looks at the stack and the heads - when that change was the last one on the stack and the heads
+  // have all been seen, the fast path still answers, without the changes that are concurrent to `haveDeps`.
+  while (!stack.empty()) {
+    const u32 c = stack.back(); stack.pop_back(); seen[c] = 1; out.push_back(c);
+    bool all = true;
+    for (u32 k = g.depBase[c]; k < g.depBase[c + 1] && all; k++) all = seen[g.deps[k]] != 0;
+    if (!all) break;
+    g.eachDependent(c, push);
+  }
+  bool headsSeen = true;
+  for (size_t h = 0; h < H; h++) if (idx[n + h] == DEP_MISSING || !seen[idx[n + h]]) headsSeen = false;
+  if (stack.empty() && headsSeen) return;
+  out.clear(); std::fill(seen.begin(), seen.end(), 0);
+  stack.assign(idx.begin(), idx.begin() + n);
+  while (!stack.empty()) {
+    const u32 c = stack.back(); stack.pop_back();
+    if (seen[c]) continue;
+    seen[c] = 1; stack.insert(stack.end(), g.deps.begin() + g.depBase[c], g.deps.begin() + g.depBase[c + 1]);
+  }
+  for (size_t i = 0; i < changes.size(); i++) if (!seen[i]) out.push_back((u32)i);
+}
+
+// new.js:1999-2002: one lookup among the applied changes (a queued change has no index yet)
+inline bool Engine::changeIndexOf(const u8* hash, u32& idx) {
+  computeHashGraph();
+  spans.start(SPAN_GRAPH);
+  std::vector<u32> found; lookupHashes(hash, 1, found);
+  spans.stop();
+  idx = found[0];
+  return idx != DEP_MISSING;
+}
+
+// new.js:2014-2028. The queued changes' headers are parsed and their hashes computed on the device (SHA-256 over bytes
+// [8, len) of the inflated change, written behind the applied hashes); their dependencies and the given heads are looked up
+// in one table over the applied and the queued hashes. Whatever is in neither is missing.
+inline void Engine::missingDeps(const u8* heads, size_t n, std::vector<std::array<u8, 32>>& out) {
+  out.clear();
+  computeHashGraph();
+  spans.start(SPAN_GRAPH);
+  const size_t C = numApplied, Q = queue.size();
+  u32 D = 0;
+  clearErr();
+  if (Q > 0) {
+    D = parseChangeHeaders(arena.p, queue.data(), Q);
+    checkErr();
+    hashes.ensure(ctx, (C + Q) * 32 + 64, C * 32);
+    foreach(ctx, Q, ShaKernel{arena.p, chOff.p, chLen.p, hashes.p + C * 32, errWord.p, nullptr, nullptr});
+  }
+  graphQueries.ensure(ctx, ((size_t)D + n) * 32 + 32);
+  if (D > 0) foreach(ctx, Q, DepHashCopyKernel{arena.p, meta.p, depBase.p, graphQueries.p});
+  if (n > 0) h2d(ctx, graphQueries.p + (size_t)D * 32, heads, n * 32);
+  std::vector<u32> idx; lookupQueries((size_t)D + n, C + Q, idx);
+  std::vector<std::array<u8, 32>> deps(D);
+  if (D > 0) { d2h(ctx, deps.data(), graphQueries.p, (size_t)D * 32); sync(ctx); }
+  checkErr();
+  spans.stop();
+  for (size_t i = 0; i < (size_t)D + n; i++) {
+    if (idx[i] != DEP_MISSING) continue;
+    if (i < D) out.push_back(deps[i]);
+    else { out.emplace_back(); memcpy(out.back().data(), heads + (i - D) * 32, 32); }
+  }
+  std::sort(out.begin(), out.end());
+  out.erase(std::unique(out.begin(), out.end()), out.end());
+}
+
+// hashesByActor[actor][index] (the host-side applyLocalChange's previous hash, backend.js:54-91)
+inline bool Engine::hashByActor(const std::string& actor, u64 index, u8* out) {
+  computeHashGraph();
+  spans.start(SPAN_GRAPH);
+  extendGraph();
+  const size_t a = (size_t)(std::find(st.actorIds.begin(), st.actorIds.end(), actor) - st.actorIds.begin());
+  const bool found = a < graph.byActor.size() && index < graph.byActor[a].size();
+  if (found) memcpy(out, graph.hash[graph.byActor[a][index]].data(), 32);
+  spans.stop();
+  return found;
 }
 
 }  // namespace amg

@@ -93,7 +93,8 @@ class Library:
         L.amg_apply_local_change.restype = C.c_int
         L.amg_apply_local_change.argtypes = [vp, vp, C.c_size_t, C.c_int, vp, vp, vp]
         L.amg_clock_of.argtypes = [vp, vp, C.c_size_t, vp, vp]
-        for name in ('amg_last_sync_ms', 'amg_last_decode_ms', 'amg_last_encode_ms', 'amg_last_history_ms', 'amg_last_merge_ms', 'amg_last_local_ms'):
+        for name in ('amg_last_sync_ms', 'amg_last_decode_ms', 'amg_last_encode_ms', 'amg_last_history_ms', 'amg_last_merge_ms', 'amg_last_local_ms',
+                     'amg_last_graph_ms'):
             getattr(L, name).restype = C.c_float
             getattr(L, name).argtypes = [vp]
 
@@ -672,6 +673,10 @@ class GpuBackendDoc:
         bl, err = C.c_void_p(), _ErrStruct()
         self._lib.check(self._lib.L.amg_get_missing_deps(self.h, hs, C.c_size_t(len(heads)), C.byref(bl), C.byref(err)), err)
         return [b.hex() for b in self._buffers(bl)]
+
+    def last_graph_ms(self):
+        """Device span of the last get_changes / get_change_by_hash / get_missing_deps / hash_by_actor call (CUDA events), ms."""
+        return float(self._lib.L.amg_last_graph_ms(self.h))
 
     # ---- sync protocol (automerge_classic_b200/sync.py uses these when the document has them)
     def sync_bloom(self, last_sync):

@@ -65,7 +65,10 @@ int amg_get_state(amg_backend* b, amg_patch** out, amg_error* err);
 /* Backend.save (backend/backend.js:93-95, new.js:2033-2055): one buffer = the document chunk */
 int amg_save(amg_backend* b, amg_buffers** out, amg_error* err);
 int amg_get_heads(amg_backend* b, amg_buffers** out, amg_error* err);
-/* Backend.getAllChanges / getChanges(haveDeps) — backend.js:142-156 -> new.js:1921-1973; have_deps = n hashes x 32 bytes */
+/* Backend.getAllChanges / getChanges(haveDeps) — backend.js:142-156 -> new.js:1921-1973; have_deps = n hashes x 32 bytes.
+ * The reference's traversal runs on the host over a graph of change indexes the engine keeps: dependencies resolved on the
+ * device (by the causal gate of applyChanges, or from the change headers for loaded changes), brought up to date by each
+ * query, with the changes' hashes, against which have_deps are looked up. */
 int amg_get_changes(amg_backend* b, const uint8_t* have_deps, size_t n, amg_buffers** out, amg_error* err);
 /* Backend.getChangesAdded(old, new) — backend.js:166-168 -> new.js:1979-1997. The changes of b_new that b_old lacks are
  * found by hash lookups on the device and ordered on the host over their dependency indexes; no host hash graph is built.
@@ -91,7 +94,8 @@ int amg_merge(amg_backend* dst, amg_backend* src, int want_patch, amg_patch** ou
 float amg_last_merge_ms(amg_backend* dst);
 /* Backend.getChangeByHash — backend.js:176-178 -> new.js:1999-2002; zero buffers when unknown */
 int amg_get_change_by_hash(amg_backend* b, const uint8_t hash[32], amg_buffers** out, amg_error* err);
-/* Backend.getMissingDeps — backend.js:190-192 -> new.js:2014-2028: hashes of 32 bytes */
+/* Backend.getMissingDeps — backend.js:190-192 -> new.js:2014-2028: hashes of 32 bytes, ascending. The queued changes are
+ * hashed and parsed on the device; their dependencies and `heads` are looked up among the applied and queued hashes there. */
 int amg_get_missing_deps(amg_backend* b, const uint8_t* heads, size_t n, amg_buffers** out, amg_error* err);
 /* backend/backend.js:54-91 applyLocalChange. `table`: a change table (amg_decode_changes layout) holding one change request;
  * pinned, pageable or device memory. *out: the patch applyChanges(isLocal) returns, without the new change's hash in its deps
@@ -243,6 +247,10 @@ int amg_last_timings(amg_backend* b, float* ms_out, int n);
 /* device span of the last amg_sync_bloom / amg_sync_changes_to_send call in ms: CUDA events around its uploads, kernels and
  * read-backs on the engine's main stream (host work in between included when the stream waits for it) */
 float amg_last_sync_ms(amg_backend* b);
+/* device span of the last amg_get_changes / amg_get_change_by_hash / amg_get_missing_deps / amg_hash_by_actor call in ms
+ * (CUDA events on the engine's main stream, like amg_last_sync_ms): the graph update, hashing and lookups of the query; the
+ * host walks of getChanges and the copy of the returned changes are not in it */
+float amg_last_graph_ms(amg_backend* b);
 uint64_t amg_kernel_launches(amg_backend* b);
 /* labelled host wall-clock marks of the last applyChanges call ("label=ms ..."), development aid */
 size_t amg_debug_marks(amg_backend* b, char* buf, size_t cap);

@@ -7,9 +7,12 @@ the host path (Sync(device=False)), which copies, inflates and hashes every chan
   (c) (a) and (b) with device=False
 
 Wall clock per call: median of --reps repetitions (--host-reps for the host path) with the same sync state each time
-(neither call changes the document). Next to it: the device span of the engine's sync calls inside (CUDA events), and the
-one-time host hash graph (ensureGraph: getMissingDeps and getChangeByHash build it on their first call), timed on a fresh
-copy of the document.
+(neither call changes the document). Next to it: the device span of the engine's sync calls inside (CUDA events).
+
+Before that, the first call of each hash-graph query on a fresh copy of the document (the first query that walks the graph
+brings the engine's change graph up to date), wall clock and last_graph_ms (CUDA events), each on its own copy:
+  getMissingDeps([]); getChanges(haveDeps) on the fast path (haveDeps = the heads of a 99 % prefix); getChanges(haveDeps)
+  on the slow path (a hash concurrent to later changes); getChangeByHash.
 
   python tools/time_sync.py [--c3-ops 1000000] [--c4-ops 100000] [--reps 5] [--host-reps 1] [--out FILE.json]
 """
@@ -60,13 +63,23 @@ def run(cfg, n_ops, n_actors, reps, host_reps):
         d.apply_packed_flat(t.blob, t.offsets, t.n_changes, want_patch=False)
         return {'state': d, 'heads': d.heads()}
     res = {'config': cfg, 'ops': t.n_ops, 'changes': t.n_changes, 'change_bytes': int(t.offsets[-1])}
-    g = fresh()
-    t0 = time.perf_counter()
-    g['state'].get_missing_deps([])
-    res['ensure_graph_ms'] = (time.perf_counter() - t0) * 1e3
-    del g
+    metas = [sync._change_meta(c) for c in t.changes()]
+    prefix = metas[:len(metas) * 99 // 100]
+    dep = {d for m in prefix for d in m['deps']}
+    fast = sorted(m['hash'] for m in prefix if m['hash'] not in dep)
+    # a hash concurrent to later changes: one parent of the last merge in the 99 % prefix (the other parent is not its ancestor)
+    slow = [next(m for m in reversed(prefix) if len(m['deps']) >= 2)['deps'][0]]
+    first = {}
+    for name, query in (('missing_deps', lambda d: d.get_missing_deps([])), ('changes_fast', lambda d: d.get_changes(fast)),
+                        ('changes_slow', lambda d: d.get_changes(slow)), ('change_by_hash', lambda d: d.get_change_by_hash(metas[len(metas) // 3]['hash']))):
+        g = fresh()['state']
+        t0 = time.perf_counter()
+        out = query(g)
+        first[name] = {'wall_ms': (time.perf_counter() - t0) * 1e3, 'device_ms': g.last_graph_ms(), 'returned': len(out) if isinstance(out, list) else 1}
+        del g
+    res['first_call'] = first
+    print('%s first calls: %s' % (cfg, ', '.join('%s %.1f ms wall / %.2f ms device (%d)' % (k, v['wall_ms'], v['device_ms'], v['returned']) for k, v in first.items())), flush=True)
     a = fresh()
-    a['state'].get_missing_deps([])   # the graph is built once per document; (a) and (b) are timed after that
     hashes = a['state'].sync_changes_to_send([], [sync.BloomFilter(b'')], [])[1]
     rnd = random.Random(99)
     peer = {'heads': [], 'need': [], 'changes': [],
@@ -86,7 +99,7 @@ def run(cfg, n_ops, n_actors, reps, host_reps):
         print('%s %s: (a) %.1f ms wall, %.2f ms device | (b) %.1f ms wall, %.2f ms device' % (cfg, name, ta['wall_ms'], ta['device_ms'], tb['wall_ms'], tb['device_ms']), flush=True)
     res['messages_equal'] = msgs['device'] == msgs['host']
     assert res['messages_equal'], 'device and host messages differ'
-    print('%s: %d changes, ensureGraph %.1f ms, (b) sends %d changes, messages identical' % (cfg, t.n_changes, res['ensure_graph_ms'], res['b_changes_sent']), flush=True)
+    print('%s: %d changes, (b) sends %d changes, messages identical' % (cfg, t.n_changes, res['b_changes_sent']), flush=True)
     return res
 
 
@@ -98,7 +111,12 @@ def main():
     ap.add_argument('--host-reps', type=int, default=1)
     ap.add_argument('--out')
     args = ap.parse_args()
+    import subprocess
+    gpu = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True).stdout.strip()
+    print('GPU: %s' % gpu, flush=True)
     out = [run('C3', args.c3_ops, 10, args.reps, args.host_reps), run('C4', args.c4_ops, 100, args.reps, args.host_reps)]
+    for r in out:
+        r['gpu'] = gpu
     if args.out:
         with open(args.out, 'w') as f:
             json.dump(out, f, indent=1)
