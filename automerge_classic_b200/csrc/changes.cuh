@@ -166,8 +166,8 @@ struct ChgColumnsKernel {
       RleReader r(arena, co, ce, col == CX_CHLD_CTR ? 1 : 0); long long acc = 0;
       for (u32 k = 0; k < m; k++) {
         long long v = 0; u32 o, l; const bool nn = r.next(v, o, l);
-        if (col == CX_CHLD_CTR) { if (nn) { acc += v; if (acc < 0 || acc > 0xfffffffeLL) kerr = KE_TOO_LARGE; } chldCtr[base + k] = nn ? (u32)acc : NULL32; }
-        else { if (nn && (u64)v > 0xfffffffeULL) kerr = KE_TOO_LARGE; chldActor[base + k] = nn ? (u32)v : NULL32; }
+        if (col == CX_CHLD_CTR) { if (nn) { acc += v; if (acc < 0 || acc > 0xfffffffeLL) kerr = KE_TOO_LARGE; } chldCtr[base + k] = nn ? clamp_u32(acc) : NULL32; }
+        else { if (nn && (u64)v > 0xfffffffeULL) kerr = KE_TOO_LARGE; chldActor[base + k] = nn ? clamp_u32(v) : NULL32; }
       }
     } else {
       const int vr = CX_VAL_RAW;

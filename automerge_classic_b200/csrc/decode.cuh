@@ -43,8 +43,12 @@ enum KErr {
   KE_OBJ_MISMATCH, KE_KEY_MISMATCH, KE_ACTOR_INDEX, KE_TOO_LARGE, KE_UNKNOWN_ACTOR, KE_PRED_MISSING, KE_REF_ELEM, KE_DUP_OPID,
   KE_UNSUPPORTED_OP, KE_LAMPORT, KE_HASH_COLLISION, KE_LIST_ELEM, KE_PRED_ORDER, KE_DEFLATE, KE_UNKNOWN_COUNTER, KE_HIST_RANGE, KE_HIST_OPID, KE_HIST_DEP, KE_FLOAT_LEN /* columnar.js:316 */,
   KE_SUBARRAY,  // raw bytes (a string, a hash, a column, a chunk body) reach past the end: encoding.js:497, where a number that runs out is KE_TRUNCATED (:353)
-  KE_GROUP_COLUMN   // an unknown GROUP_CARD column in the group of known scalar columns: readOperation (new.js:576-597) would read those as arrays
+  KE_GROUP_COLUMN,  // an unknown GROUP_CARD column in the group of known scalar columns: readOperation (new.js:576-597) would read those as arrays
+  KE_COUNTER_RANGE  // a counter total that reaches a patch lies outside [-2^63, 2^63), the range of the patch's int64 field
 };
+// A column value the 32-bit row fields cannot hold (raised as KE_TOO_LARGE) is stored as 0xfffffffe: truncated it could
+// turn into the 0xffffffff null, or into another counter, and a check further on would report a different error first.
+HD u32 clamp_u32(long long v) { return (v < 0 || (u64)v > 0xfffffffeULL) ? 0xfffffffeu : (u32)v; }
 // error word: (code << 32 | item index); the smallest item index wins so that the error reported is
 // the one the sequential reference would hit first within a phase.
 HD void raise(u64* errWord, u32 code, u64 item) {
@@ -489,7 +493,7 @@ template <class S> HD u32 decode_one_column_t(const S& arena, int col, u32 nOps,
       for (u32 i = 0; i < nOps; i++) {
         long long n = 0; u32 o, l; const bool nn = r.next(n, o, l);
         if (nn && (u64)n > 0xfffffffeULL) kerr = KE_TOO_LARGE;
-        out[base + i] = nn ? (u32)n : NULL32;
+        out[base + i] = nn ? clamp_u32(n) : NULL32;
         if (col == CX_VAL_LEN) { rows.valOff[base + i] = rawBase + running; running += nn ? (u32)((u64)n >> 4) : 0; }
         if (col == CX_PRED_NUM) { rows.predOff[base + i] = rawBase + running; running += nn ? (u32)n : 0; if (!nn) out[base + i] = 0; }
       }
@@ -502,7 +506,7 @@ template <class S> HD u32 decode_one_column_t(const S& arena, int col, u32 nOps,
       for (u32 i = 0; i < nOps; i++) {
         long long n = 0; u32 o, l; const bool nn = r.next(n, o, l);
         if (nn) { acc += n; if (acc < 0 || acc > 0xfffffffeLL) kerr = KE_TOO_LARGE; }
-        rows.keyCtr[base + i] = nn ? (u32)acc : NULL32;
+        rows.keyCtr[base + i] = nn ? clamp_u32(acc) : NULL32;
       }
       if (!kerr) kerr = r.r.err;
       break;
@@ -539,8 +543,8 @@ template <class S> HD u32 decode_one_column_t(const S& arena, int col, u32 nOps,
       RleReaderT<S> r(arena, cOff, cEnd, col == CX_PRED_CTR ? 1 : 0); long long acc = 0;
       for (u32 j = 0; j < nPreds; j++) {
         long long n = 0; u32 o, l; const bool nn = r.next(n, o, l);
-        if (col == CX_PRED_CTR) { if (nn) { acc += n; if (acc < 0 || acc > 0xfffffffeLL) kerr = KE_TOO_LARGE; } rows.predCtr[predBase + j] = nn ? (u32)acc : NULL32; }
-        else { if (nn && (u64)n > 0xfffffffeULL) kerr = KE_TOO_LARGE; rows.predActor[predBase + j] = nn ? (u32)n : NULL32; }
+        if (col == CX_PRED_CTR) { if (nn) { acc += n; if (acc < 0 || acc > 0xfffffffeLL) kerr = KE_TOO_LARGE; } rows.predCtr[predBase + j] = nn ? clamp_u32(acc) : NULL32; }
+        else { if (nn && (u64)n > 0xfffffffeULL) kerr = KE_TOO_LARGE; rows.predActor[predBase + j] = nn ? clamp_u32(n) : NULL32; }
       }
       if (!kerr) kerr = r.r.err;
       break;

@@ -329,6 +329,7 @@ class Engine {
       case KE_HASH_COLLISION: throw Error(AMG_ERR_UNSUPPORTED, "amgpu: 64-bit string hash collision");
       case KE_GROUP_COLUMN: throw Error(AMG_ERR_UNSUPPORTED, "amgpu: a GROUP_CARD column of an unknown version in the group of known columns (the reference would read those as arrays)");
       case KE_UNSUPPORTED_OP: throw Error(AMG_ERR_UNSUPPORTED, "amgpu: operation pattern outside the incremental-patch subset (see DESIGN.md)");
+      case KE_COUNTER_RANGE: throw Error(AMG_ERR_UNSUPPORTED, "amgpu: a counter total outside [-2^63, 2^63) (the patch holds counters as int64)");
       default: throw Error(AMG_ERR_INTERNAL, "amgpu: kernel error " + std::to_string(code));
     }
   }

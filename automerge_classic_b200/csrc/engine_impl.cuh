@@ -861,7 +861,7 @@ inline void Engine::buildPatch(const PatchInputs& in, PatchOut& out) {
   scan_exclusive(ctx, scanTmp, emit.p, slot.p, N);
   const size_t numProps = readU32(slot.p + N);
   propOut.ensure(ctx, numProps + 1);
-  foreach(ctx, N, PropEmitKernel{d, emit.p, marker.p, slot.p, propOut.p, counterLast.p, counterTotal.p});
+  foreach(ctx, N, PropEmitKernel{d, emit.p, marker.p, slot.p, propOut.p, counterLast.p, counterTotal.p, errWord.p});
   trace.phase("patch:list-index");
   // ---- list edits
   size_t numEdits = 0; bool shipElem = true;
@@ -875,7 +875,7 @@ inline void Engine::buildPatch(const PatchInputs& in, PatchOut& out) {
     scan_exclusive(ctx, scanTmp, rowEmit.p, slot.p, N);
     numEdits = readU32(slot.p + N);
     editOut.ensure(ctx, numEdits + 1); editElem.ensure(ctx, numEdits + 1);
-    foreach(ctx, N, DocEditEmitKernel{d, rowEmit.p, slot.p, elemVisScan.p, objIdx.p, objStart.p, groupOf.p, groupFirst.p, rowClass.p, firstVis.p, firstBare.p, editOut.p, counterOwner.p, counterTotal.p});
+    foreach(ctx, N, DocEditEmitKernel{d, rowEmit.p, slot.p, elemVisScan.p, objIdx.p, objStart.p, groupOf.p, groupFirst.p, rowClass.p, firstVis.p, firstBare.p, editOut.p, counterOwner.p, counterTotal.p, errWord.p});
     foreach(ctx, N, EditElemKernel{d, rowEmit.p, slot.p, groupOf.p, groupFirst.p, editElem.p});
   } else {
     size_t numGroupRecs = 0, numLink = 0, numLive = 0;

@@ -217,25 +217,40 @@ HD long long counter_operand(const u8* arena, u32 valLen, u32 valOff) {
   ByteReader br(arena, valOff, valOff + (valLen >> 4));
   return tag == 3 ? (long long)br.uleb() : br.sleb();
 }
+// A counter's total is a JavaScript number in the reference: the operands (53-bit integers, exact in a double) are added
+// as doubles, in document order - the counter's `set` row first, then its increments by opId - so a total past 2^53 is
+// rounded at each step exactly as the reference rounds it. The patch carries the total as an int64, which holds every
+// such double in [-2^63, 2^63); a total outside that range is refused (KE_COUNTER_RANGE, DESIGN.md section 5).
+HD u64 counter_bits(double v) { u64 b; memcpy(&b, &v, 8); return b; }
+HD bool counter_int64(u64 bits, long long* out) {
+  double v; memcpy(&v, &bits, 8);
+  if (!(v >= -9223372036854775808.0 && v < 9223372036854775808.0)) return false;
+  *out = (long long)v; return true;
+}
 // Counters (new.js:941-966): increments are successors of the `set` that created the counter. The counter shows with the
 // summed value once every successor turned out to be an `inc`; the reference emits it while processing the last of them.
 struct CounterKernel {
   const u8* arena; DocRows d; const u32* succOff; const u64* succ; const u32* groupOf; const u32* groupFirst; const u32* groupRows;
-  u32* counterLast /* position of the last inc row, ROW_NONE = not a visible counter */; u64* counterTotal; u32* counterOwner /* per inc row that completes a counter: the counter's row */;
+  u32* counterLast /* position of the last inc row, ROW_NONE = not a visible counter */; u64* counterTotal /* double bits */; u32* counterOwner /* per inc row that completes a counter: the counter's row */;
   HD long long valueOf(u32 r) const { return counter_operand(arena, d.valLen[r], d.valOff[r]); }
   HD void operator()(size_t p) const {
     counterLast[p] = ROW_NONE;
     if (flags_action(d.flags[p]) != ACT_SET || (d.valLen[p] & 15) != 8) return;
     const u32 s0 = succOff[p], s1 = succOff[p + 1]; if (s0 == s1) return;
     const u32 g = groupOf[p], gf = groupFirst[g], rows = groupRows[g];
-    long long total = valueOf((u32)p); u32 last = 0;
+    u32 last = 0;
     for (u32 s = s0; s < s1; s++) {
       u32 r = ROW_NONE;
       for (u32 q = gf; q < gf + rows; q++) if (d.id[q] == succ[s]) { r = q; break; }
       if (r == ROW_NONE || flags_action(d.flags[r]) != ACT_INC) return;   // deleted or overwritten: the counter is gone
-      total += valueOf(r); if (r > last) last = r;
+      if (r > last) last = r;
     }
-    counterLast[p] = last; counterTotal[p] = (u64)total; counterOwner[last] = (u32)p;
+    double total = (double)valueOf((u32)p);
+    for (u32 q = (u32)p + 1; q <= last; q++) {   // the increments in row (= opId) order
+      bool mine = false; for (u32 s = s0; s < s1 && !mine; s++) mine = d.id[q] == succ[s];
+      if (mine) total += (double)valueOf(q);
+    }
+    counterLast[p] = last; counterTotal[p] = counter_bits(total); counterOwner[last] = (u32)p;
   }
 };
 struct PropFlagKernel {   // which positions emit a prop record
@@ -267,12 +282,15 @@ struct PropMarkerKernel {   // a touched key with nothing to show is reported as
   }
 };
 struct PropEmitKernel {
-  DocRows d; const u32* emit; const u32* marker; const u32* slot; PropRec* out; const u32* counterLast; const u64* counterTotal;
+  DocRows d; const u32* emit; const u32* marker; const u32* slot; PropRec* out; const u32* counterLast; const u64* counterTotal; u64* errWord;
   HD void operator()(size_t p) const {
     if (!emit[p]) return;
     PropRec r; r.obj = d.obj[p]; r.opId = d.id[p]; r.keyOff = d.keyStrOff[p]; r.keyLen = d.keyStrLen[p]; r.valLen = d.valLen[p]; r.valOff = d.valOff[p];
     r.flags = (flags_action(d.flags[p]) << 8) | (marker[p] ? 1u : 0u); r.pad = 0;
-    if (!marker[p] && counterLast[p] != ROW_NONE) { r.flags |= 2u; r.valOff = (u32)counterTotal[p]; r.pad = (u32)(counterTotal[p] >> 32); }   // summed counter value instead of arena bytes
+    if (!marker[p] && counterLast[p] != ROW_NONE) {   // summed counter value instead of arena bytes
+      long long total = 0; if (!counter_int64(counterTotal[p], &total)) raise(errWord, KE_COUNTER_RANGE, p);
+      r.flags |= 2u; r.valOff = (u32)(u64)total; r.pad = (u32)((u64)total >> 32);
+    }
     out[slot[p]] = r;
   }
 };
@@ -318,7 +336,7 @@ struct ObjStartKernel {   // objIdx = exclusive scan of heads (+head-1 fix-up); 
 struct DocEditEmitKernel {   // getPatch: visible rows of list objects in document order
   DocRows d; const u32* rowEmit; const u32* slot; const u32* elemVisScan /* exclusive */; const u32* objIdx; const u32* objStart;
   const u32* groupOf; const u32* groupFirst; const u32* rowClass; const u32* firstPv; const u32* firstBare; EditRec* out;
-  const u32* counterOwner; const u64* counterTotal;
+  const u32* counterOwner; const u64* counterTotal; u64* errWord;
   HD void operator()(size_t p) const {
     if (!rowEmit[p]) return;
     const u32 g = groupOf[p]; const u32 gp = groupFirst[g];
@@ -328,7 +346,10 @@ struct DocEditEmitKernel {   // getPatch: visible rows of list objects in docume
     if (rowClass[p] == 2) { e.kind = (u32)EK_REMOVE | (ACT_DEL << 16); e.valLen = 0; e.valOff = 0; out[slot[p]] = e; return; }
     const u32 kind = (firstPv[g] == (u32)p && !(firstBare[g] < (u32)p)) ? EK_INSERT : EK_UPDATE;
     e.kind = kind | (flags_action(d.flags[src]) << 16); e.valLen = d.valLen[src]; e.valOff = d.valOff[src];
-    if (src != (u32)p) { e.kind |= EF_COUNTER; e.valLen = (u32)counterTotal[src]; e.valOff = (u32)(counterTotal[src] >> 32); }
+    if (src != (u32)p) {
+      long long total = 0; if (!counter_int64(counterTotal[src], &total)) raise(errWord, KE_COUNTER_RANGE, p);
+      e.kind |= EF_COUNTER; e.valLen = (u32)(u64)total; e.valOff = (u32)((u64)total >> 32);
+    }
     out[slot[p]] = e;
   }
 };
@@ -353,22 +374,27 @@ struct ListCtx {
   HD long long valueOf(u32 r) const { return counter_operand(arena, d.valLen[r], d.valOff[r]); }
   HD bool isCounterRow(u32 r) const { return flags_action(d.flags[r]) == ACT_SET && (d.valLen[r] & 15) == 8; }
   // Counter row c of the element [e, e + rows) at time T: true if it has increments by then and nothing else overwrote it;
-  // *total = summed value, *lastInc = position of the latest of those increments (new.js:941-966).
-  HD bool counterAt(u32 e, u32 rows, u32 c, u32 T, long long* total, u32* lastInc) const {
-    long long sum = valueOf(c); u32 last = ROW_NONE;
+  // *total = summed value (double bits, counter_bits), *lastInc = position of the latest of those increments (new.js:941-966).
+  HD bool counterAt(u32 e, u32 rows, u32 c, u32 T, u64* total, u32* lastInc) const {
+    u32 last = ROW_NONE;
     for (u32 s = succOff[c]; s < succOff[c + 1]; s++) {
       if (succTime[s] > T) continue;
       u32 q = ROW_NONE;
       for (u32 r = e; r < e + rows; r++) if (d.id[r] == succ[s]) { q = r; break; }
       if (q == ROW_NONE || flags_action(d.flags[q]) != ACT_INC) return false;
-      sum += valueOf(q); if (last == ROW_NONE || q > last) last = q;
+      if (last == ROW_NONE || q > last) last = q;
     }
     if (last == ROW_NONE) return false;
-    *total = sum; *lastInc = last; return true;
+    double sum = (double)valueOf(c);
+    for (u32 q = c + 1; q <= last; q++) {   // the increments present at T, in row (= opId) order
+      bool mine = false; for (u32 s = succOff[c]; s < succOff[c + 1] && !mine; s++) mine = succTime[s] <= T && d.id[q] == succ[s];
+      if (mine) sum += (double)valueOf(q);
+    }
+    *total = counter_bits(sum); *lastInc = last; return true;
   }
   // What the element shows at position q at time T: 1 = the row's own value, 2 = a counter completed by the increment
   // sitting at q (*owner = the counter's row), 0 = nothing
-  HD int shownAt(u32 e, u32 rows, u32 q, u32 T, u32* owner, long long* total) const {
+  HD int shownAt(u32 e, u32 rows, u32 q, u32 T, u32* owner, u64* total) const {
     if (d.time[q] > T) return 0;
     const u32 a = flags_action(d.flags[q]);
     if (a == ACT_INC) {
@@ -480,7 +506,7 @@ struct ListGroupKernel {
           for (u32 r = e; r < e + rows; r++) {
             const u32 s = L.d.time[r], x = L.minSucc(r);
             if (s < T0 && x >= T0) W = true;
-            u32 owner; long long total;
+            u32 owner; u64 total;
             if (L.shownAt(e, rows, r, T1, &owner, &total)) nV++;
           }
           n = nV ? nV : (W ? 1u : 0u);
@@ -530,12 +556,15 @@ struct ListGroupKernel {
     }
     u32 k = gBase[t0], nV = 0;
     for (u32 q = e; q < e + rows; q++) {
-      u32 owner = 0; long long total = 0; const int what = L.shownAt(e, rows, q, T1, &owner, &total);
+      u32 owner = 0; u64 total = 0; const int what = L.shownAt(e, rows, q, T1, &owner, &total);
       if (!what) continue;
       const u32 r = what == 2 ? owner : q;
       EditRec rec; rec.obj = L.d.obj[r]; rec.opId = L.d.id[r]; rec.index = q == e ? headIdx : idx; rec.valLen = L.d.valLen[r]; rec.valOff = L.d.valOff[r];
       rec.kind = (nV == 0 ? (W ? (u32)EK_UPDATE | EF_POP : (u32)EK_INSERT) | EF_GROUP_FIRST : (u32)EK_UPDATE) | (flags_action(L.d.flags[r]) << 16);
-      if (what == 2) { rec.kind |= EF_COUNTER; rec.valLen = (u32)(u64)total; rec.valOff = (u32)((u64)total >> 32); }
+      if (what == 2) {
+        long long v = 0; if (!counter_int64(total, &v)) raise(errWord, KE_COUNTER_RANGE, t0);
+        rec.kind |= EF_COUNTER; rec.valLen = (u32)(u64)v; rec.valOff = (u32)((u64)v >> 32);
+      }
       out[k] = rec; elemOut[k] = L.d.id[e]; objKeyOut[k] = objIdx[e]; elemPosOut[k] = e; rowPosOut[k] = r; k++; nV++;
     }
     if (nV == 0) {

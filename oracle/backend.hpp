@@ -78,7 +78,9 @@ static void convertInsertToUpdate(std::vector<Edit>& edits, int64_t index, const
   for (auto& u : updates) { appendUpdate(edits, index, elemId, u.opId, u.value, firstUpdate); firstUpdate = false; }
 }
 
-struct CounterState { std::string opId; double value = 0; bool isInt = true; int64_t ivalue = 0; std::set<std::string> succs; };
+// value is a JavaScript number, as in the reference: `counterState.value += ...` (new.js:944, 958) adds doubles, so a total
+// past 2^53 is rounded at each step
+struct CounterState { std::string opId; double value = 0; std::set<std::string> succs; };
 struct PropState {
   std::vector<Op> visibleOps; bool hasChild = false; int action = 0;   // 0 none, 1 insert, 2 update, 3 remove
   std::map<std::string, std::shared_ptr<CounterState>> counterStates; bool hasCounterStates = false;
@@ -130,7 +132,7 @@ static void updatePatchProperty(Patches& patches, Block* newBlock, const std::st
     // The initial set operation that creates a counter
     ps.hasCounterStates = true;
     auto cs = std::make_shared<CounterState>(); cs->opId = opId;
-    Prim p = decodeValue(op.valLen, op.valRaw); cs->ivalue = p.i;
+    Prim p = decodeValue(op.valLen, op.valRaw); cs->value = p.num();
     for (int64_t i = 0; i < op.succNum(); i++) {
       const std::string succOp = opIdStr(op.succCtr[i], ds.actorOf(op.succActor[i]));
       ps.counterStates[succOp] = cs; cs->succs.insert(succOp);
@@ -138,10 +140,13 @@ static void updatePatchProperty(Patches& patches, Block* newBlock, const std::st
   } else if (op.action == A_INC) {
     if (!ps.hasCounterStates || !ps.counterStates.count(opId)) throw RangeError("increment operation " + opId + " for unknown counter");
     auto cs = ps.counterStates[opId];
-    Prim p = decodeValue(op.valLen == NUL ? 0 : op.valLen, op.valRaw); cs->ivalue += p.i;
+    Prim p = decodeValue(op.valLen == NUL ? 0 : op.valLen, op.valRaw); cs->value += p.k == Prim::P_BOOL ? (p.b ? 1.0 : 0.0) : p.num();
     cs->succs.erase(opId);
     if (cs->succs.empty()) {
-      hasPatch = true; patchKey = cs->opId; patchValue.prim.k = Prim::P_INT; patchValue.prim.i = cs->ivalue; patchValue.prim.datatype = "counter";
+      // an integer-valued double in [-2^63, 2^63) is written as that integer, exactly; a larger one as a float
+      hasPatch = true; patchKey = cs->opId; patchValue.prim.datatype = "counter";
+      if (cs->value >= -9223372036854775808.0 && cs->value < 9223372036854775808.0) { patchValue.prim.k = Prim::P_INT; patchValue.prim.i = (int64_t)cs->value; }
+      else { patchValue.prim.k = Prim::P_FLOAT; patchValue.prim.f = cs->value; }
     }
   } else if (!isOverwritten) {
     if (op.action == A_SET) { hasPatch = true; patchKey = opId; patchValue = primVal(op); }
@@ -685,7 +690,7 @@ struct BackendDoc {
       dependenciesByHash[change.hash] = change.deps; dependentsByHash[change.hash];
       for (auto& dep : change.deps) dependentsByHash[dep].push_back(change.hash);
       // appendChange new.js:1680-1692
-      ChangeMeta m; m.actor = -1; for (size_t i = 0; i < ds.actorIds.size(); i++) if (ds.actorIds[i] == change.actor) m.actor = (int64_t)i;
+      ChangeMeta m; m.actor = ds.indexOfActor(change.actor);   // (actorIds holds each id once)
       m.seq = change.seq; m.maxOp = change.maxOp; m.time = change.time; m.message = change.message;
       for (auto& dep : change.deps) m.depsIndex.push_back(changeIndexByHash.count(dep) ? changeIndexByHash[dep] : NUL);
       m.extra = change.extraBytes; changeMetas.push_back(m);

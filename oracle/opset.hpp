@@ -131,7 +131,20 @@ struct DocState {
   std::vector<int> extraColumnIds;   // unknown column ids present in the doc (sorted)
   std::unordered_map<std::string, int64_t>* changeIndexByHash = nullptr;
   const std::string& actorOf(int64_t n) const { static const std::string undef = "undefined"; return (n >= 0 && n < (int64_t)actorIds.size()) ? actorIds[n] : undef; }
-  int64_t indexOfActor(const std::string& a) const { for (size_t i = 0; i < actorIds.size(); i++) if (actorIds[i] == a) return (int64_t)i; return -1; }
+  // actorIds.indexOf(a): the first index holding a, or -1. A DocState only appends to actorIds after filling it, so the
+  // index map is extended with the new entries; it is rebuilt if the vector shrank. (A linear scan per change made a call
+  // that brings tens of thousands of new actors quadratic.)
+  int64_t indexOfActor(const std::string& a) const {
+    if (actorIndexed > actorIds.size()) { actorIndex.clear(); actorIndexed = 0; }
+    for (; actorIndexed < actorIds.size(); actorIndexed++) actorIndex.emplace(actorIds[actorIndexed], (int64_t)actorIndexed);
+    auto it = actorIndex.find(a);
+    if (it != actorIndex.end() && actorIds[it->second] == a) return it->second;
+    if (it == actorIndex.end()) return -1;
+    for (size_t i = 0; i < actorIds.size(); i++) if (actorIds[i] == a) return (int64_t)i;   // the vector was rewritten in place
+    return -1;
+  }
+  mutable std::unordered_map<std::string, int64_t> actorIndex;
+  mutable size_t actorIndexed = 0;
 };
 
 struct SeekOps {   // the `ops` argument of seekToOp / seekWithinBlock (new.js:1308-1312)
