@@ -338,6 +338,9 @@ class Engine {
   // ---------------------------------------------------------------- helpers
   DBuf<u64> gateBest;   // causal gate with several copies of a waiting change: best (pass, position) per hash
   bool domLocalReady = false;   // k_dom_local's dynamic shared memory size has been raised on this device
+#ifndef AMG_EMU
+  DomPassTemp domPass;          // dominance count: look-back state and parked items of the global passes
+#endif
   std::vector<HostChange> batchStore;   // applyChanges: (offset, length) of the batch entries
   HBuf<HostChange> pairStage;           // the same table in pinned memory: uploaded by DMA
   HBuf<u32> pinnedScratch; HBuf<u64> hostWord;   // pinned landing slots for the small device -> host reads that size the next stage

@@ -639,14 +639,21 @@ inline void Engine::orderOpSet(ApplyCall& a) {
     foreach(ctx, I, ItemIndexKernel{sortVals.p, itemIdx.p});
     foreach(ctx, N, ListObjFlagKernel{w, emit.p}); scan_exclusive(ctx, scanTmp, emit.p, objSlot.p, N);
     const size_t Lo = readU32(objSlot.p + N);
-    const size_t S = 2 * I + 2 * Lo; eNext.ensure(ctx, S + 1); eRank.ensure(ctx, S + 1); ePacked.ensure(ctx, S + 1); ePacked2.ensure(ctx, S + 1);
+    const size_t S = 2 * I + 2 * Lo; eNext.ensure(ctx, S + 1); eRank.ensure(ctx, S + 1); ePacked.ensure(ctx, S + 1);
     foreach(ctx, S, EulerInitKernel{eNext.p, eRank.p});
     foreach(ctx, I, EulerLinkKernel{sortKeys.p, ordBits, itemIdx.p, objSlot.p, eNext.p, eRank.p, I});
     foreach(ctx, S, ListRankPackKernel{eNext.p, eRank.p, ePacked.p});
     const int rounds = bits_for(S);
+#ifdef AMG_EMU
+    ePacked2.ensure(ctx, S + 1);
+#endif
     for (int k = 0; k < rounds; k++) {
+#ifdef AMG_EMU
       foreach(ctx, S, ListRankPackedKernel{ePacked.p, ePacked2.p});
       ePacked.swap(ePacked2);
+#else
+      foreach(ctx, S, ListRankInPlaceKernel{ePacked.p});
+#endif
     }
     foreach(ctx, S, ListRankUnpackKernel{ePacked.p, eRank.p});
     foreach(ctx, N, ListPosKernel{eRank.p, elemRow.p, objRow.p, itemIdx.p, objSlot.p, (u32)I, listPos.p});
@@ -904,14 +911,15 @@ inline void Engine::buildPatch(const PatchInputs& in, PatchOut& out) {
 #else
       const int localBits = std::min(tbits, DOM_LOCAL_BITS);   // the last levels run inside shared memory (k_dom_local)
 #endif
+#ifdef AMG_EMU
       for (int bit = tbits - 1; bit >= localBits; bit--) {
         scan_exclusive64(ctx, scanTmp, DomScanInput{domTw.p, domW.p, bit}, zwScan.p, T);
         foreach(ctx, T, DomLevelKernel{items.p, items2.p, domTw2.p, domW2.p, zwScan.p, bit});
         items.swap(items2); domTw.swap(domTw2); domW.swap(domW2);
       }
-#ifdef AMG_EMU
       foreach(ctx, T, DomResultKernel{items.p, qIndex.p});
 #else
+      dom_global_passes(ctx, domPass, items, items2, T, tbits, localBits);   // the global levels, DOM_PASS_BITS time bits per pass
       {   // partition heads -> compact list (device-side count), then one CTA per partition
         DBuf<u32>& partFlag = domTw2; DBuf<u32>& partScan = nItems; DBuf<u32>& partHead = itemBase;   // scratch that is free by now
         partScan.ensure(ctx, T + 2); partHead.ensure(ctx, T + 2);

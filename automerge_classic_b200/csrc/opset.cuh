@@ -9,7 +9,8 @@
 // RGA order equals the pre-order of the insertion tree with siblings in descending opId order,
 // provided every insert has a greater counter than its reference element (Lamport property; checked
 // in ResolveRowsKernel, KE_LAMPORT otherwise). The pre-order is computed with an Euler tour over
-// 4 slots per row and Wyllie pointer jumping (ListRankPackedKernel), log2(n) passes.
+// 4 slots per row and Wyllie pointer jumping, log2(n) passes (ListRankInPlaceKernel on the device, ListRankPackedKernel in
+// the emulation build).
 #pragma once
 #include "gate.cuh"
 
@@ -196,6 +197,18 @@ struct ListRankPackedKernel {
     if (n == (u32)s) { out[s] = me; return; }
     const u64 nb = in[n];
     out[s] = (u64)(u32)nb | ((u64)((u32)(me >> 32) + (u32)(nb >> 32)) << 32);
+  }
+};
+// The device runs the same jump on one array, in place: a word read while another thread rewrites it is either its old or
+// its new (next, weight up to next) pair, both consistent and at least as far along as at the launch's start, so a round
+// covers at least what a round over two buffers does, and the last round leaves the same ranks.
+struct ListRankInPlaceKernel {
+  u64* packed;
+  HD void operator()(size_t s) const {
+    const u64 me = packed[s]; const u32 n = (u32)me;
+    if (n == (u32)s) return;
+    const u64 nb = packed[n];
+    packed[s] = (u64)(u32)nb | ((u64)((u32)(me >> 32) + (u32)(nb >> 32)) << 32);
   }
 };
 struct ListRankUnpackKernel { const u64* packed; u32* rank; HD void operator()(size_t s) const { rank[s] = (u32)(packed[s] >> 32); } };

@@ -447,6 +447,8 @@ struct DomScanInput {   // per level: low word = 1 if the time bit is clear, hig
   const u32* tw; const int* w; int bit;
   HD u64 operator()(size_t i) const { return ((tw[i] >> bit) & 1u) == 0 ? (1ull | ((u64)(u32)w[i] << 32)) : 0ull; }
 };
+// (the emulation build runs every level this way; the device build runs the global levels DOM_PASS_BITS bits at a time,
+// k_dom_pass_tile in domlocal.cuh)
 struct DomLevelKernel {   // accumulate + stable split of every partition on `bit`; ZW = packed exclusive scan of DomScanInput
   const DomItem* in; DomItem* out; u32* twOut; int* wOut; const u64* ZW; int bit;
   HD void operator()(size_t i) const {
