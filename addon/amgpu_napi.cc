@@ -265,13 +265,19 @@ napi_value HistoryPatches(napi_env env, napi_callback_info info) {
   if (amg_get_history_patches(b, lens.data(), n, &l, &err)) return throwAmg(env, err);
   return buffersToJs(env, l);
 }
-// merge(state, other) — src/automerge.js:61-67 at the backend level: applies the changes of `other` that `state` lacks,
-// copied device to device (amg_merge); returns the flat patch applyChanges returns. Documents on different devices throw an
-// Error with code 'AMG_UNSUPPORTED' and change nothing (js/index.js then applies getChangesAdded itself).
-napi_value Merge(napi_env env, napi_callback_info info) {
-  napi_value argv[2]; amg_backend *dst, *src; if (!getArgs(env, info, 2, argv) || !getBackend(env, argv[0], &dst) || !getBackend(env, argv[1], &src)) return nullptr;
+// mergeMany(state, others) — src/automerge.js:61-67 at the backend level, folded over an array of backend states in one
+// apply (amg_merge_many): the changes of each that `state` and the earlier ones lack, copied device to device, a change
+// several hold sent once. Returns the flat patch applyChanges returns for that list. A document on another device throws an
+// Error with code 'AMG_UNSUPPORTED' and changes nothing (js/index.js then applies the changes itself).
+napi_value MergeMany(napi_env env, napi_callback_info info) {
+  napi_value argv[2]; amg_backend* dst; if (!getArgs(env, info, 2, argv) || !getBackend(env, argv[0], &dst)) return nullptr;
+  bool isArray = false; napi_is_array(env, argv[1], &isArray);
+  if (!isArray) { napi_throw_type_error(env, nullptr, "expected an array of backend states"); return nullptr; }
+  uint32_t n = 0; napi_get_array_length(env, argv[1], &n);
+  std::vector<amg_backend*> srcs(n);
+  for (uint32_t i = 0; i < n; i++) { napi_value v; napi_get_element(env, argv[1], i, &v); if (!getBackend(env, v, &srcs[i])) return nullptr; }
   amg_patch* patch = nullptr; amg_error err;
-  if (amg_merge(dst, src, 1, &patch, &err)) {
+  if (amg_merge_many(dst, srcs.data(), n, 1, &patch, &err)) {
     if (err.code == AMG_UNSUPPORTED) { napi_throw_error(env, "AMG_UNSUPPORTED", err.msg); return nullptr; }
     return throwAmg(env, err);
   }
@@ -304,7 +310,7 @@ napi_value InitModule(napi_env env, napi_value exports) {
     {"getHeads", GetHeads}, {"getChanges", GetChanges}, {"getChangesAdded", GetChangesAdded}, {"getChangeByHash", GetChangeByHash},
     {"getMissingDeps", GetMissingDeps}, {"clockOf", ClockOf}, {"hashByActor", HashByActor}, {"syncBloom", SyncBloom},
     {"syncChangesToSend", SyncChangesToSend}, {"decodeChanges", DecodeChanges}, {"decodeHistory", DecodeHistory},
-    {"encodeChanges", EncodeChanges}, {"historyPatches", HistoryPatches}, {"merge", Merge},
+    {"encodeChanges", EncodeChanges}, {"historyPatches", HistoryPatches}, {"mergeMany", MergeMany},
     {"applyLocalChangeTable", ApplyLocalChangeTable}};
   for (auto& f : fns) { napi_value fn; napi_create_function(env, f.name, NAPI_AUTO_LENGTH, f.fn, nullptr, &fn); napi_set_named_property(env, exports, f.name, fn); }
   return exports;

@@ -75,25 +75,43 @@ def getHistory(backend):
     return [HistoryEntry(history, i) for i in range(n)]
 
 
-def merge(local, remote):
-    """Automerge.merge (src/automerge.js:61-67) at the backend level: [newLocalHandle, patch], where the patch is the one
-    applyChanges(local, getChangesAdded(local, remote)) returns. The changes go from remote's device memory to local's
-    without leaving the device. The local handle is frozen, as applyChanges freezes it; remote is not changed. When the
-    document class has no device merge, or the engine declines (Unsupported, e.g. documents on different devices), the
-    changes take the host route."""
-    state, other = _backend_state(local), _backend_state(remote)
+def changes_added(state, others):
+    """The changes a merge of `others` into `state` applies, on the host: getChangesAdded(state, other) for each document in
+    turn, without the changes an earlier one already contributes (compared by change hash). Applied to `state` in one call,
+    they give what merging the documents one after the other gives (see merge)."""
+    if len(others) == 1:
+        return others[0].get_changes_added(state)   # nothing to compare with
+    sent, out = set(), []
+    for other in others:
+        for change in other.get_changes_added(state):
+            h = _sync._change_meta(change)['hash']
+            if h not in sent:
+                sent.add(h)
+                out.append(change)
+    return out
+
+
+def merge(local, *remotes):
+    """Automerge.merge (src/automerge.js:61-67) at the backend level, folded over one or more remotes in one apply:
+    [newLocalHandle, patch], where the patch is the one applyChanges(local, L) returns, L being changes_added(local,
+    remotes). The resulting document equals merging the remotes one by one in order, except that a queued change of local
+    that becomes applicable part-way through that fold is not re-sent by it but may be in L (the apply drops the copy).
+    The changes go from the remotes' device memory to local's without leaving the device. The local handle is frozen, as
+    applyChanges freezes it; the remotes are not changed. When the document class has no device merge, or the engine
+    declines (Unsupported, e.g. documents on different devices), the changes take the host route."""
+    state, others = _backend_state(local), [_backend_state(r) for r in remotes]
     patch = None
-    if hasattr(state, 'merge'):
+    if hasattr(state, 'merge_many'):
         try:
-            patch = state.merge(other)
+            patch = state.merge_many(others)
         except Unsupported:
             pass   # nothing changed: the host route below
     if patch is None:
-        patch = state.apply_changes(other.get_changes_added(state))
+        patch = state.apply_changes(changes_added(state, others))
     local['frozen'] = True
     return [{'state': state, 'heads': state.heads()}, patch]
 
 
 Backend = bind_sync(_Facade(GpuBackendDoc))
 __all__ = ['Backend', 'GpuBackendDoc', 'AmgError', 'Unsupported', 'bind_sync', 'decodeChange', 'decodeChanges', 'encodeChange', 'encodeChanges',
-           'getHistory', 'HistoryEntry', 'merge']
+           'getHistory', 'HistoryEntry', 'merge', 'changes_added']

@@ -217,12 +217,17 @@ float amg_last_history_ms(amg_backend* b) { return b->eng.spans.ms[SPAN_HISTORY]
 // new.js:1979-1997: the changes in their order from Engine::changesAddedFrom (no host hash graph is built)
 int amg_get_changes_added(amg_backend* bn, amg_backend* bo, amg_buffers** out, amg_error* err) {
   AMG_GUARD(
-    std::vector<u32> idx; bo->eng.changesAddedFrom(bn->eng, idx);
-    *out = buffers([&](Items& l) { for (u32 i : idx) l.push_back(bn->changeBytes(i)); }).release(); return 0;)
+    Engine* src = &bn->eng; std::vector<Engine::MergePick> picks; bo->eng.changesAddedFrom(&src, 1, picks);
+    *out = buffers([&](Items& l) { for (const Engine::MergePick& m : picks) l.push_back(bn->changeBytes(m.idx)); }).release(); return 0;)
 }
 // src/automerge.js:61-67 merge(local, remote): applyChanges(local, getChangesAdded(local, remote)), the bytes device to device
 int amg_merge(amg_backend* dst, amg_backend* src, int want_patch, amg_patch** out, amg_error* err) {
-  AMG_GUARD(PatchOut p; dst->eng.mergeFrom(src->eng, want_patch != 0, p);
+  return amg_merge_many(dst, &src, 1, want_patch, out, err);
+}
+// the same folded over n remotes in one applyChanges (Engine::changesAddedFrom drops the changes an earlier remote sends)
+int amg_merge_many(amg_backend* dst, amg_backend* const* srcs, size_t n, int want_patch, amg_patch** out, amg_error* err) {
+  AMG_GUARD(std::vector<Engine*> engs(n); for (size_t s = 0; s < n; s++) engs[s] = &srcs[s]->eng;
+            PatchOut p; dst->eng.mergeFrom(engs.data(), n, want_patch != 0, p);
             if (out) *out = want_patch ? serialize(p) : nullptr; return 0;)
 }
 float amg_last_merge_ms(amg_backend* b) { return b->eng.spans.ms[SPAN_MERGE]; }

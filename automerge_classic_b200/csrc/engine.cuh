@@ -541,13 +541,17 @@ class Engine {
   DocBufs snapDoc; DBuf<u32> snapSuccOff, snapSuccCnt; DBuf<u64> snapSucc;   // the prefix document (grow-only; never the document's own)
 
   // ---------------------------------------------------------------- merge (merge.cuh)
-  // The applied changes of `src` this document lacks, as indexes into src.changes, in the order getChangesAdded returns
-  // them (new.js:1979-1997). Runs on this engine's stream and scratch; src is only read (its history is rebuilt first when
-  // it was loaded, as getChangesAdded does). Both documents must be on the same device (AMG_ERR_UNSUPPORTED otherwise).
-  void changesAddedFrom(Engine& src, std::vector<u32>& order);
-  // Automerge.merge (src/automerge.js:61-67): those changes, gathered from src's arena into one device blob, through applyChanges
-  void mergeFrom(Engine& src, bool wantPatch, PatchOut& out);
-  DBuf<u32> mergeAbsent, mergeSlot, mergeList, mergeHeadIdx; DBuf<u8> mergeHeads, mergeBlob; DBuf<MergeRange> mergeRanges;
+  // The applied changes of n sources this document lacks, as (source, index into that source's changes) pairs: walk_0 ++
+  // walk_1 ++ ..., where walk_s holds the changes of srcs[s] whose hash is neither applied here nor in an earlier walk, in
+  // the order getChangesAdded returns them (new.js:1979-1997). With one source this is getChangesAdded(this, src). Runs on
+  // this engine's stream and scratch; the sources are only read (a loaded one has its history rebuilt first, as
+  // getChangesAdded does). Every source must be on this document's device (AMG_ERR_UNSUPPORTED otherwise).
+  struct MergePick { u32 src, idx; };
+  void changesAddedFrom(Engine* const* srcs, size_t n, std::vector<MergePick>& order);
+  // Automerge.merge (src/automerge.js:61-67) folded over the sources: those changes, gathered from the sources' arenas into
+  // one device blob, through one applyChanges
+  void mergeFrom(Engine* const* srcs, size_t n, bool wantPatch, PatchOut& out);
+  DBuf<u32> mergeAbsent, mergeSlot, mergeList, mergeFirst, mergeHeadIdx; DBuf<u8> mergeHeads, mergeCand, mergeBlob; DBuf<MergeRange> mergeRanges;
 
   // ---------------------------------------------------------------- applyLocalChange (backend.js:54-91)
   // One change request (a change table holding one change) encoded on the device with the author's previous change hash as

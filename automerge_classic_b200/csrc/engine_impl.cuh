@@ -2415,70 +2415,114 @@ inline void Engine::snapHeader(HistoryPatchCall& h, size_t k, PatchOut& out) {
 // after its dependencies, so every ancestor of a change this document has is here as well, and every absent change is
 // reached from src's heads through absent changes only. The order is the walk's; it runs on the host over the absent
 // changes' dependency indexes, for the reason syncChangesToSend gives (a device walk needs one launch per level).
-inline void Engine::changesAddedFrom(Engine& src, std::vector<u32>& order) {
+// With several sources, a change absent here that an earlier source also holds is dropped from the later one. What is
+// left of a source is still closed under its descendants within that source (a descendant of a change this document or
+// an earlier source lacks is lacked there too), so the same walk over it gives getChangesAdded of this document after the
+// earlier sources were merged.
+inline void Engine::changesAddedFrom(Engine* const* srcs, size_t n, std::vector<MergePick>& order) {
   order.clear();
-  computeHashGraph();   // new.js:1980; the package builds both documents' graphs (DESIGN.md section 5)
-  src.computeHashGraph();
-  if (src.ctx.device != ctx.device)
-    throw Error(AMG_ERR_UNSUPPORTED, "amgpu: the documents are on different devices (" + std::to_string(src.ctx.device) + ", " + std::to_string(ctx.device) + ")");
-  sync(src.ctx);   // src's buffers are read on this engine's stream
-  const size_t C = src.numApplied;
-  if (C == 0) return;
+  for (size_t s = 0; s < n; s++)
+    if (srcs[s]->ctx.device != ctx.device)
+      throw Error(AMG_ERR_UNSUPPORTED, "amgpu: the documents are on different devices (" + std::to_string(srcs[s]->ctx.device) + ", " + std::to_string(ctx.device) + ")");
+  computeHashGraph();   // new.js:1980; the package builds every document's graph (DESIGN.md section 5)
+  std::vector<size_t> base(n + 1, 0);   // source s's changes are [base[s], base[s + 1]) of the concatenated probe
+  for (size_t s = 0; s < n; s++) {
+    srcs[s]->computeHashGraph();
+    sync(srcs[s]->ctx);   // the source's buffers are read on this engine's stream
+    base[s + 1] = base[s] + srcs[s]->numApplied;
+  }
+  const size_t T = base[n];
+  if (T == 0) return;
   clearErr();
-  // 1. presence: this document's hashes in a table, one probe per change of src, then flag -> scan -> compact
+  // 1. presence: this document's hashes in a table, one probe per change of every source, then flag -> scan -> compact.
+  //    The compact runs per source and writes the source's own change index, so the list is in (source, index) order.
   const u64 ownMask = hashTableOf(hashes.p, numApplied);
-  mergeAbsent.ensure(ctx, C + 1); mergeSlot.ensure(ctx, C + 2);
-  foreach(ctx, C, MergeProbeKernel{hashes.p, hashTable.p, ownMask, src.hashes.p, mergeAbsent.p});
-  scan_exclusive(ctx, scanTmp, mergeAbsent.p, mergeSlot.p, C);
-  const size_t K = readU32(mergeSlot.p + C);
+  mergeAbsent.ensure(ctx, T + 1); mergeSlot.ensure(ctx, T + 2);
+  for (size_t s = 0; s < n; s++)
+    foreach(ctx, base[s + 1] - base[s], MergeProbeKernel{hashes.p, hashTable.p, ownMask, srcs[s]->hashes.p, mergeAbsent.p + base[s]});
+  scan_exclusive(ctx, scanTmp, mergeAbsent.p, mergeSlot.p, T);
+  std::vector<u32> first(n + 1, 0);   // source s's candidates are [first[s], first[s + 1]) of the list
+  for (size_t s = 1; s <= n; s++) d2h(ctx, &first[s], mergeSlot.p + base[s], 4);
+  sync(ctx);
+  const size_t K = first[n];
   if (K == 0) return;
   mergeList.ensure(ctx, K + 1);
-  foreach(ctx, C, CompactKernel{mergeAbsent.p, mergeSlot.p, mergeList.p});
-  std::vector<u32> absent(K); d2h(ctx, absent.data(), mergeList.p, K * 4); sync(ctx);
-  // 2. the absent changes' dependencies in header order (the order of dependenciesByHash) and src's heads, as change
-  //    indexes of src: their headers in src's arena, resolved against src's hashes (parseChangeHeaders, resolveChangeDeps)
-  std::vector<HostChange> pairs(K); for (size_t k = 0; k < K; k++) pairs[k] = src.changes[absent[k]];
-  const u32 D = parseChangeHeaders(src.arena.p, pairs.data(), K);
-  checkErr();
-  const u64 srcMask = resolveChangeDeps(src.arena.p, src.hashes.p, C, K, 0, D);
-  const size_t H = src.st.heads.size();
-  mergeHeads.ensure(ctx, H * 32 + 32); mergeHeadIdx.ensure(ctx, H + 1);
-  std::vector<u8> headBytes(H * 32); for (size_t i = 0; i < H; i++) memcpy(headBytes.data() + 32 * i, src.st.heads[i].data(), 32);
-  h2d(ctx, mergeHeads.p, headBytes.data(), H * 32);
-  foreach(ctx, H, HashLookupKernel{src.hashes.p, hashTable.p, srcMask, mergeHeads.p, mergeHeadIdx.p});
-  std::vector<u32> base(K + 1), deps(D), stack(H);
-  d2h(ctx, base.data(), depBase.p, (K + 1) * 4); d2h(ctx, deps.data(), depIdx.p, (size_t)D * 4); d2h(ctx, stack.data(), mergeHeadIdx.p, H * 4); sync(ctx);
-  // 3. new.js:1983-1994: heads in order, popped from the back; the seen test at pop time; dependencies pushed in header
-  //    order; a change this document has stops the walk. Then reversed (:1996).
-  std::vector<u32> posOf(C, EMPTY32); for (size_t k = 0; k < K; k++) posOf[absent[k]] = (u32)k;
-  std::vector<u8> seen(K, 0);
-  while (!stack.empty()) {
-    const u32 c = stack.back(); stack.pop_back();
-    const u32 k = c < C ? posOf[c] : EMPTY32;
-    if (k == EMPTY32 || seen[k]) continue;
-    seen[k] = 1; order.push_back(c);
-    stack.insert(stack.end(), deps.begin() + base[k], deps.begin() + base[k + 1]);
+  size_t holders = 0;   // sources with candidates
+  for (size_t s = 0; s < n; s++) {
+    if (first[s + 1] == first[s]) continue;
+    holders++;
+    foreach(ctx, base[s + 1] - base[s], CompactKernel{mergeAbsent.p + base[s], mergeSlot.p + base[s], mergeList.p});
   }
-  std::reverse(order.begin(), order.end());
+  std::vector<u32> absent(K); d2h(ctx, absent.data(), mergeList.p, K * 4);
+  // 2. across sources: the candidates' hashes in list order, a table over them (equal hashes keep the smallest position),
+  //    and a candidate kept only when its own hash leads back to its position. The earliest source wins, whatever the
+  //    scheduling of the inserts.
+  std::vector<u32> firstPos;
+  if (holders > 1) {
+    mergeCand.ensure(ctx, K * 32 + 32); mergeFirst.ensure(ctx, K + 1);
+    for (size_t s = 0; s < n; s++)
+      foreach(ctx, first[s + 1] - first[s], SyncHashGatherKernel{srcs[s]->hashes.p, mergeList.p + first[s], mergeCand.p + (size_t)first[s] * 32});
+    const u64 candMask = hashTableOf(mergeCand.p, K);
+    foreach(ctx, K, HashLookupKernel{mergeCand.p, hashTable.p, candMask, mergeCand.p, mergeFirst.p});
+    firstPos.resize(K); d2h(ctx, firstPos.data(), mergeFirst.p, K * 4);
+  }
+  sync(ctx);
+  // 3. per source, over its surviving candidates: their dependencies in header order (the order of dependenciesByHash)
+  //    and the source's heads, as change indexes of the source: their headers in its arena, resolved against its hashes
+  //    (parseChangeHeaders, resolveChangeDeps)
+  for (size_t s = 0; s < n; s++) {
+    Engine& src = *srcs[s]; const size_t C = src.numApplied;
+    std::vector<u32> kept;
+    for (size_t k = first[s]; k < first[s + 1]; k++) if (firstPos.empty() || firstPos[k] == (u32)k) kept.push_back(absent[k]);
+    const size_t Ks = kept.size();
+    if (Ks == 0) continue;
+    std::vector<HostChange> pairs(Ks); for (size_t k = 0; k < Ks; k++) pairs[k] = src.changes[kept[k]];
+    const u32 D = parseChangeHeaders(src.arena.p, pairs.data(), Ks);
+    checkErr();
+    const u64 srcMask = resolveChangeDeps(src.arena.p, src.hashes.p, C, Ks, 0, D);
+    const size_t H = src.st.heads.size();
+    mergeHeads.ensure(ctx, H * 32 + 32); mergeHeadIdx.ensure(ctx, H + 1);
+    std::vector<u8> headBytes(H * 32); for (size_t i = 0; i < H; i++) memcpy(headBytes.data() + 32 * i, src.st.heads[i].data(), 32);
+    h2d(ctx, mergeHeads.p, headBytes.data(), H * 32);
+    foreach(ctx, H, HashLookupKernel{src.hashes.p, hashTable.p, srcMask, mergeHeads.p, mergeHeadIdx.p});
+    std::vector<u32> depStart(Ks + 1), deps(D), stack(H);
+    d2h(ctx, depStart.data(), depBase.p, (Ks + 1) * 4); d2h(ctx, deps.data(), depIdx.p, (size_t)D * 4); d2h(ctx, stack.data(), mergeHeadIdx.p, H * 4); sync(ctx);
+    // 4. new.js:1983-1994: heads in order, popped from the back; the seen test at pop time; dependencies pushed in header
+    //    order; a change outside the kept ones (this document or an earlier source has it) stops the walk. Then reversed
+    //    (:1996).
+    std::vector<u32> posOf(C, EMPTY32); for (size_t k = 0; k < Ks; k++) posOf[kept[k]] = (u32)k;
+    std::vector<u8> seen(Ks, 0);
+    const size_t from = order.size();
+    while (!stack.empty()) {
+      const u32 c = stack.back(); stack.pop_back();
+      const u32 k = c < C ? posOf[c] : EMPTY32;
+      if (k == EMPTY32 || seen[k]) continue;
+      seen[k] = 1; order.push_back(MergePick{(u32)s, c});
+      stack.insert(stack.end(), deps.begin() + depStart[k], deps.begin() + depStart[k + 1]);
+    }
+    std::reverse(order.begin() + from, order.end());
+  }
 }
 
 // The changes to send are the bytes getChangesAdded returns (amg_backend::changeBytes): a change's DEFLATEd original when
-// it has one, else its plain bytes. A change getChangesAdded would DEFLATE on the way out (exportsDeflated) goes over
-// plain and marked instead, so that this document hands it out DEFLATEd later, as if it had received it that way.
-inline void Engine::mergeFrom(Engine& src, bool wantPatch, PatchOut& out) {
+// it has one, else its plain bytes. A change getChangesAdded would DEFLATE on the way out (exportsDeflated of the source
+// that sends it) goes over plain and marked instead, so that this document hands it out DEFLATEd later, as if it had
+// received it that way.
+inline void Engine::mergeFrom(Engine* const* srcs, size_t n, bool wantPatch, PatchOut& out) {
   spans.start(SPAN_MERGE);
-  std::vector<u32> idx; changesAddedFrom(src, idx);
-  const size_t K = idx.size();
+  std::vector<MergePick> picks; changesAddedFrom(srcs, n, picks);
+  const size_t K = picks.size();
   std::vector<u64> offs(K + 1, 0); std::vector<MergeRange> ranges(K); std::vector<u8> marks(K + 1, 0);
   for (size_t k = 0; k < K; k++) {
-    const u32 c = idx[k]; const HostChange* o = src.originalOf(c); const HostChange r = o ? *o : src.changes[c];
+    const Engine& src = *srcs[picks[k].src]; const u32 c = picks[k].idx;
+    const HostChange* o = src.originalOf(c); const HostChange r = o ? *o : src.changes[c];
     marks[k] = src.exportsDeflated(c) ? 1 : 0;
-    ranges[k] = MergeRange{offs[k], r.off, r.len}; offs[k + 1] = offs[k] + r.len;
+    ranges[k] = MergeRange{offs[k], src.arena.p + r.off, r.len}; offs[k + 1] = offs[k] + r.len;
   }
   if ((u64)arenaLen + offs[K] + 64 >= 0xfff00000ULL) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: change arena limited to 4 GiB per document");
   mergeBlob.ensure(ctx, offs[K] + 64); mergeRanges.ensure(ctx, K + 1);
   h2d(ctx, mergeRanges.p, ranges.data(), K * sizeof(MergeRange));
-  merge_gather(ctx, K, MergeGatherKernel{src.arena.p, mergeBlob.p, mergeRanges.p});
+  merge_gather(ctx, K, MergeGatherKernel{mergeBlob.p, mergeRanges.p});
   applyChanges(nullptr, nullptr, K, mergeBlob.p, offs.data(), false, wantPatch, out, marks.data());   // the device-blob path of amg_apply_changes_packed
   spans.stop();
 }

@@ -1,16 +1,20 @@
-// amgpu — kernels #12: merge, the changes one document lacks, found by hash lookup and copied device to device.
+// amgpu — kernels #12: merge, the changes one document lacks from one or more others, found by hash lookup and copied
+// device to device.
 //
 // Replaces (reference paths relative to /root/reference):
 //   backend/new.js:1979-1997  getChangesAdded: which changes of `this` the other document does not have (its
 //                             changeIndexByHash lookup, one per change here instead of one per visited hash)
 //   src/automerge.js:61-67    merge = applyChanges(local, getChangesAdded(local, remote)): the changes' bytes, gathered
-//                             from the remote document's arena into one blob the local document applies
+//                             from the remote documents' arenas into one blob the local document applies. Several remotes
+//                             share one call: a change two of them hold goes over once, from the first (HashLookupKernel
+//                             over a table of the candidates' own hashes, built by HashInsertKernel, which keeps the
+//                             smallest position of equal hashes).
 #pragma once
 #include "gate.cuh"
 
 namespace amg {
 
-// absent[i] = 1 when change i of the source document is not among the target's applied changes (table: the target's hashes)
+// absent[i] = 1 when change i of a source document is not among the target's applied changes (table: the target's hashes)
 struct MergeProbeKernel {
   const u8* dstHashes; const u32* table; u64 mask; const u8* srcHashes; u32* absent;
   HD void operator()(size_t i) const { absent[i] = hash_lookup(dstHashes, table, mask, srcHashes + i * 32) == DEP_MISSING ? 1u : 0u; }
@@ -22,17 +26,17 @@ struct HashLookupKernel {
   HD void operator()(size_t i) const { idx[i] = hash_lookup(hashes, table, mask, queries + i * 32); }
 };
 
-// One change to copy: src[srcOff, srcOff + len) -> dst[dstOff, dstOff + len). dstOff is 64-bit: the blob may pass 4 GiB
-// before the target's arena limit is checked.
-struct MergeRange { u64 dstOff; u32 srcOff, len; };
+// One change to copy: src[0, len) -> dst[dstOff, dstOff + len), src pointing into the arena of the document that holds the
+// change (a merge reads several). dstOff is 64-bit: the blob may pass 4 GiB before the target's arena limit is checked.
+struct MergeRange { u64 dstOff; const u8* src; u32 len; };
 
 // One warp per change. When source and destination agree modulo 16, the aligned middle goes as 16-byte words (the
 // prefix and the tail byte by byte); otherwise every byte is its own load, still coalesced across the warp.
 struct MergeGatherKernel {
-  const u8* src; u8* dst; const MergeRange* r;
+  u8* dst; const MergeRange* r;
   struct alignas(16) V16 { u64 a, b; };
   HD void copy(size_t k, u32 lane, u32 lanes) const {
-    const MergeRange m = r[k]; const u8* s = src + m.srcOff; u8* d = dst + m.dstOff; const u64 n = m.len;
+    const MergeRange m = r[k]; const u8* s = m.src; u8* d = dst + m.dstOff; const u64 n = m.len;
     u64 head = n;
     if ((((size_t)s ^ (size_t)d) & 15) == 0) { head = (16 - ((size_t)d & 15)) & 15; if (head > n) head = n; }
     for (u64 i = lane; i < head; i += lanes) d[i] = s[i];

@@ -90,6 +90,8 @@ class Library:
         L.amg_get_history_patches.argtypes = [vp, vp, C.c_size_t, vp, vp]
         L.amg_merge.restype = C.c_int
         L.amg_merge.argtypes = [vp, vp, C.c_int, vp, vp]
+        L.amg_merge_many.restype = C.c_int
+        L.amg_merge_many.argtypes = [vp, vp, C.c_size_t, C.c_int, vp, vp]
         L.amg_apply_local_change.restype = C.c_int
         L.amg_apply_local_change.argtypes = [vp, vp, C.c_size_t, C.c_int, vp, vp, vp]
         L.amg_clock_of.argtypes = [vp, vp, C.c_size_t, vp, vp]
@@ -637,8 +639,23 @@ class GpuBackendDoc:
         fp = self.merge_flat(other, want_patch)
         return fp.to_patch(False) if want_patch else None
 
+    def merge_many_flat(self, others, want_patch=True):
+        """amg_merge_many: merge_flat folded over `others` in one apply. Applies the changes of each document this one and
+        the earlier ones lack, each remote's in getChangesAdded order; a change several remotes hold goes over once, from
+        the first. Returns the FlatPatch applyChanges would return for that list (None with want_patch=False). Raises
+        Unsupported when a document is on another device, before anything changed."""
+        hs = (C.c_void_p * max(len(others), 1))(*[o.h for o in others])
+        pp, err = C.c_void_p(), _ErrStruct()
+        self._lib.check(self._lib.L.amg_merge_many(self.h, hs, C.c_size_t(len(others)), int(want_patch), C.byref(pp), C.byref(err)), err)
+        return self._take_patch(pp) if want_patch else None
+
+    def merge_many(self, others, want_patch=True):
+        """merge_many_flat as the patch dict applyChanges returns."""
+        fp = self.merge_many_flat(others, want_patch)
+        return fp.to_patch(False) if want_patch else None
+
     def last_merge_ms(self):
-        """Device span of the last merge_flat call (CUDA events), ms."""
+        """Device span of the last merge_flat or merge_many_flat call (CUDA events), ms."""
         return float(self._lib.L.amg_last_merge_ms(self.h))
 
     # ---- applyLocalChange (backend.js:54-91), on the device

@@ -90,7 +90,25 @@ int amg_get_changes_added(amg_backend* b_new, amg_backend* b_old, amg_buffers** 
  *   - An apply error (e.g. both documents hold a different change for the same actor and seq) is the error applyChanges
  *     reports for the same changes, and dst is unchanged. */
 int amg_merge(amg_backend* dst, amg_backend* src, int want_patch, amg_patch** out, amg_error* err);
-/* device span of the last amg_merge call in ms, lookups, copy and apply (CUDA events on dst's main stream, like amg_last_history_ms) */
+/* Automerge.merge folded over n remotes in one call: srcs.reduce(merge, dst) with one apply instead of n. dst applies one
+ * list L = walk_1 ++ ... ++ walk_n through the device-memory path of amg_apply_changes_packed, and *out is the patch that
+ * applyChanges(dst, L) returns. amg_merge(dst, src) is amg_merge_many(dst, &src, 1).
+ *   - walk_i: the changes of srcs[i] whose hash is neither among dst's applied changes nor among those of an earlier
+ *     srcs[j] (j < i), in getChangesAdded's order: what getChangesAdded(dst', srcs[i]) returns, dst' being dst after
+ *     merging srcs[0 .. i-1]. A change several remotes hold goes over once, from the first of them.
+ *   - The document that results equals n amg_merge calls in order (heads, clock, maxOp, getPatch, save, getChanges). The
+ *     one exception: a queued change of dst that becomes applicable part-way through that fold is not re-sent by it, but
+ *     L may hold it; the apply drops the copy, and only the patch of applyChanges(dst, L) is promised then.
+ *   - A remote that is dst, a clone of dst, repeated in srcs, or whose changes dst and earlier remotes already hold adds
+ *     nothing. n == 0 or nothing to send: dst applies an empty batch, as amg_merge does.
+ *   - The remotes are not changed; their queued changes are never sent; loaded documents have their history rebuilt
+ *     first. The DEFLATE mark of amg_merge applies per remote.
+ *   - A remote on another CUDA device, or a total of changes that would take dst's change arena past its 4 GiB limit:
+ *     AMG_UNSUPPORTED, nothing changed. An apply error (e.g. two remotes holding different changes for the same actor
+ *     and seq) is the error applyChanges(dst, L) reports, and dst is unchanged. */
+int amg_merge_many(amg_backend* dst, amg_backend* const* srcs, size_t n, int want_patch, amg_patch** out, amg_error* err);
+/* device span of the last amg_merge or amg_merge_many call in ms, lookups, copy and apply (CUDA events on dst's main
+ * stream, like amg_last_history_ms) */
 float amg_last_merge_ms(amg_backend* dst);
 /* Backend.getChangeByHash — backend.js:176-178 -> new.js:1999-2002; zero buffers when unknown */
 int amg_get_change_by_hash(amg_backend* b, const uint8_t hash[32], amg_buffers** out, amg_error* err);

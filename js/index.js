@@ -7,7 +7,7 @@
 'use strict'
 
 const native = require('../addon/build/Release/amgpu_napi')
-const { encodeChange } = require('automerge/backend/columnar')   // stays JS, exactly as in backend.js:83
+const { encodeChange, decodeChangeMeta } = require('automerge/backend/columnar')   // stays JS, exactly as in backend.js:83
 const { inflatePatch } = require('./inflate_patch')
 
 const OUTDATED = 'Attempting to use an outdated Automerge document that has already been updated. ' +
@@ -85,23 +85,40 @@ function historyPatches(backend, prefixLengths) {
   return native.historyPatches(backendState(backend), prefixLengths).map(flat => inflatePatch(flat, true))
 }
 
-// Automerge.merge (src/automerge.js:61-67) at the backend level: applyChanges(backend1, getChangesAdded(backend1, backend2)),
-// with the changes copied from backend2's device memory to backend1's. backend1 is frozen, as applyChanges freezes it.
-// Documents on different devices take the same route through JavaScript.
-function merge(backend1, backend2) {
-  const state = backendState(backend1), other = backendState(backend2)
+// The changes merging `backends` into backend1 applies: getChangesAdded(backend1, b) for each in turn, without the changes
+// an earlier one already contributes (compared by hash)
+function changesAddedMany(backend1, backends) {
+  if (backends.length === 1) return getChangesAdded(backend1, backends[0])
+  const sent = new Set(), out = []
+  for (const b of backends) {
+    for (const change of getChangesAdded(backend1, b)) {
+      const hash = decodeChangeMeta(change, true).hash
+      if (!sent.has(hash)) { sent.add(hash); out.push(change) }
+    }
+  }
+  return out
+}
+
+// Automerge.merge (src/automerge.js:61-67) at the backend level, folded over an array of backends in one apply:
+// applyChanges(backend1, changesAddedMany(backend1, backends)), with the changes copied from the backends' device memory
+// to backend1's. The document equals merging them one by one (a queued change of backend1 that becomes applicable part-way
+// may be sent once more and is dropped by the apply). backend1 is frozen, as applyChanges freezes it. Documents on
+// different devices take the same route through JavaScript.
+function mergeMany(backend1, backends) {
+  const state = backendState(backend1), others = backends.map(backendState)
   let flat
-  try { flat = native.merge(state, other) } catch (e) {
+  try { flat = native.mergeMany(state, others) } catch (e) {
     if (e.code !== 'AMG_UNSUPPORTED') throw e
-    return applyChanges(backend1, getChangesAdded(backend1, backend2))
+    return applyChanges(backend1, changesAddedMany(backend1, backends))
   }
   const patch = inflatePatch(flat, false)
   backend1.frozen = true
   return [{state, heads: patch.deps}, patch]
 }
+function merge(backend1, backend2) { return mergeMany(backend1, [backend2]) }
 
 const backendApi = { init, clone, free, applyChanges, applyLocalChange, save, load, loadChanges, getPatch,
-  getHeads, getAllChanges, getChanges, getChangesAdded, getChangeByHash, getMissingDeps, historyPatches, merge }
+  getHeads, getAllChanges, getChanges, getChangesAdded, getChangeByHash, getMissingDeps, historyPatches, merge, mergeMany }
 
 // backend/sync.js:19 hard-imports './backend': the sync functions of backend/index.js are re-created over this backend by
 // loading the reference's sync.js with its backend import redirected (it only calls getHeads / getChanges /
