@@ -466,6 +466,31 @@ def _cuts(lo, hi, sizes):
     return out
 
 
+def compare_calls(Doc, oracle_mod, name, W, cuts, reload=False):
+    """The calls W.log[lo:hi] of `cuts` in order on one engine and one oracle: after each the patch (or error), maxOp,
+    clock, deps, pendingChanges, heads and getMissingDeps; at the end getPatch, save() and the op table, and with `reload`
+    getPatch after load(save()). A known difference of the reference fails the test."""
+    g, o = Doc(), oracle_mod.OracleDoc()
+    corners = []
+    try:
+        for i, (lo, hi) in enumerate(cuts):
+            _apply_both(g, o, [c for c, _, _, _ in W.log[lo:hi]], corners, (name, i))
+            assert corners == [], (name, i, corners)   # no nested objects: the children-snapshot allowance never applies
+            _state_equal(g, o, (name, i))
+        assert not o.get_missing_deps() and not g.get_missing_deps(), name
+        pg, po = g.get_patch(), o.get_patch()
+        if (replay.deep_equal(replay.decode(pg), replay.decode(po)) is not None or g.save() != o.save()) and _misplaced(o):
+            raise KnownDifference('block misplacement')
+        _same(pg, po, (name, 'getPatch'))
+        saved = g.save()
+        assert saved == o.save(), name
+        parity_checks._dump_equal(g, o)
+        if reload:
+            _same(Doc(saved).get_patch(), oracle_mod.OracleDoc(saved).get_patch(), (name, 'getPatch after load'))
+    except KnownDifference as e:
+        pytest.fail('%s meets a known difference of the reference (DESIGN.md section 5: %s): choose another seed' % (name, e))
+
+
 def run_scenario(Doc, oracle_mod, name, made, multi=False):
     """The base history in one call, then the scenario's call (or its changes in calls of 1, 7 and 1 000 changes), each
     against the oracle; at the end getPatch, save() and the op table. A known difference of the reference fails the test."""
@@ -475,22 +500,7 @@ def run_scenario(Doc, oracle_mod, name, made, multi=False):
     shapes = count_shape(W.log, base_end, calls)
     if not multi:
         check_claims(shapes, claims, name)
-    g, o = Doc(), oracle_mod.OracleDoc()
-    corners = []
-    try:
-        for i, (lo, hi) in enumerate(([(0, base_end)] if base_end else []) + calls):
-            _apply_both(g, o, [c for c, _, _, _ in W.log[lo:hi]], corners, (name, i))
-            assert corners == [], (name, i, corners)   # no nested objects: the children-snapshot allowance never applies
-            _state_equal(g, o, (name, i))
-        assert not o.get_missing_deps() and not g.get_missing_deps(), name
-        pg, po = g.get_patch(), o.get_patch()
-        if (replay.deep_equal(replay.decode(pg), replay.decode(po)) is not None or g.save() != o.save()) and _misplaced(o):
-            raise KnownDifference('block misplacement')
-        _same(pg, po, (name, 'getPatch'))
-        assert g.save() == o.save(), name
-        parity_checks._dump_equal(g, o)
-    except KnownDifference as e:
-        pytest.fail('%s meets a known difference of the reference (DESIGN.md section 5: %s): choose another seed' % (name, e))
+    compare_calls(Doc, oracle_mod, name, W, ([(0, base_end)] if base_end else []) + calls)
     s = shapes[0] if not multi else None
     print('%s: compared, %d calls, %s, %.1f s' % (name, len(calls), 'M %d tbits %d max items %d partitions %d runs %s' % (
         s['M'], s['tbits'], s['max_items'], s['parts'], s['runs']) if s else 'M %s' % [x['M'] for x in shapes][:6], time.time() - t0))
