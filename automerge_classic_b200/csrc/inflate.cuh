@@ -64,7 +64,9 @@ HD bool infl_build(const u8* lengths, int n, uint16_t* count, uint16_t* symbol, 
         uint16_t offs[16]; offs[1] = 0;
         for (int len = 1; len < 15; len++) offs[len + 1] = (uint16_t)(offs[len] + count[len]);
         for (int i = 0; i < n; i++) if (lengths[i]) symbol[offs[lengths[i]]++] = (uint16_t)i;
-        ok = (!mustBeComplete || left == 0 || (n - count[0]) == 1) ? 1 : 0;   // (the fixed distance code of RFC 1951 3.2.6 uses 30 of 32 codes)
+        // an incomplete code is refused unless it is one symbol of one bit, as zlib's inflate_table does for literal/length
+        // and distance codes (the fixed distance code of RFC 1951 3.2.6 uses 30 of 32 codes and is exempt)
+        ok = (!mustBeComplete || left == 0 || (count[1] == 1 && n - count[0] == 1)) ? 1 : 0;
       }
     }
   }
@@ -132,7 +134,7 @@ HD u32 inflate_tabled(InflWarpTables& T, const u8* src, u32 begin, u32 end, u8* 
             if (cnt[0] == 19) { /* no codes: decode fails below */ }
             else {
               int left = 1; for (int l2 = 1; l2 < 16; l2++) { left <<= 1; left -= cnt[l2]; if (left < 0) { e = KE_DEFLATE; break; } }
-              if (!e) { uint16_t offs[16]; offs[1] = 0; for (int l2 = 1; l2 < 15; l2++) offs[l2 + 1] = (uint16_t)(offs[l2] + cnt[l2]); for (int i = 0; i < 19; i++) if (cl[i]) sym[offs[cl[i]]++] = (uint16_t)i; if (!(left == 0 || (19 - cnt[0]) == 1)) e = KE_DEFLATE; }
+              if (!e) { uint16_t offs[16]; offs[1] = 0; for (int l2 = 1; l2 < 15; l2++) offs[l2 + 1] = (uint16_t)(offs[l2] + cnt[l2]); for (int i = 0; i < 19; i++) if (cl[i]) sym[offs[cl[i]]++] = (uint16_t)i; if (left != 0) e = KE_DEFLATE; }   // a code-length code must be complete (zlib)
             }
           }
           int idx = 0;
