@@ -201,25 +201,33 @@ class Engine {
   // ---- scratch (grow-only)
   DBuf<u32> chOff, chLen, nOps, nPreds, nDeps, nActors, colOff, colLen, depBase, depIdx, primary, pass, flagWord, appRank, opBase, predBase, timeBase, amapBase, amap, authorSlot, newSlots;
   DBuf<u8> applied; DBuf<ChangeHot> hot; DBuf<ChangeMeta> meta /* save(): full headers */; DBuf<u64> errWord; DBuf<u32> hashTable;
-  DBuf<u32> inflCap, inflCapOff, inflOvf; DBuf<u8> inflScratch; DBuf<u64> inflTotal;
+  DBuf<u32> inflCap, inflCapOff, inflOvf, inflLen, inflOff, deflList, patchTriples; DBuf<u8> inflScratch; DBuf<u64> inflTotal;
   u64 inflateSpeculate(InflateArgs& ia);   // first inflate pass + inflOff; returns the 64-bit total of the inflated sizes
   DBuf<u32> rawBase, rawPredBase, decErr, decDirect; DBuf<u64> decCursor; size_t lastDeflCount = 0, lastDeflStart = 0;
   u32* decTotalsPtr() { return reinterpret_cast<u32*>(decCursor.p + 2); }
-  DBuf<u32> patchByteLen, patchByteOff; DBuf<u8> patchBytesD;   // key / value bytes shipped inside the patch   // fused decode (decode.cuh k_decode_tiles)
+  // fused decode (decode.cuh k_decode_tiles)
   DBuf<u32> r_objActor, r_objCtr, r_keyActor, r_keyCtr, r_keyStrOff, r_keyStrLen, r_insert, r_action, r_valLen, r_valOff, r_predNum, r_predOff, r_predActor, r_predCtr;
   DBuf<u64> o_id, o_obj, o_key, o_predId; DBuf<u32> o_keyStrOff, o_keyStrLen, o_flags, o_valLen, o_valOff, o_predOff, o_predNum, o_change, o_time;
-  DBuf<u32> isRow, rowSlot, rowOfOp; DocBufs work, sorted;
-  DBuf<u64> idKeys; DBuf<u32> idVals; DBuf<u32> objRow, elemRow, parentRow, keySlot, repList, repCount, listPos, perm, pos;
-  DBuf<KeySlot> keySlots; DBuf<u64> sortKeys; DBuf<u32> sortVals; SortTemp sortTmp; ScanTemp scanTmp;
+  DBuf<u64> sortKeys; DBuf<u32> sortVals; SortTemp sortTmp; ScanTemp scanTmp; DBuf<u32> emit, slot;   // shared by the phases (emit, slot: a flag array and its scan; linkEdits names slot linkBase)
   ParColumnDecoder parCols{ctx, scanTmp}; size_t parDocMinRows = 4096;   // documents with at least this many rows decode their columns in parallel (doccols.cuh); AMG_PAR_DOC_MIN overrides
-  DBuf<u32> eNext, eRank, insItems, itemIdx, objSlot; DBuf<u64> ePacked, ePacked2;
-  DBuf<u64> pairKey, pairSucc, newSucc; DBuf<u32> pairIdx, pairPos, pairTime, succCnt, newSuccCnt, newSuccOff, firstNewSucc;
-  DBuf<u32> elemPos, keyRankAt, objPos, head, headScan, groupOf, groupRows, groupVisible, groupFirst, groupTouched, groupLinked, objTouchedAt, linkDone, emit, marker, slot;
-  DBuf<u32> isObjHead, objIdx, objStart, elemVis, elemVisScan, rowEmit, firstVis, state, nItems, itemBase, qIndex, zero, wzero, zscan, wscan, editObjKey;
-  DBuf<DomItem> items, items2; DBuf<PropRec> propOut; DBuf<EditRec> editOut, editOut2; DBuf<u64> editElem, editElem2;
-  std::unique_ptr<ColumnEncoder> encoder; DBuf<long long> saveVals; DBuf<u32> saveStrOff, saveStrLen; DBuf<u64> counterTotal; DBuf<int> domW, domW2; DBuf<u32> elemMinT, editRowPos, editRowPos2, editObjKey2, rowClass, firstBare, counterOwner, newSuccTime, counterLast, runHeadFlag, runScan, runStart, elemFollower, domTw, domTw2, oldVisScan, inflLen, inflOff, groupHasChild, gCount, gElem, gT1, gQOrd, gBase, nQ, elemHasRecs, listLinkTime, editElemPos, editElemPos2, editKind, editPred, editDead, editMerge, editMulti, editLive;
-  DBuf<u32> seqSlot, actorCnt, actorBaseD, clockD, changeActor, editTime; DBuf<u8> hashTmp; DBuf<u32> headsPack, headsOut;
-  DBuf<u32> finalTime, gFailed, memberFinal, opAt, runHead, opGroupHead; DBuf<u64> gBound; DBuf<HostChange> chPairs; DBuf<u32> largeFlag, largeSlot, largeList; size_t lastNumLarge = 0; DBuf<u64> zwScan; DBuf<u32> deflList, patchTriples;
+  std::unique_ptr<ColumnEncoder> encoder; DBuf<long long> saveVals; DBuf<u32> saveStrOff, saveStrLen;
+  DBuf<HostChange> chPairs; DBuf<u32> seqSlot, actorCnt, actorBaseD, changeActor, largeFlag, largeSlot, largeList, headsPack, headsOut; DBuf<u8> hashTmp; size_t lastNumLarge = 0;
+  // op set and patch: one line per step that sizes them, and who else borrows them (under which name)
+  DBuf<u32> isRow, rowSlot, rowOfOp, objRow, elemRow, parentRow; DBuf<u64> idKeys; DBuf<u32> idVals;   // appendRows
+  DBuf<KeySlot> keySlots; DBuf<u32> keySlot, repList, repCount;   // rankMapKeys
+  DBuf<u32> listPos, insItems, itemIdx, objSlot, eNext, eRank; DBuf<u64> ePacked, ePacked2;   // rankLists
+  DBuf<u32> perm, pos;   // sortDocOrder
+  DBuf<u64> pairKey, pairSucc, newSucc; DBuf<u32> pairIdx, pairPos, pairTime, succCnt, newSuccCnt, newSuccOff, firstNewSucc, newSuccTime; DocBufs sorted;   // linkSuccessors; pairKey: checkSequence (clockDev), linkEdits (k2); pairIdx: linkEdits (v2); pairSucc: finalizeOps, finalizeRows (maxOpD), parseChangeMeta (sumD)
+  DBuf<u32> objPos;   // batchPatch
+  DBuf<u32> head, headScan, groupOf, isObjHead, objIdx, groupRows, groupVisible, groupFirst, groupTouched, groupHasChild, objStart, marker, groupLinked;   // patchGroups; objStart: computeHeads; groupLinked: computeHeads (isDep)
+  DBuf<u32> nQ, elemHasRecs, listLinkTime, elemMinT, opAt, runHead, opGroupHead, gCount, gElem, gT1, gQOrd, gBase, qIndex, runHeadFlag, runScan, runStart, elemFollower;   // batchOpGroups; elemHasRecs: batchListEdits (elemHasLive)
+  DBuf<u32> objTouchedAt, linkDone;   // markTouched
+  DBuf<u32> finalTime, gFailed, memberFinal, counterLast, counterOwner; DBuf<u64> gBound, counterTotal; DBuf<PropRec> propOut;   // mapProps
+  DBuf<u32> elemVis, elemVisScan, rowEmit, firstVis, rowClass, firstBare;   // docListEdits; elemVis: mapProps (groupEmitted), linkEdits; rowEmit: linkEdits (linkCount)
+  DBuf<u32> nItems, itemBase, oldVisScan, domTw, domTw2; DBuf<int> domW, domW2; DBuf<DomItem> items, items2; DBuf<u64> zwScan;   // listIndex, dominanceCount; domTw2, nItems, itemBase: the device's dominanceCount (partFlag, partScan, partHead)
+  DBuf<EditRec> editOut, editOut2; DBuf<u64> editElem, editElem2; DBuf<u32> editObjKey, editObjKey2, editElemPos, editElemPos2, editRowPos, editRowPos2, editKind, editPred, editDead, editMerge, editMulti, editLive;   // groupEdits; editPred: groupEdits (liveSlot)
+  DBuf<u32> editTime;   // linkEdits
+  DBuf<u32> patchByteLen, patchByteOff; DBuf<u8> patchBytesD;   // shipPatch: key / value bytes shipped inside the patch
 
   explicit Engine(int device) {
     ctx.device = device;
@@ -382,7 +390,7 @@ class Engine {
     size_t G = 0, numNew = 0; bool inOrder = true; u32 D = 0;   // gate: G = applied before + batch; D dependency entries
     std::vector<u8> appliedH; std::vector<u32> primaryH, appRankH; std::vector<HostChange> newQueue, newQueueOriginal;   // host copies: only when an entry waits or the order differs
     DocState now;   // the document's host state as this call leaves it
-    size_t M = 0, P = 0, N = 0, numPairs = 0; OpRows ops{}; IdTable idt{nullptr, nullptr, 0}; Ord ord{}; DocRows w{};   // w: rows before the sort
+    size_t M = 0, P = 0, N = 0, numPairs = 0; int ordBits = 0; OpRows ops{}; IdTable idt{nullptr, nullptr, 0}; Ord ord{}; DocRows w{};   // w: rows before the sort
     std::vector<std::pair<u64, UnknownRow>> unknownRows; std::set<u32> unknownIds;
     std::thread fill;   // fills the host's list of the batch entries; needBatch() joins it before the list is first read
     void needBatch() { if (fill.joinable()) fill.join(); }
@@ -393,6 +401,7 @@ class Engine {
   void applyChangesOnce(ApplyCall& a, PatchOut& out);   // the phases, in order:
   void stageBatch(ApplyCall& a), inflateBatch(ApplyCall& a), runGate(ApplyCall& a), internActors(ApplyCall& a), checkSequence(ApplyCall& a), finalizeOps(ApplyCall& a),
        orderOpSet(ApplyCall& a), computeHeads(ApplyCall& a), commit(ApplyCall& a);
+  void appendRows(ApplyCall& a), rankMapKeys(ApplyCall& a), rankLists(ApplyCall& a), rankEulerTour(size_t S), sortDocOrder(ApplyCall& a), linkSuccessors(ApplyCall& a);   // orderOpSet's steps
   void queueCopy(ApplyCall& a, ApplyCall::Piece& pc, size_t byte0, size_t ch0); void fillPairs(ApplyCall& a);
   // error messages of the rare paths
   [[noreturn]] void throwActorError(u64 ew, const std::vector<std::string>& actors); [[noreturn]] void throwSequenceError(ApplyCall& a);
@@ -404,6 +413,17 @@ class Engine {
     const u32 *newSuccCnt = nullptr, *firstNewSucc = nullptr, *newSuccTime = nullptr, *objPos = nullptr, *pass = nullptr; DocRows unsorted{};   // rows before the sort
   };
   void buildPatch(const PatchInputs& in, PatchOut& out);
+  void batchPatch(ApplyCall& a, PatchOut& out);   // applyChanges' PatchInputs
+  // What buildPatch's steps hand to each other. The device scratch stays in the engine: the copy-out reads propOut, editOut,
+  // editElem and patchBytesD on the side stream until the caller joins it.
+  struct PatchCall {
+    const PatchInputs& in; const DocRows d = in.d; const size_t N = in.N, numOps = in.numOps;
+    size_t numGroups = 0, numObjs = 0, numGroupRecs = 0, numLive = 0, numLink = 0, numProps = 0, numEdits = 0; bool shipElem = true, anyListLink = false; ListCtx lctx{}; MapGroupCtx mg{};
+  };
+  void patchGroups(PatchCall& p), batchOpGroups(PatchCall& p), markTouched(PatchCall& p), mapProps(PatchCall& p), docListEdits(PatchCall& p), batchListEdits(PatchCall& p),
+       listIndex(PatchCall& p), dominanceCount(size_t T, int tbits), groupEdits(PatchCall& p, u32* elemHasLive), linkEdits(PatchCall& p, const u32* elemHasLive),
+       shipPatch(PatchCall& p, PatchOut& out), ensureEdits(const PatchCall& p, size_t n);   // buildPatch's steps, in order, and a helper
+  ListGroupKernel listGroups(const PatchCall& p, int pass);
   void fillPatchHeader(PatchOut& out);
   void finishPatch(PatchOut& out);
   void reset();

@@ -110,12 +110,7 @@ inline void Engine::applyChangesOnce(ApplyCall& a, PatchOut& out) {
   if (a.numNew > 0) {
     internActors(a); checkSequence(a); finalizeOps(a); trace.phase("opset");
     orderOpSet(a);                                      trace.phase("patch");
-    if (a.wantPatch) {   // incremental patch
-      objPos.ensure(ctx, a.N + 1);
-      foreach(ctx, a.N, ObjPosKernel{perm.p, objRow.p, pos.p, objPos.p});
-      buildPatch(PatchInputs{sorted.view(), a.N, false, newSuccOff.p, newSucc.p, succCnt.p, a.ord, &a.ops, a.M, &a.idt, rowOfOp.p, pos.p,
-                             newSuccCnt.p, firstNewSucc.p, newSuccTime.p, objPos.p, pass.p, a.w}, out);
-    }
+    if (a.wantPatch) batchPatch(a, out);
     checkErr();                                         trace.phase("heads+commit");
     computeHeads(a);
   }
@@ -585,29 +580,40 @@ inline void Engine::finalizeOps(ApplyCall& a) {
 
 // ------------------------------------------------------------ 7. op set: the new rows, RGA list order, document order, succ lists
 inline void Engine::orderOpSet(ApplyCall& a) {
-  const size_t M = a.M; const Ord ord = a.ord;
   if (a.now.maxOp >= (1ULL << 40)) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: op counters above 2^40");
-  const int ordBits = bits_for(a.now.maxOp) + ord.rb;
-  isRow.ensure(ctx, M + 1); rowSlot.ensure(ctx, M + 1); rowOfOp.ensure(ctx, M + 1);
-  foreach(ctx, M, RowFlagKernel{o_flags.p, isRow.p}); scan_exclusive(ctx, scanTmp, isRow.p, rowSlot.p, M);
-  const size_t R = readU32(rowSlot.p + M); const size_t N = a.N = numRows + R;
+  a.ordBits = bits_for(a.now.maxOp) + a.ord.rb;
+  appendRows(a);
+  rankMapKeys(a);
+  rankLists(a);
+  sortDocOrder(a);
+  linkSuccessors(a);
+}
+
+// the batch's rows appended behind the document's, every row's id in the id table, and its object, element and parent rows
+inline void Engine::appendRows(ApplyCall& a) {
+  isRow.ensure(ctx, a.M + 1); rowSlot.ensure(ctx, a.M + 1); rowOfOp.ensure(ctx, a.M + 1);
+  foreach(ctx, a.M, RowFlagKernel{o_flags.p, isRow.p}); scan_exclusive(ctx, scanTmp, isRow.p, rowSlot.p, a.M);
+  const size_t R = readU32(rowSlot.p + a.M); const size_t N = a.N = numRows + R;
   if (N >= (1u << 29)) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: more than 2^29 document rows");
   doc.ensure(ctx, N + 1, numRows);
   const DocRows w = a.w = doc.view();
-  foreach(ctx, M, AppendRowsKernel{a.ops, isRow.p, rowSlot.p, numRows, w, rowOfOp.p});
+  foreach(ctx, a.M, AppendRowsKernel{a.ops, isRow.p, rowSlot.p, numRows, w, rowOfOp.p});
   const size_t icap = pow2_at_least(2 * N + 2); idKeys.ensure(ctx, icap); idVals.ensure(ctx, icap); dev_memset(ctx, idKeys.p, 0, icap * 8);
   a.idt = IdTable{idKeys.p, idVals.p, (u64)icap - 1};
   foreach(ctx, N, IdInsertKernel{w.id, a.idt, errWord.p});
   objRow.ensure(ctx, N + 1); elemRow.ensure(ctx, N + 1); parentRow.ensure(ctx, N + 1);
-  foreach(ctx, N, ResolveRowsKernel{w, a.idt, ord, numRows, objRow.p, elemRow.p, parentRow.p, errWord.p});
+  foreach(ctx, N, ResolveRowsKernel{w, a.idt, a.ord, numRows, objRow.p, elemRow.p, parentRow.p, errWord.p});
   checkErr();
   trace.mark("opset:resolved");
-  // map keys: intern, verify, rank distinct keys with an LSD string sort
-  const size_t kcap = pow2_at_least(2 * N + 2); keySlots.ensure(ctx, kcap); keySlot.ensure(ctx, N + 1); repList.ensure(ctx, N + 1); repCount.ensure(ctx, 4);
+}
+
+// map keys: intern, verify, rank distinct keys with an LSD string sort
+inline void Engine::rankMapKeys(ApplyCall& a) {
+  const size_t kcap = pow2_at_least(2 * a.N + 2); keySlots.ensure(ctx, kcap); keySlot.ensure(ctx, a.N + 1); repList.ensure(ctx, a.N + 1); repCount.ensure(ctx, 4);
   foreach(ctx, kcap, KeySlotInitKernel{keySlots.p});
-  foreach(ctx, N, KeyInternKernel{arena.p, w, keySlots.p, (u64)kcap - 1, keySlot.p});
+  foreach(ctx, a.N, KeyInternKernel{arena.p, a.w, keySlots.p, (u64)kcap - 1, keySlot.p});
   dev_memset(ctx, repCount.p, 0, 16);
-  foreach(ctx, N, KeyVerifyKernel{arena.p, w, keySlots.p, keySlot.p, repList.p, repCount.p, errWord.p});
+  foreach(ctx, a.N, KeyVerifyKernel{arena.p, a.w, keySlots.p, keySlot.p, repList.p, repCount.p, errWord.p});
   u32 rc[2]; readU32x2(repCount.p, repCount.p + 1, &rc[0], &rc[1]);
   const size_t D = rc[0]; const u32 maxKeyLen = rc[1];
   trace.mark("opset:keys-interned");
@@ -616,84 +622,94 @@ inline void Engine::orderOpSet(ApplyCall& a) {
     d2d(ctx, sortVals.p, repList.p, D * 4);
     const int chunks = (int)((maxKeyLen + 6) / 7);
     for (int ch = std::max(chunks, 1) - 1; ch >= 0; ch--) {
-      foreach(ctx, D, KeyChunkKernel{arena.p, w, sortVals.p, (u32)ch * 7, sortKeys.p});
+      foreach(ctx, D, KeyChunkKernel{arena.p, a.w, sortVals.p, (u32)ch * 7, sortKeys.p});
       sortPairs(sortKeys, sortVals, D, 64);
     }
     foreach(ctx, D, KeyRankKernel{sortVals.p, keySlot.p, keySlots.p});
   }
-  // RGA order of every list: sibling sort, Euler tour, pointer jumping
-  listPos.ensure(ctx, N + 1); insItems.ensure(ctx, N + 1); emit.ensure(ctx, N + 1); slot.ensure(ctx, N + 2);
-  foreach(ctx, N, InsertFlagKernel{w, emit.p}); scan_exclusive(ctx, scanTmp, emit.p, slot.p, N);
-  const size_t I = readU32(slot.p + N);
+}
+
+// RGA order of every list: sibling sort, Euler tour, list ranking
+inline void Engine::rankLists(ApplyCall& a) {
+  listPos.ensure(ctx, a.N + 1); insItems.ensure(ctx, a.N + 1); emit.ensure(ctx, a.N + 1); slot.ensure(ctx, a.N + 2);
+  foreach(ctx, a.N, InsertFlagKernel{a.w, emit.p}); scan_exclusive(ctx, scanTmp, emit.p, slot.p, a.N);
+  const size_t I = readU32(slot.p + a.N);
   trace.mark("opset:inserts-counted");
   if (I > 0) {
-    const int parentBits = bits_for(N) + 1;
-    if (ordBits + parentBits > 64) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: opId range x document size exceeds the 64-bit sibling sort key");
-    foreach(ctx, N, CompactKernel{emit.p, slot.p, insItems.p});
+    const int parentBits = bits_for(a.N) + 1;
+    if (a.ordBits + parentBits > 64) throw Error(AMG_ERR_UNSUPPORTED, "amgpu: opId range x document size exceeds the 64-bit sibling sort key");
+    foreach(ctx, a.N, CompactKernel{emit.p, slot.p, insItems.p});
     sortKeys.ensure(ctx, I); sortVals.ensure(ctx, I);
-    foreach(ctx, I, SiblingKeyKernel{w, insItems.p, parentRow.p, objRow.p, ord, ordBits, sortKeys.p, errWord.p});
+    foreach(ctx, I, SiblingKeyKernel{a.w, insItems.p, parentRow.p, objRow.p, a.ord, a.ordBits, sortKeys.p, errWord.p});
     d2d(ctx, sortVals.p, insItems.p, I * 4);
-    sortPairs(sortKeys, sortVals, I, ordBits + parentBits);
+    sortPairs(sortKeys, sortVals, I, a.ordBits + parentBits);
     checkErr();
-    itemIdx.ensure(ctx, N + 1); objSlot.ensure(ctx, N + 2);
+    itemIdx.ensure(ctx, a.N + 1); objSlot.ensure(ctx, a.N + 2);
     foreach(ctx, I, ItemIndexKernel{sortVals.p, itemIdx.p});
-    foreach(ctx, N, ListObjFlagKernel{w, emit.p}); scan_exclusive(ctx, scanTmp, emit.p, objSlot.p, N);
-    const size_t Lo = readU32(objSlot.p + N);
+    foreach(ctx, a.N, ListObjFlagKernel{a.w, emit.p}); scan_exclusive(ctx, scanTmp, emit.p, objSlot.p, a.N);
+    const size_t Lo = readU32(objSlot.p + a.N);
     const size_t S = 2 * I + 2 * Lo; eNext.ensure(ctx, S + 1); eRank.ensure(ctx, S + 1); ePacked.ensure(ctx, S + 1);
     foreach(ctx, S, EulerInitKernel{eNext.p, eRank.p});
-    foreach(ctx, I, EulerLinkKernel{sortKeys.p, ordBits, itemIdx.p, objSlot.p, eNext.p, eRank.p, I});
-    foreach(ctx, S, ListRankPackKernel{eNext.p, eRank.p, ePacked.p});
-    const int rounds = bits_for(S);
-#ifdef AMG_EMU
-    ePacked2.ensure(ctx, S + 1);
-#endif
-    for (int k = 0; k < rounds; k++) {
-#ifdef AMG_EMU
-      foreach(ctx, S, ListRankPackedKernel{ePacked.p, ePacked2.p});
-      ePacked.swap(ePacked2);
-#else
-      foreach(ctx, S, ListRankInPlaceKernel{ePacked.p});
-#endif
-    }
-    foreach(ctx, S, ListRankUnpackKernel{ePacked.p, eRank.p});
-    foreach(ctx, N, ListPosKernel{eRank.p, elemRow.p, objRow.p, itemIdx.p, objSlot.p, (u32)I, listPos.p});
-  } else dev_memset(ctx, listPos.p, 0, (N + 1) * 4);
+    foreach(ctx, I, EulerLinkKernel{sortKeys.p, a.ordBits, itemIdx.p, objSlot.p, eNext.p, eRank.p, I});
+    rankEulerTour(S);
+    foreach(ctx, a.N, ListPosKernel{eRank.p, elemRow.p, objRow.p, itemIdx.p, objSlot.p, (u32)I, listPos.p});
+  } else dev_memset(ctx, listPos.p, 0, (a.N + 1) * 4);
   checkErr();
   trace.mark("opset:list-ranked");
-  // document order: stable LSD over (object, key rank | list position, opId within the key / element)
-  perm.ensure(ctx, N + 1); pos.ensure(ctx, N + 1); sortKeys.ensure(ctx, N);
-  foreach(ctx, N, IotaKernel{perm.p});
-  const int fieldBits[3] = {ordBits + 1, bits_for(N), ordBits + 1};
+}
+
+// rank of every slot of the S-slot Euler tour (eNext, eRank) by pointer jumping over packed (next, rank) words: in place
+// on one array on the device, from one buffer into the other in the emulation build
+inline void Engine::rankEulerTour(size_t S) {
+  foreach(ctx, S, ListRankPackKernel{eNext.p, eRank.p, ePacked.p});
+  const int rounds = bits_for(S);
+#ifdef AMG_EMU
+  ePacked2.ensure(ctx, S + 1);
+  for (int k = 0; k < rounds; k++) { foreach(ctx, S, ListRankPackedKernel{ePacked.p, ePacked2.p}); ePacked.swap(ePacked2); }
+#else
+  for (int k = 0; k < rounds; k++) foreach(ctx, S, ListRankInPlaceKernel{ePacked.p});
+#endif
+  foreach(ctx, S, ListRankUnpackKernel{ePacked.p, eRank.p});
+}
+
+// document order: stable LSD over (object, key rank | list position, opId within the key / element)
+inline void Engine::sortDocOrder(ApplyCall& a) {
+  perm.ensure(ctx, a.N + 1); pos.ensure(ctx, a.N + 1); sortKeys.ensure(ctx, a.N);
+  foreach(ctx, a.N, IotaKernel{perm.p});
+  const int fieldBits[3] = {a.ordBits + 1, bits_for(a.N), a.ordBits + 1};
   for (int f = 0; f < 3; f++) {
-    foreach(ctx, N, DocKeyKernel{f, w, perm.p, listPos.p, keySlots.p, keySlot.p, ord, sortKeys.p});
-    sortPairs(sortKeys, perm, N, fieldBits[f]);
+    foreach(ctx, a.N, DocKeyKernel{f, a.w, perm.p, listPos.p, keySlots.p, keySlot.p, a.ord, sortKeys.p});
+    sortPairs(sortKeys, perm, a.N, fieldBits[f]);
   }
-  foreach(ctx, N, InversePermKernel{perm.p, pos.p});
+  foreach(ctx, a.N, InversePermKernel{perm.p, pos.p});
   trace.mark("opset:doc-ordered(enqueued)");
-  // succ lists of the new document (old pairs re-keyed + the batch's preds), the checks on what the preds refer to, and the
-  // rows gathered into document order
+}
+
+// succ lists of the new document (old pairs re-keyed + the batch's preds), the checks on what the preds refer to, and the
+// rows gathered into document order
+inline void Engine::linkSuccessors(ApplyCall& a) {
   const size_t numPairs = a.numPairs = numSucc + a.P;
   pairKey.ensure(ctx, numPairs + 1); pairSucc.ensure(ctx, numPairs + 1); pairIdx.ensure(ctx, numPairs + 1); pairPos.ensure(ctx, numPairs + 1); pairTime.ensure(ctx, numPairs + 1);
-  foreach(ctx, M, DelElemCheckKernel{a.ops, a.idt, w, errWord.p});
+  foreach(ctx, a.M, DelElemCheckKernel{a.ops, a.idt, a.w, errWord.p});
   checkErr();
-  foreach(ctx, numRows, OldPairsKernel{succOff.p, succ.p, pos.p, ord, pairKey.p, pairIdx.p, pairSucc.p, pairPos.p, pairTime.p});
-  foreach(ctx, M, PredPairsKernel{a.ops, a.idt, pos.p, rowOfOp.p, w, elemRow.p, keySlot.p, ord, pairKey.p, pairIdx.p, pairSucc.p, pairPos.p, pairTime.p, numSucc, errWord.p});
-  foreach(ctx, M, DelKeyCheckKernel{arena.p, a.ops, a.idt, w, errWord.p});
-  foreach(ctx, M, IncCheckKernel{a.ops, a.idt, w, arena.p, errWord.p});
+  foreach(ctx, numRows, OldPairsKernel{succOff.p, succ.p, pos.p, a.ord, pairKey.p, pairIdx.p, pairSucc.p, pairPos.p, pairTime.p});
+  foreach(ctx, a.M, PredPairsKernel{a.ops, a.idt, pos.p, rowOfOp.p, a.w, elemRow.p, keySlot.p, a.ord, pairKey.p, pairIdx.p, pairSucc.p, pairPos.p, pairTime.p, numSucc, errWord.p});
+  foreach(ctx, a.M, DelKeyCheckKernel{arena.p, a.ops, a.idt, a.w, errWord.p});
+  foreach(ctx, a.M, IncCheckKernel{a.ops, a.idt, a.w, arena.p, errWord.p});
   if (const u64 ew = fetchErr()) throwOpError(ew, a.now.actorIds);
-  sortPairs(pairKey, pairIdx, numPairs, ordBits);
+  sortPairs(pairKey, pairIdx, numPairs, a.ordBits);
   foreach(ctx, numPairs, PairPosKeyKernel{pairPos.p, pairIdx.p, pairKey.p});
-  sortPairs(pairKey, pairIdx, numPairs, bits_for(N));
-  succCnt.ensure(ctx, N + 2); newSuccCnt.ensure(ctx, N + 2); newSuccOff.ensure(ctx, N + 2); firstNewSucc.ensure(ctx, N + 2); newSucc.ensure(ctx, numPairs + 1);
-  dev_memset(ctx, succCnt.p, 0, (N + 2) * 4); dev_memset(ctx, newSuccCnt.p, 0, (N + 2) * 4); dev_memset(ctx, firstNewSucc.p, 0xff, (N + 2) * 4);
+  sortPairs(pairKey, pairIdx, numPairs, bits_for(a.N));
+  succCnt.ensure(ctx, a.N + 2); newSuccCnt.ensure(ctx, a.N + 2); newSuccOff.ensure(ctx, a.N + 2); firstNewSucc.ensure(ctx, a.N + 2); newSucc.ensure(ctx, numPairs + 1);
+  dev_memset(ctx, succCnt.p, 0, (a.N + 2) * 4); dev_memset(ctx, newSuccCnt.p, 0, (a.N + 2) * 4); dev_memset(ctx, firstNewSucc.p, 0xff, (a.N + 2) * 4);
   foreach(ctx, numPairs, CountSuccKernel{pairPos.p, succCnt.p});
   foreach(ctx, numPairs, NewSuccFlagKernel{pairPos.p, pairTime.p, newSuccCnt.p});
   foreach(ctx, numPairs, FirstSuccTimeKernel{pairPos.p, pairTime.p, firstNewSucc.p});
-  scan_exclusive(ctx, scanTmp, succCnt.p, newSuccOff.p, N);
+  scan_exclusive(ctx, scanTmp, succCnt.p, newSuccOff.p, a.N);
   newSuccTime.ensure(ctx, numPairs + 1);
   foreach(ctx, numPairs, WriteSuccKernel{pairIdx.p, pairSucc.p, newSucc.p, pairTime.p, newSuccTime.p});
-  sorted.ensure(ctx, N + 1);
-  foreach(ctx, N, GatherRowsKernel{w, sorted.view(), perm.p});
+  sorted.ensure(ctx, a.N + 1);
+  foreach(ctx, a.N, GatherRowsKernel{a.w, sorted.view(), perm.p});
   trace.mark("opset:succ+gather(enqueued)");
 }
 
@@ -780,208 +796,246 @@ inline void Engine::commit(ApplyCall& a) {
   arenaLen = a.cur; queue = a.newQueue; queueOriginal = a.newQueueOriginal;
 }
 
+// The incremental patch of the batch: the op set's tables and the batch as PatchInputs
+inline void Engine::batchPatch(ApplyCall& a, PatchOut& out) {
+  objPos.ensure(ctx, a.N + 1);
+  foreach(ctx, a.N, ObjPosKernel{perm.p, objRow.p, pos.p, objPos.p});
+  buildPatch(PatchInputs{sorted.view(), a.N, false, newSuccOff.p, newSucc.p, succCnt.p, a.ord, &a.ops, a.M, &a.idt, rowOfOp.p, pos.p,
+                         newSuccCnt.p, firstNewSucc.p, newSuccTime.p, objPos.p, pass.p, a.w}, out);
+}
 
 // Patch emission over a document table `in.d` in document order (N rows). wholeDoc = getPatch semantics
 // (new.js:1604-1635), otherwise incremental semantics for the batch `ops` (new.js:884-1040, 1461-1528).
 inline void Engine::buildPatch(const PatchInputs& in, PatchOut& out) {
-  const DocRows d = in.d; const size_t N = in.N, numOps = in.numOps; const bool wholeDoc = in.wholeDoc; const OpRows* ops = in.ops;
-  const u32* succCntD = in.succCnt;
   out.numProps = out.numEdits = 0; out.bigEnd = 0;
-  if (N == 0) return;
-  // groups (map key / list element) and their visibility
-  head.ensure(ctx, N + 1); headScan.ensure(ctx, N + 2); groupOf.ensure(ctx, N + 1);
-  foreach(ctx, N, GroupHeadKernel{arena.p, d, head.p});
-  scan_exclusive(ctx, scanTmp, head.p, headScan.p, N);
-  isObjHead.ensure(ctx, N + 1); objIdx.ensure(ctx, N + 2);
-  foreach(ctx, N, ObjHeadKernel{d, isObjHead.p});
-  scan_exclusive(ctx, scanTmp, isObjHead.p, objIdx.p, N);
-  u32 numGroups32 = 0, numObjs32 = 0; readU32x2(headScan.p + N, objIdx.p + N, &numGroups32, &numObjs32);
-  const size_t numGroups = numGroups32, numObjs = numObjs32;
+  if (in.N == 0) return;
+  PatchCall p{in};
+  patchGroups(p);
+  if (!in.wholeDoc) { batchOpGroups(p); markTouched(p); }
+  mapProps(p);
+  trace.phase("patch:list-index");
+  if (in.wholeDoc) docListEdits(p); else batchListEdits(p);
+  shipPatch(p, out);
+}
+
+// groups (map key / list element) and their visibility, objects in document order
+inline void Engine::patchGroups(PatchCall& p) {
+  head.ensure(ctx, p.N + 1); headScan.ensure(ctx, p.N + 2); groupOf.ensure(ctx, p.N + 1);
+  foreach(ctx, p.N, GroupHeadKernel{arena.p, p.d, head.p});
+  scan_exclusive(ctx, scanTmp, head.p, headScan.p, p.N);
+  isObjHead.ensure(ctx, p.N + 1); objIdx.ensure(ctx, p.N + 2);
+  foreach(ctx, p.N, ObjHeadKernel{p.d, isObjHead.p});
+  scan_exclusive(ctx, scanTmp, isObjHead.p, objIdx.p, p.N);
+  u32 numGroups32 = 0, numObjs32 = 0; readU32x2(headScan.p + p.N, objIdx.p + p.N, &numGroups32, &numObjs32);
+  const size_t numGroups = p.numGroups = numGroups32, numObjs = p.numObjs = numObjs32;
   groupRows.ensure(ctx, numGroups + 1); groupVisible.ensure(ctx, numGroups + 1); groupFirst.ensure(ctx, numGroups + 1); groupTouched.ensure(ctx, numGroups + 1);
   dev_memset(ctx, groupRows.p, 0, (numGroups + 1) * 4); dev_memset(ctx, groupVisible.p, 0, (numGroups + 1) * 4); dev_memset(ctx, groupTouched.p, 0, (numGroups + 1) * 4);
   groupHasChild.ensure(ctx, numGroups + 1); dev_memset(ctx, groupHasChild.p, 0, (numGroups + 1) * 4);
-  foreach(ctx, N, GroupStatsKernel{headScan.p, head.p, succCntD, d, groupOf.p, groupRows.p, groupVisible.p, groupFirst.p, errWord.p, 0, groupHasChild.p});
-  // objects in document order
+  foreach(ctx, p.N, GroupStatsKernel{headScan.p, head.p, p.in.succCnt, p.d, groupOf.p, groupRows.p, groupVisible.p, groupFirst.p, errWord.p, 0, groupHasChild.p});
   objStart.ensure(ctx, numObjs + 2);
-  foreach(ctx, N, ObjStartKernel{isObjHead.p, objIdx.p, objStart.p, N});
-  { const u32 nn = (u32)N; h2d(ctx, objStart.p + numObjs, &nn, 4); }
-  emit.ensure(ctx, N + 1); marker.ensure(ctx, N + 1); slot.ensure(ctx, N + 2);
-  groupLinked.ensure(ctx, std::max(numGroups, numApplied + 1) + 2);
+  foreach(ctx, p.N, ObjStartKernel{isObjHead.p, objIdx.p, objStart.p, p.N});
+  { const u32 nn = (u32)p.N; h2d(ctx, objStart.p + numObjs, &nn, 4); }
+  emit.ensure(ctx, p.N + 1); marker.ensure(ctx, p.N + 1); slot.ensure(ctx, p.N + 2);
+  groupLinked.ensure(ctx, std::max(numGroups, numApplied + 1) + 2);   // computeHeads' isDep too: numApplied + 1
   dev_memset(ctx, groupLinked.p, 0, (numGroups + 1) * 4);
-  ListCtx lctx{d, succCntD, in.newSuccCnt, in.firstNewSucc, groupOf.p, groupFirst.p, groupRows.p, arena.p, in.succOff, in.succ, in.newSuccTime};
-  MapGroupCtx mg{arena.p, ops ? *ops : OpRows{}, opAt.p, numOps, in.pass};
-  bool anyListLink = false;
-  auto listGroups = [&](int pass) {
-    return ListGroupKernel{pass, mg, opGroupHead.p, *in.idt, in.rowOfOp, in.pos, lctx, gCount.p, gElem.p, gT1.p, gQOrd.p, nQ.p, elemHasRecs.p, elemMinT.p,
-                           itemBase.p, objIdx.p, objStart.p, items.p, domTw.p, domW.p, oldVisScan.p, runHeadFlag.p, runScan.p, runStart.p, gBase.p, qIndex.p, editOut.p, editElem.p, editObjKey.p, editElemPos.p, editRowPos.p, errWord.p};
-  };
-  if (!wholeDoc) {
-    // op groups of the batch (new.js:1085-1138), then what each list group nets out to
-    nQ.ensure(ctx, N + 1); elemHasRecs.ensure(ctx, N + 1); listLinkTime.ensure(ctx, N + 1); elemMinT.ensure(ctx, N + 1);
-    dev_memset(ctx, elemMinT.p, 0xff, (N + 1) * 4);
-    dev_memset(ctx, nQ.p, 0, (N + 1) * 4); dev_memset(ctx, elemHasRecs.p, 0, (N + 1) * 4); dev_memset(ctx, listLinkTime.p, 0xff, (N + 1) * 4);
-    if (numOps > 0) {
-      opAt.ensure(ctx, numOps + 1); runHead.ensure(ctx, numOps + 1); opGroupHead.ensure(ctx, numOps + 1);
-      for (DBuf<u32>* b : {&gCount, &gElem, &gT1, &gQOrd, &gBase, &qIndex}) b->ensure(ctx, numOps + 2);
-      mg.opAt = opAt.p;
-      foreach(ctx, numOps, OpAtTimeKernel{ops->time, opAt.p});
-      foreach(ctx, numOps, RunHeadKernel{mg, runHead.p});
-      foreach(ctx, numOps, GroupSplitKernel{mg, runHead.p, opGroupHead.p});
-      foreach(ctx, numOps, listGroups(0));
-      runHeadFlag.ensure(ctx, numOps + 1); runScan.ensure(ctx, numOps + 2); runStart.ensure(ctx, numOps + 2); elemFollower.ensure(ctx, N + 1);
-      dev_memset(ctx, elemFollower.p, 0, (N + 1) * 4);
-      foreach(ctx, numOps, FollowerFlagKernel{mg, opGroupHead.p, lctx, gElem.p, gT1.p, gCount.p, nQ.p, runHeadFlag.p, elemFollower.p});
-      scan_exclusive(ctx, scanTmp, runHeadFlag.p, runScan.p, numOps);
-      foreach(ctx, numOps, RunStartKernel{runHeadFlag.p, runScan.p, runStart.p});
-      foreach(ctx, 1, RunEndKernel{runScan.p, runStart.p, (u32)numOps});
-    }
-    objTouchedAt.ensure(ctx, N + 1); linkDone.ensure(ctx, N + 1);
-    dev_memset(ctx, objTouchedAt.p, 0xff, (N + 1) * 4); dev_memset(ctx, linkDone.p, 0xff, (N + 1) * 4); dev_memset(ctx, flagWord.p, 0, 16);
-    foreach(ctx, N, TouchKernel{d, groupOf.p, in.firstNewSucc, groupTouched.p, objTouchedAt.p, in.objPos, flagWord.p + 2});
-    u32 linkChanged = 1, anyLink32 = 0;
-    // Three sweeps per host round trip, until a sweep changes nothing. A touch climbs at least one level of nesting per
-    // sweep (a parent's make row lies below its child's rows, so a serial sweep climbs exactly one), so a fixed number of
-    // rounds would leave the outer levels of deeply nested objects unlinked. It ends: objTouchedAt only decreases.
-    while (linkChanged) {
-      LinkKernel lk{d, groupOf.p, groupHasChild.p, groupFirst.p, groupTouched.p, in.objPos, groupLinked.p, objTouchedAt.p, flagWord.p + 2, linkDone.p, flagWord.p, listLinkTime.p, flagWord.p + 3};
-      foreach(ctx, N, lk); foreach(ctx, N, lk);
-      dev_memset(ctx, flagWord.p, 0, 4);
-      foreach(ctx, N, lk);
-      readU32x2(flagWord.p, flagWord.p + 3, &linkChanged, &anyLink32);
-    }
-    anyListLink = anyLink32 != 0;
+  p.lctx = ListCtx{p.d, p.in.succCnt, p.in.newSuccCnt, p.in.firstNewSucc, groupOf.p, groupFirst.p, groupRows.p, arena.p, p.in.succOff, p.in.succ, p.in.newSuccTime};
+}
+
+// op groups of the batch (new.js:1085-1138), then what each list group nets out to
+inline void Engine::batchOpGroups(PatchCall& p) {
+  nQ.ensure(ctx, p.N + 1); elemHasRecs.ensure(ctx, p.N + 1); listLinkTime.ensure(ctx, p.N + 1); elemMinT.ensure(ctx, p.N + 1);
+  dev_memset(ctx, elemMinT.p, 0xff, (p.N + 1) * 4);
+  dev_memset(ctx, nQ.p, 0, (p.N + 1) * 4); dev_memset(ctx, elemHasRecs.p, 0, (p.N + 1) * 4); dev_memset(ctx, listLinkTime.p, 0xff, (p.N + 1) * 4);
+  if (p.numOps == 0) return;
+  opAt.ensure(ctx, p.numOps + 1); runHead.ensure(ctx, p.numOps + 1); opGroupHead.ensure(ctx, p.numOps + 1);
+  for (DBuf<u32>* b : {&gCount, &gElem, &gT1, &gQOrd, &gBase, &qIndex}) b->ensure(ctx, p.numOps + 2);
+  const MapGroupCtx mg = p.mg = MapGroupCtx{arena.p, *p.in.ops, opAt.p, p.numOps, p.in.pass};
+  foreach(ctx, p.numOps, OpAtTimeKernel{p.in.ops->time, opAt.p});
+  foreach(ctx, p.numOps, RunHeadKernel{mg, runHead.p});
+  foreach(ctx, p.numOps, GroupSplitKernel{mg, runHead.p, opGroupHead.p});
+  foreach(ctx, p.numOps, listGroups(p, 0));
+  runHeadFlag.ensure(ctx, p.numOps + 1); runScan.ensure(ctx, p.numOps + 2); runStart.ensure(ctx, p.numOps + 2); elemFollower.ensure(ctx, p.N + 1);
+  dev_memset(ctx, elemFollower.p, 0, (p.N + 1) * 4);
+  foreach(ctx, p.numOps, FollowerFlagKernel{mg, opGroupHead.p, p.lctx, gElem.p, gT1.p, gCount.p, nQ.p, runHeadFlag.p, elemFollower.p});
+  scan_exclusive(ctx, scanTmp, runHeadFlag.p, runScan.p, p.numOps);
+  foreach(ctx, p.numOps, RunStartKernel{runHeadFlag.p, runScan.p, runStart.p});
+  foreach(ctx, 1, RunEndKernel{runScan.p, runStart.p, (u32)p.numOps});
+}
+
+// ListGroupKernel pass 0 (group records), 1 (dominance items) or 2 (edits) over the batch's op groups
+inline ListGroupKernel Engine::listGroups(const PatchCall& p, int pass) {
+  return ListGroupKernel{pass, p.mg, opGroupHead.p, *p.in.idt, p.in.rowOfOp, p.in.pos, p.lctx, gCount.p, gElem.p, gT1.p, gQOrd.p, nQ.p, elemHasRecs.p, elemMinT.p,
+                         itemBase.p, objIdx.p, objStart.p, items.p, domTw.p, domW.p, oldVisScan.p, runHeadFlag.p, runScan.p, runStart.p, gBase.p, qIndex.p, editOut.p, editElem.p, editObjKey.p, editElemPos.p, editRowPos.p, errWord.p};
+}
+
+// groups the batch touched, and the groups of their parents up the nesting (setupPatches)
+inline void Engine::markTouched(PatchCall& p) {
+  objTouchedAt.ensure(ctx, p.N + 1); linkDone.ensure(ctx, p.N + 1);
+  dev_memset(ctx, objTouchedAt.p, 0xff, (p.N + 1) * 4); dev_memset(ctx, linkDone.p, 0xff, (p.N + 1) * 4); dev_memset(ctx, flagWord.p, 0, 16);
+  foreach(ctx, p.N, TouchKernel{p.d, groupOf.p, p.in.firstNewSucc, groupTouched.p, objTouchedAt.p, p.in.objPos, flagWord.p + 2});
+  u32 linkChanged = 1, anyLink32 = 0;
+  // Three sweeps per host round trip, until a sweep changes nothing. A touch climbs at least one level of nesting per
+  // sweep (a parent's make row lies below its child's rows, so a serial sweep climbs exactly one), so a fixed number of
+  // rounds would leave the outer levels of deeply nested objects unlinked. It ends: objTouchedAt only decreases.
+  while (linkChanged) {
+    LinkKernel lk{p.d, groupOf.p, groupHasChild.p, groupFirst.p, groupTouched.p, p.in.objPos, groupLinked.p, objTouchedAt.p, flagWord.p + 2, linkDone.p, flagWord.p, listLinkTime.p, flagWord.p + 3};
+    foreach(ctx, p.N, lk); foreach(ctx, p.N, lk);
+    dev_memset(ctx, flagWord.p, 0, 4);
+    foreach(ctx, p.N, lk);
+    readU32x2(flagWord.p, flagWord.p + 3, &linkChanged, &anyLink32);
   }
-  // ---- map props
-  DBuf<u32>& groupEmitted = elemVis;   // scratch reuse (list edits re-initialise it later)
-  groupEmitted.ensure(ctx, std::max(numGroups, N) + 2); dev_memset(ctx, groupEmitted.p, 0, (numGroups + 1) * 4);
-  finalTime.ensure(ctx, numGroups + 1); gBound.ensure(ctx, numGroups + 1); gFailed.ensure(ctx, numGroups + 1); memberFinal.ensure(ctx, N + 1);
-  dev_memset(ctx, finalTime.p, 0, (numGroups + 1) * 4);
-  if (!wholeDoc && numOps > 0) {
-    dev_memset(ctx, memberFinal.p, 0, (N + 1) * 4); dev_memset(ctx, gFailed.p, 0, (numGroups + 1) * 4);
+  p.anyListLink = anyLink32 != 0;
+}
+
+inline void Engine::mapProps(PatchCall& p) {
+  DBuf<u32>& groupEmitted = elemVis;   // scratch reuse (list edits re-initialise it later); sized for their elemVis too
+  groupEmitted.ensure(ctx, std::max(p.numGroups, p.N) + 2); dev_memset(ctx, groupEmitted.p, 0, (p.numGroups + 1) * 4);
+  finalTime.ensure(ctx, p.numGroups + 1); gBound.ensure(ctx, p.numGroups + 1); gFailed.ensure(ctx, p.numGroups + 1); memberFinal.ensure(ctx, p.N + 1);
+  dev_memset(ctx, finalTime.p, 0, (p.numGroups + 1) * 4);
+  if (!p.in.wholeDoc && p.numOps > 0) {
+    dev_memset(ctx, memberFinal.p, 0, (p.N + 1) * 4); dev_memset(ctx, gFailed.p, 0, (p.numGroups + 1) * 4);
     for (int pass = 0; pass < 2; pass++)
-      foreach(ctx, numOps, GroupFinalKernel{pass, mg, opGroupHead.p, *in.idt, in.rowOfOp, in.pos, groupOf.p, in.unsorted, in.ord, finalTime.p, gBound.p, gFailed.p, memberFinal.p});
+      foreach(ctx, p.numOps, GroupFinalKernel{pass, p.mg, opGroupHead.p, *p.in.idt, p.in.rowOfOp, p.in.pos, groupOf.p, p.in.unsorted, p.in.ord, finalTime.p, gBound.p, gFailed.p, memberFinal.p});
   }
-  counterLast.ensure(ctx, N + 1); counterTotal.ensure(ctx, N + 1); counterOwner.ensure(ctx, N + 1); dev_memset(ctx, counterOwner.p, 0xff, (N + 1) * 4);
-  foreach(ctx, N, CounterKernel{arena.p, d, in.succOff, in.succ, groupOf.p, groupFirst.p, groupRows.p, counterLast.p, counterTotal.p, counterOwner.p});
-  foreach(ctx, N, PropFlagKernel{d, groupOf.p, groupTouched.p, groupLinked.p, succCntD, wholeDoc ? 1 : 0, finalTime.p, gBound.p, gFailed.p, memberFinal.p, in.ord, emit.p, groupEmitted.p, counterLast.p});
-  foreach(ctx, N, PropMarkerKernel{d, groupOf.p, groupTouched.p, head.p, groupEmitted.p, wholeDoc ? 1 : 0, emit.p, marker.p});
-  scan_exclusive(ctx, scanTmp, emit.p, slot.p, N);
-  const size_t numProps = readU32(slot.p + N);
+  counterLast.ensure(ctx, p.N + 1); counterTotal.ensure(ctx, p.N + 1); counterOwner.ensure(ctx, p.N + 1); dev_memset(ctx, counterOwner.p, 0xff, (p.N + 1) * 4);
+  foreach(ctx, p.N, CounterKernel{arena.p, p.d, p.in.succOff, p.in.succ, groupOf.p, groupFirst.p, groupRows.p, counterLast.p, counterTotal.p, counterOwner.p});
+  foreach(ctx, p.N, PropFlagKernel{p.d, groupOf.p, groupTouched.p, groupLinked.p, p.in.succCnt, p.in.wholeDoc ? 1 : 0, finalTime.p, gBound.p, gFailed.p, memberFinal.p, p.in.ord, emit.p, groupEmitted.p, counterLast.p});
+  foreach(ctx, p.N, PropMarkerKernel{p.d, groupOf.p, groupTouched.p, head.p, groupEmitted.p, p.in.wholeDoc ? 1 : 0, emit.p, marker.p});
+  scan_exclusive(ctx, scanTmp, emit.p, slot.p, p.N);
+  const size_t numProps = p.numProps = readU32(slot.p + p.N);
   propOut.ensure(ctx, numProps + 1);
-  foreach(ctx, N, PropEmitKernel{d, emit.p, marker.p, slot.p, propOut.p, counterLast.p, counterTotal.p, errWord.p});
-  trace.phase("patch:list-index");
-  // ---- list edits
-  size_t numEdits = 0; bool shipElem = true;
-  if (wholeDoc) {
-    elemVis.ensure(ctx, N + 1); elemVisScan.ensure(ctx, N + 2); rowEmit.ensure(ctx, N + 1); firstVis.ensure(ctx, numGroups + 1);
-    rowClass.ensure(ctx, N + 1); firstBare.ensure(ctx, numGroups + 1);
-    dev_memset(ctx, firstVis.p, 0xff, (numGroups + 1) * 4); dev_memset(ctx, firstBare.p, 0xff, (numGroups + 1) * 4);
-    foreach(ctx, N, ListRowClassKernel{d, groupOf.p, succCntD, counterOwner.p, rowClass.p, firstVis.p, firstBare.p});
-    foreach(ctx, N, ListVisFlagKernel{d, groupOf.p, groupVisible.p, head.p, succCntD, elemVis.p, rowEmit.p, rowClass.p, firstVis.p, firstBare.p});
-    scan_exclusive(ctx, scanTmp, elemVis.p, elemVisScan.p, N);
-    scan_exclusive(ctx, scanTmp, rowEmit.p, slot.p, N);
-    numEdits = readU32(slot.p + N);
-    editOut.ensure(ctx, numEdits + 1); editElem.ensure(ctx, numEdits + 1);
-    foreach(ctx, N, DocEditEmitKernel{d, rowEmit.p, slot.p, elemVisScan.p, objIdx.p, objStart.p, groupOf.p, groupFirst.p, rowClass.p, firstVis.p, firstBare.p, editOut.p, counterOwner.p, counterTotal.p, errWord.p});
-    foreach(ctx, N, EditElemKernel{d, rowEmit.p, slot.p, groupOf.p, groupFirst.p, editElem.p});
-  } else {
-    size_t numGroupRecs = 0, numLink = 0, numLive = 0;
-    if (numOps > 0) { scan_exclusive(ctx, scanTmp, gCount.p, gBase.p, numOps); numGroupRecs = readU32(gBase.p + numOps); }
-    DBuf<u32>& elemHasLive = elemHasRecs; dev_memset(ctx, elemHasLive.p, 0, (N + 1) * 4);
-    auto ensureEdits = [&](size_t n) {
-      editOut.ensure(ctx, n + 1, numLive); editElem.ensure(ctx, n + 1, numLive); editObjKey.ensure(ctx, n + 1, numLive); editElemPos.ensure(ctx, n + 1);
-      editOut2.ensure(ctx, n + 1); editElem2.ensure(ctx, n + 1); editElemPos2.ensure(ctx, n + 1); editObjKey2.ensure(ctx, n + 1); editRowPos.ensure(ctx, n + 1); editRowPos2.ensure(ctx, n + 1);
-      sortKeys.ensure(ctx, n + 1); sortVals.ensure(ctx, n + 1);
-    };
-    // ---- A. records of the op groups: indexes, emission, per-object order, pops / coalescing, compaction
-    if (numGroupRecs > 0) {
-      // list index of a group = elements in front that were visible before the batch (one prefix sum)
-      //                       + net visibility changes in front that earlier groups of the batch made (dominance count)
-      nItems.ensure(ctx, N + 1); itemBase.ensure(ctx, N + 2); oldVisScan.ensure(ctx, N + 2);
-      foreach(ctx, N, OldVisFlagKernel{lctx, head.p, nItems.p});
-      scan_exclusive(ctx, scanTmp, nItems.p, oldVisScan.p, N);
-      foreach(ctx, N, DomItemCountKernel{nQ.p, elemFollower.p, nItems.p});
-      scan_exclusive(ctx, scanTmp, nItems.p, itemBase.p, N);
-      const size_t T = readU32(itemBase.p + N);
-      items.ensure(ctx, T + 1); items2.ensure(ctx, T + 1); zwScan.ensure(ctx, T + 2); domTw.ensure(ctx, T + 1); domTw2.ensure(ctx, T + 1); domW.ensure(ctx, T + 1); domW2.ensure(ctx, T + 1);
-      foreach(ctx, numOps, listGroups(1));
-      const int tbits = bits_for(numOps + 1);
+  foreach(ctx, p.N, PropEmitKernel{p.d, emit.p, marker.p, slot.p, propOut.p, counterLast.p, counterTotal.p, errWord.p});
+}
+
+// list edits of the whole document: every visible element as an insert
+inline void Engine::docListEdits(PatchCall& p) {
+  elemVisScan.ensure(ctx, p.N + 2); rowEmit.ensure(ctx, p.N + 1); firstVis.ensure(ctx, p.numGroups + 1);
+  rowClass.ensure(ctx, p.N + 1); firstBare.ensure(ctx, p.numGroups + 1);
+  dev_memset(ctx, firstVis.p, 0xff, (p.numGroups + 1) * 4); dev_memset(ctx, firstBare.p, 0xff, (p.numGroups + 1) * 4);
+  foreach(ctx, p.N, ListRowClassKernel{p.d, groupOf.p, p.in.succCnt, counterOwner.p, rowClass.p, firstVis.p, firstBare.p});
+  foreach(ctx, p.N, ListVisFlagKernel{p.d, groupOf.p, groupVisible.p, head.p, p.in.succCnt, elemVis.p, rowEmit.p, rowClass.p, firstVis.p, firstBare.p});
+  scan_exclusive(ctx, scanTmp, elemVis.p, elemVisScan.p, p.N);
+  scan_exclusive(ctx, scanTmp, rowEmit.p, slot.p, p.N);
+  const size_t numEdits = p.numEdits = readU32(slot.p + p.N);
+  editOut.ensure(ctx, numEdits + 1); editElem.ensure(ctx, numEdits + 1);
+  foreach(ctx, p.N, DocEditEmitKernel{p.d, rowEmit.p, slot.p, elemVisScan.p, objIdx.p, objStart.p, groupOf.p, groupFirst.p, rowClass.p, firstVis.p, firstBare.p, editOut.p, counterOwner.p, counterTotal.p, errWord.p});
+  foreach(ctx, p.N, EditElemKernel{p.d, rowEmit.p, slot.p, groupOf.p, groupFirst.p, editElem.p});
+}
+
+// list edits of the batch: A. the records of its op groups, B. the link edits on list parents
+inline void Engine::batchListEdits(PatchCall& p) {
+  if (p.numOps > 0) { scan_exclusive(ctx, scanTmp, gCount.p, gBase.p, p.numOps); p.numGroupRecs = readU32(gBase.p + p.numOps); }
+  DBuf<u32>& elemHasLive = elemHasRecs;   // ListGroupKernel pass 0 is done with it
+  dev_memset(ctx, elemHasLive.p, 0, (p.N + 1) * 4);
+  if (p.numGroupRecs > 0) listIndex(p);
+  trace.phase("patch:edits+copy-out");
+  if (p.numGroupRecs > 0) groupEdits(p, elemHasLive.p);
+  if (p.anyListLink) linkEdits(p, elemHasLive.p);
+  p.numEdits = p.numLive + p.numLink;
+}
+
+// list index of a group = elements in front that were visible before the batch (one prefix sum)
+//                       + net visibility changes in front that earlier groups of the batch made (dominance count)
+inline void Engine::listIndex(PatchCall& p) {
+  nItems.ensure(ctx, p.N + 1); itemBase.ensure(ctx, p.N + 2); oldVisScan.ensure(ctx, p.N + 2);
+  foreach(ctx, p.N, OldVisFlagKernel{p.lctx, head.p, nItems.p});
+  scan_exclusive(ctx, scanTmp, nItems.p, oldVisScan.p, p.N);
+  foreach(ctx, p.N, DomItemCountKernel{nQ.p, elemFollower.p, nItems.p});
+  scan_exclusive(ctx, scanTmp, nItems.p, itemBase.p, p.N);
+  const size_t T = readU32(itemBase.p + p.N);
+  items.ensure(ctx, T + 1); items2.ensure(ctx, T + 1); domTw.ensure(ctx, T + 1); domTw2.ensure(ctx, T + 1); domW.ensure(ctx, T + 1);
+  foreach(ctx, p.numOps, listGroups(p, 1));
+  dominanceCount(T, bits_for(p.numOps + 1));
+}
+
+// qIndex of every query item from the T dominance items over tbits time bits. The emulation build runs every level as a
+// global pass; the device runs the global levels DOM_PASS_BITS time bits per pass and the last DOM_LOCAL_BITS levels
+// inside shared memory (k_dom_local), one CTA per partition.
+inline void Engine::dominanceCount(size_t T, int tbits) {
 #ifdef AMG_EMU
-      const int localBits = 0;
-#else
-      const int localBits = std::min(tbits, DOM_LOCAL_BITS);   // the last levels run inside shared memory (k_dom_local)
-#endif
-#ifdef AMG_EMU
-      for (int bit = tbits - 1; bit >= localBits; bit--) {
-        scan_exclusive64(ctx, scanTmp, DomScanInput{domTw.p, domW.p, bit}, zwScan.p, T);
-        foreach(ctx, T, DomLevelKernel{items.p, items2.p, domTw2.p, domW2.p, zwScan.p, bit});
-        items.swap(items2); domTw.swap(domTw2); domW.swap(domW2);
-      }
-      foreach(ctx, T, DomResultKernel{items.p, qIndex.p});
-#else
-      dom_global_passes(ctx, domPass, items, items2, T, tbits, localBits);   // the global levels, DOM_PASS_BITS time bits per pass
-      {   // partition heads -> compact list (device-side count), then one CTA per partition
-        DBuf<u32>& partFlag = domTw2; DBuf<u32>& partScan = nItems; DBuf<u32>& partHead = itemBase;   // scratch that is free by now
-        partScan.ensure(ctx, T + 2); partHead.ensure(ctx, T + 2);
-        foreach(ctx, T, DomPartHeadKernel{items.p, partFlag.p});
-        scan_exclusive(ctx, scanTmp, partFlag.p, partScan.p, T);
-        foreach(ctx, T, CompactKernel{partFlag.p, partScan.p, partHead.p});
-        if (!domLocalReady) { CUDA_CHECK(cudaFuncSetAttribute(k_dom_local, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DomLocalSmem))); domLocalReady = true; }
-        k_dom_local<<<ctx.numSMs * 2, 256, sizeof(DomLocalSmem), ctx.stream>>>(items.p, partHead.p, partScan.p + T, qIndex.p, localBits, errWord.p);
-        CUDA_CHECK(cudaGetLastError()); ctx.launches++;
-      }
-#endif
-      trace.phase("patch:edits+copy-out");
-      ensureEdits(numGroupRecs);
-      foreach(ctx, numOps, listGroups(2));
-      // the records are in application order by construction: one stable sort by object gives the per-object edit lists
-      foreach(ctx, numGroupRecs, EditKeyKernel{editObjKey.p, editOut.p, sortKeys.p, sortVals.p});
-      sortPairs(sortKeys, sortVals, numGroupRecs, bits_for(numObjs));
-      foreach(ctx, numGroupRecs, EditGatherKernel{editOut.p, editElem.p, editElemPos.p, editObjKey.p, sortVals.p, editOut2.p, editElem2.p, editElemPos2.p, editObjKey2.p});
-      foreach(ctx, numGroupRecs, GatherU32Kernel{editRowPos.p, sortVals.p, editRowPos2.p});
-      for (DBuf<u32>* b : {&editKind, &editPred, &editDead, &editMerge, &editMulti, &editLive}) b->ensure(ctx, numGroupRecs + 2);
-      dev_memset(ctx, editDead.p, 0, (numGroupRecs + 1) * 4); dev_memset(ctx, editMulti.p, 0, (numGroupRecs + 1) * 4);
-      foreach(ctx, numGroupRecs, EditFixKernel{editOut2.p, editElemPos2.p, editKind.p, editPred.p, editDead.p, numGroupRecs});
-      foreach(ctx, numGroupRecs, EditMergeKernel{editOut2.p, editElem2.p, editKind.p, editPred.p, editMerge.p, editMulti.p});
-      dev_memset(ctx, flagWord.p, 0, 4);
-      foreach(ctx, numGroupRecs, EditLiveKernel{editDead.p, editLive.p, editOut2.p, editElem2.p, editKind.p, flagWord.p, editElemPos2.p, elemHasLive.p, editRowPos2.p, succCntD, counterLast.p});
-      DBuf<u32>& liveSlot = editPred;   // pred is consumed by now
-      scan_exclusive(ctx, scanTmp, editLive.p, liveSlot.p, numGroupRecs);
-      u32 numLive32 = 0, needElem32 = 0; readU32x2(liveSlot.p + numGroupRecs, flagWord.p, &numLive32, &needElem32);
-      numLive = numLive32; shipElem = needElem32 != 0;
-      foreach(ctx, numGroupRecs, EditCompactKernel{editOut2.p, editElem2.p, editDead.p, liveSlot.p, editKind.p, editMerge.p, editMulti.p, editOut.p, editElem.p, editObjKey2.p, editObjKey.p});
-    } else trace.phase("patch:edits+copy-out");
-    // ---- B. setupPatches link edits on list parents: only for elements that did not keep an edit of their own; appended
-    //         behind the object's other edits in the order the child objects were first touched
-    if (anyListLink) {
-      DBuf<u32>& linkCount = rowEmit; DBuf<u32>& linkBase = slot;
-      elemVis.ensure(ctx, N + 1); elemVisScan.ensure(ctx, N + 2); linkCount.ensure(ctx, N + 1); linkBase.ensure(ctx, N + 2);
-      foreach(ctx, N, ListVisFlagKernel{d, groupOf.p, groupVisible.p, head.p, succCntD, elemVis.p, linkCount.p, nullptr, nullptr, nullptr});
-      scan_exclusive(ctx, scanTmp, elemVis.p, elemVisScan.p, N);   // index of a linked element = visible elements before it once the whole batch is applied
-      foreach(ctx, N, ListLinkKernel{0, lctx, listLinkTime.p, elemVisScan.p, objIdx.p, objStart.p, linkCount.p, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, elemHasLive.p});
-      scan_exclusive(ctx, scanTmp, linkCount.p, linkBase.p, N);
-      numLink = readU32(linkBase.p + N);
-      if (numLink > 0) {
-        const size_t total = numLive + numLink;
-        ensureEdits(total); editTime.ensure(ctx, total + 1);
-        foreach(ctx, N, ListLinkKernel{1, lctx, listLinkTime.p, elemVisScan.p, objIdx.p, objStart.p, linkCount.p, linkBase.p, (u32)numLive, editOut.p, editElem.p, editObjKey.p, editElemPos.p, editTime.p, elemHasLive.p});
-        // order: surviving group records as they are, then the link edits by first-touch time; then stably by object
-        foreach(ctx, numLive, OffsetIotaKernel{sortVals.p, 0});
-        if (numLink > 1) {
-          DBuf<u64>& k2 = pairKey; DBuf<u32>& v2 = pairIdx; k2.ensure(ctx, numLink + 1); v2.ensure(ctx, numLink + 1);
-          foreach(ctx, numLink, EditTimeKeyAtKernel{editTime.p, (u32)numLive, k2.p, v2.p});
-          sortPairs(k2, v2, numLink, 32);
-          d2d(ctx, sortVals.p + numLive, v2.p, numLink * 4);
-        } else foreach(ctx, numLink, OffsetIotaKernel{sortVals.p + numLive, (u32)numLive});
-        foreach(ctx, total, GatherToU64Kernel{editObjKey.p, sortVals.p, sortKeys.p});
-        sortPairs(sortKeys, sortVals, total, bits_for(numObjs));
-        foreach(ctx, total, EditGatherKernel{editOut.p, editElem.p, nullptr, nullptr, sortVals.p, editOut2.p, editElem2.p, nullptr, nullptr});
-        editOut.swap(editOut2); editElem.swap(editElem2);
-      }
-    }
-    numEdits = numLive + numLink;
+  zwScan.ensure(ctx, T + 2); domW2.ensure(ctx, T + 1);
+  for (int bit = tbits - 1; bit >= 0; bit--) {
+    scan_exclusive64(ctx, scanTmp, DomScanInput{domTw.p, domW.p, bit}, zwScan.p, T);
+    foreach(ctx, T, DomLevelKernel{items.p, items2.p, domTw2.p, domW2.p, zwScan.p, bit});
+    items.swap(items2); domTw.swap(domTw2); domW.swap(domW2);
   }
-  if (wholeDoc && numEdits > 0) foreach(ctx, numEdits, RunFlagKernel{editOut.p, editElem.p, numEdits});
+  foreach(ctx, T, DomResultKernel{items.p, qIndex.p});
+#else
+  const int localBits = std::min(tbits, DOM_LOCAL_BITS);
+  dom_global_passes(ctx, domPass, items, items2, T, tbits, localBits);
+  // partition heads -> compact list (device-side count), then one CTA per partition
+  DBuf<u32>& partFlag = domTw2; DBuf<u32>& partScan = nItems; DBuf<u32>& partHead = itemBase;   // scratch that is free by now
+  partScan.ensure(ctx, T + 2); partHead.ensure(ctx, T + 2);
+  foreach(ctx, T, DomPartHeadKernel{items.p, partFlag.p});
+  scan_exclusive(ctx, scanTmp, partFlag.p, partScan.p, T);
+  foreach(ctx, T, CompactKernel{partFlag.p, partScan.p, partHead.p});
+  if (!domLocalReady) { CUDA_CHECK(cudaFuncSetAttribute(k_dom_local, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DomLocalSmem))); domLocalReady = true; }
+  k_dom_local<<<ctx.numSMs * 2, 256, sizeof(DomLocalSmem), ctx.stream>>>(items.p, partHead.p, partScan.p + T, qIndex.p, localBits, errWord.p);
+  CUDA_CHECK(cudaGetLastError()); ctx.launches++;
+#endif
+}
+
+// edit buffers for n records; the first numLive records of editOut / editElem / editObjKey are kept
+inline void Engine::ensureEdits(const PatchCall& p, size_t n) {
+  editOut.ensure(ctx, n + 1, p.numLive); editElem.ensure(ctx, n + 1, p.numLive); editObjKey.ensure(ctx, n + 1, p.numLive); editElemPos.ensure(ctx, n + 1);
+  editOut2.ensure(ctx, n + 1); editElem2.ensure(ctx, n + 1); editElemPos2.ensure(ctx, n + 1); editObjKey2.ensure(ctx, n + 1); editRowPos.ensure(ctx, n + 1); editRowPos2.ensure(ctx, n + 1);
+  sortKeys.ensure(ctx, n + 1); sortVals.ensure(ctx, n + 1);
+}
+
+// records of the op groups: emission, per-object order, pops / coalescing, compaction
+inline void Engine::groupEdits(PatchCall& p, u32* elemHasLive) {
+  ensureEdits(p, p.numGroupRecs);
+  foreach(ctx, p.numOps, listGroups(p, 2));
+  // the records are in application order by construction: one stable sort by object gives the per-object edit lists
+  foreach(ctx, p.numGroupRecs, EditKeyKernel{editObjKey.p, editOut.p, sortKeys.p, sortVals.p});
+  sortPairs(sortKeys, sortVals, p.numGroupRecs, bits_for(p.numObjs));
+  foreach(ctx, p.numGroupRecs, EditGatherKernel{editOut.p, editElem.p, editElemPos.p, editObjKey.p, sortVals.p, editOut2.p, editElem2.p, editElemPos2.p, editObjKey2.p});
+  foreach(ctx, p.numGroupRecs, GatherU32Kernel{editRowPos.p, sortVals.p, editRowPos2.p});
+  for (DBuf<u32>* b : {&editKind, &editPred, &editDead, &editMerge, &editMulti, &editLive}) b->ensure(ctx, p.numGroupRecs + 2);
+  dev_memset(ctx, editDead.p, 0, (p.numGroupRecs + 1) * 4); dev_memset(ctx, editMulti.p, 0, (p.numGroupRecs + 1) * 4);
+  foreach(ctx, p.numGroupRecs, EditFixKernel{editOut2.p, editElemPos2.p, editKind.p, editPred.p, editDead.p, p.numGroupRecs});
+  foreach(ctx, p.numGroupRecs, EditMergeKernel{editOut2.p, editElem2.p, editKind.p, editPred.p, editMerge.p, editMulti.p});
+  dev_memset(ctx, flagWord.p, 0, 4);
+  foreach(ctx, p.numGroupRecs, EditLiveKernel{editDead.p, editLive.p, editOut2.p, editElem2.p, editKind.p, flagWord.p, editElemPos2.p, elemHasLive, editRowPos2.p, p.in.succCnt, counterLast.p});
+  DBuf<u32>& liveSlot = editPred;   // pred is consumed by now
+  scan_exclusive(ctx, scanTmp, editLive.p, liveSlot.p, p.numGroupRecs);
+  u32 numLive32 = 0, needElem32 = 0; readU32x2(liveSlot.p + p.numGroupRecs, flagWord.p, &numLive32, &needElem32);
+  p.numLive = numLive32; p.shipElem = needElem32 != 0;
+  foreach(ctx, p.numGroupRecs, EditCompactKernel{editOut2.p, editElem2.p, editDead.p, liveSlot.p, editKind.p, editMerge.p, editMulti.p, editOut.p, editElem.p, editObjKey2.p, editObjKey.p});
+}
+
+// setupPatches link edits on list parents: only for elements that did not keep an edit of their own; appended behind the
+// object's other edits in the order the child objects were first touched
+inline void Engine::linkEdits(PatchCall& p, const u32* elemHasLive) {
+  DBuf<u32>& linkCount = rowEmit; DBuf<u32>& linkBase = slot;
+  elemVisScan.ensure(ctx, p.N + 2); linkCount.ensure(ctx, p.N + 1); linkBase.ensure(ctx, p.N + 2);
+  foreach(ctx, p.N, ListVisFlagKernel{p.d, groupOf.p, groupVisible.p, head.p, p.in.succCnt, elemVis.p, linkCount.p, nullptr, nullptr, nullptr});
+  scan_exclusive(ctx, scanTmp, elemVis.p, elemVisScan.p, p.N);   // index of a linked element = visible elements before it once the whole batch is applied
+  foreach(ctx, p.N, ListLinkKernel{0, p.lctx, listLinkTime.p, elemVisScan.p, objIdx.p, objStart.p, linkCount.p, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, elemHasLive});
+  scan_exclusive(ctx, scanTmp, linkCount.p, linkBase.p, p.N);
+  const size_t numLink = p.numLink = readU32(linkBase.p + p.N);
+  if (numLink == 0) return;
+  const size_t total = p.numLive + numLink;
+  ensureEdits(p, total); editTime.ensure(ctx, total + 1);
+  foreach(ctx, p.N, ListLinkKernel{1, p.lctx, listLinkTime.p, elemVisScan.p, objIdx.p, objStart.p, linkCount.p, linkBase.p, (u32)p.numLive, editOut.p, editElem.p, editObjKey.p, editElemPos.p, editTime.p, elemHasLive});
+  // order: surviving group records as they are, then the link edits by first-touch time; then stably by object
+  foreach(ctx, p.numLive, OffsetIotaKernel{sortVals.p, 0});
+  if (numLink > 1) {
+    DBuf<u64>& k2 = pairKey; DBuf<u32>& v2 = pairIdx; k2.ensure(ctx, numLink + 1); v2.ensure(ctx, numLink + 1);
+    foreach(ctx, numLink, EditTimeKeyAtKernel{editTime.p, (u32)p.numLive, k2.p, v2.p});
+    sortPairs(k2, v2, numLink, 32);
+    d2d(ctx, sortVals.p + p.numLive, v2.p, numLink * 4);
+  } else foreach(ctx, numLink, OffsetIotaKernel{sortVals.p + p.numLive, (u32)p.numLive});
+  foreach(ctx, total, GatherToU64Kernel{editObjKey.p, sortVals.p, sortKeys.p});
+  sortPairs(sortKeys, sortVals, total, bits_for(p.numObjs));
+  foreach(ctx, total, EditGatherKernel{editOut.p, editElem.p, nullptr, nullptr, sortVals.p, editOut2.p, editElem2.p, nullptr, nullptr});
+  editOut.swap(editOut2); editElem.swap(editElem2);
+}
+
+// the record sections' offsets, the records' key and value bytes, and the copy-out into patchBuf
+inline void Engine::shipPatch(PatchCall& p, PatchOut& out) {
+  const size_t numProps = p.numProps, numEdits = p.numEdits; const bool shipElem = p.shipElem;
+  if (p.in.wholeDoc && numEdits > 0) foreach(ctx, numEdits, RunFlagKernel{editOut.p, editElem.p, numEdits});
   out.numProps = numProps; out.numEdits = numEdits;
   out.propsOff = PATCH_HDR_WORDS * 8; out.editsOff = out.propsOff + numProps * sizeof(PropRec);
   size_t end;
